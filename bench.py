@@ -12,7 +12,7 @@ ring of input frames larger than L2, so no launch finds its source in cache.
             tables and D2H of the result inside the timed region, for the same FRAMES_PER_STEP-frame steps.  e2e.value keeps three
             frames in flight (gf_cuda_undistort_image_async on three contexts), e2e.sync_call_value is the strictly sequential
             gf_cuda_undistort_image
-  roofline  algorithmic bytes per launch (SURVEY.md §8d: in + out + rows*56 + 368) / mean launch time, vs measured HBM peak
+  roofline  algorithmic bytes per launch (SURVEY.md §8d: in + out + rows*56 + 368) / mean launch time, vs the HBM peak
   cpu_baseline  the CPU oracle (C port of the reference CPU path) on this box's host cores, bounded sample
 
 `--impl reference` times the reference CPU path instead (oracle port; the Rust original cannot be built: no rustc).
@@ -34,8 +34,8 @@ sys.path.insert(0, ROOT)
 
 import numpy as np
 
-# BASELINE.json configs.  cfg2 is the one `metric` is quoted on (default); cfg1/3/4 are selectable with --config for the
-# per-lens-model ncu captures (profiles/) — they are parity-test cases, not additional headline numbers.
+# BASELINE.json configs.  cfg2 is the one `metric` is quoted on (default); cfg1/3/4 are selectable with --config as side
+# measurements — they are parity-test cases, not additional headline numbers.
 CONFIGS = {
     1: dict(w=3840, h=2160, pix="RGBA8", lens="opencv_fisheye", digital=None, rs=False, identity=True,
             name="cfg1: 3840x2160 RGBA8, opencv_fisheye, rolling-shutter OFF, identity quaternion, bilinear"),
@@ -49,15 +49,11 @@ CONFIGS = {
             name="cfg4: 3840x2160 f32 plane (GBRAPF32), sony lens + IBIS rows + 9x9 mesh correction, rolling-shutter ON, bilinear"),
 }
 CFG = CONFIGS[2]
-# dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel, one launch, from the committed `ncu --set full` captures
-# (ncu flushes the caches before the launch and the output stays in L2 after it, hence traffic < algorithmic bytes)
-NCU_TRAFFIC = {(2, "Bilinear"): 23568896 + 1131264}
-NCU_TRAFFIC_SOURCE = "profiles/r02h_x2_filtered_fisheye_rgba8_summary.txt"
 INTERP = "Bilinear"          # BASELINE configs are bilinear; --interp measures the other resamplers (side measurement, not the headline)
 W, H = CFG["w"], CFG["h"]
 PIX, LENS = CFG["pix"], CFG["lens"]
 FRAMES_PER_STEP = 128
-RING = 8                 # 8 x 33.2 MB input frames = 265 MB > 126 MB L2
+RING = 8                 # 8 x 33.2 MB input frames = 265 MB > 50 MB L2 (H100)
 N_TIMESTAMPS = 32        # distinct matrix tables
 METRIC = "4K frames/sec (fisheye+RS warp)"
 WORKLOAD = CFG["name"]
@@ -77,8 +73,33 @@ def algorithmic_bytes(p, rows, mesh_len=0, planes=1):
     return planes * 2 * pw * ph * p.bytes_per_pixel + rows * 56 + 368 + 4 * mesh_len
 
 
+DUMP_BYTES = 48 << 20       # --dump-outputs stays under 64 MB in all
+
+
+def dump_outputs(directory, outs, frames, p, torch):
+    """--dump-outputs: what the timed path handed back in its last step, i.e. the output frames still resident in the ring when it
+    ended (`outs`, device uint8 (rows, output_stride) tensors, global frame indices `frames`).  A fixed, seeded sample of each frame's
+    pixels, all channels, as float32: frames.npy (n_frames, n_pixels, channels); frame_index.npy and pixel_index.npy (float64) say which."""
+    os.makedirs(directory, exist_ok=True)
+    w, h = CFG.get("plane", (W, H))
+    bpp, ch = p.bytes_per_pixel, p.pix_element_count
+    esize = bpp // ch
+    dt = {1: torch.uint8, 2: torch.float16 if PIX.endswith("f16") else torch.int16, 4: torch.float32}[esize]
+    n = min(w * h, DUMP_BYTES // (len(outs) * ch * 4 + 8))        # float32 samples + their float64 pixel index
+    pix = np.sort(np.random.default_rng(20240611).choice(w * h, size=n, replace=False))
+    idx = torch.from_numpy(pix).to(outs[0].device)
+    sample = []
+    for o in outs:
+        px = o[:h, :w * bpp].contiguous().view(dt).reshape(w * h, ch)[idx].float()
+        if dt == torch.int16: px = torch.where(px < 0, px + 65536.0, px)     # u16 read through the signed view
+        sample.append(px.cpu().numpy())
+    np.save(os.path.join(directory, "frames.npy"), np.stack(sample).astype(np.float32))
+    np.save(os.path.join(directory, "frame_index.npy"), np.asarray(frames, np.float64))
+    np.save(os.path.join(directory, "pixel_index.npy"), pix.astype(np.float64))
+
+
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
@@ -286,6 +307,9 @@ def run_pipeline(args, torch, dist, g, rank, world, local, dev):
     torch.cuda.synchronize()
     clocks.mark_end()
     if world > 1: dist.barrier()
+    if args.dump_outputs and rank == 0:                   # the last timed step's frames still in the ring, before anything else renders
+        last = [(W_STEPS + args.steps - 1) * FRAMES_PER_STEP + j for j in range(FRAMES_PER_STEP)][-RING:]
+        dump_outputs(args.dump_outputs, [frames_out[i % RING] for i in last], [i * world + rank for i in last], p, torch)
     total_ms = e0.elapsed_time(e1)
     launches = q.launch_count - l0
     if clocks.proc and clocks.samples_inside() < 3:
@@ -417,7 +441,7 @@ def run_pipeline(args, torch, dist, g, rank, world, local, dev):
         peaks = {}
         try: peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception: pass
-        peak = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         abytes = algorithmic_bytes(p, rows)
         achieved = abytes / (launch_ms / 1e3) / 1e9
         cpu = None
@@ -457,16 +481,14 @@ def run_pipeline(args, torch, dist, g, rank, world, local, dev):
             "value_notes": "value = the per-frame pipeline above (producer + warp kernels, multi-stream, CUDA events around the whole region); value_trusted_precomputed = warp kernel only on "
                            "%d recycled device tables with verdict words (round 1's headline shape); value_unvalidated = the same without verdict words (guarded code path)" % n_tab,
             "e2e": e2e,
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_TRAFFIC.get((args.config, INTERP)),
-                         "traffic_source": NCU_TRAFFIC_SOURCE if (args.config, INTERP) in NCU_TRAFFIC else None,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "algorithmic_bytes_per_launch": abytes, "launch_ms": launch_ms, "peak_source": peak_src,
-                         # SURVEY §8(d): the read-only variant (input planes + tables; north_star says "HBM-read roofline") and the nominal 8 TB/s
+                         # SURVEY §8(d): the read-only variant (input planes + tables; north_star says "HBM-read roofline")
                          "read_only": {"bytes_per_launch": abytes - int(W * p.bytes_per_pixel * H), "achieved": (abytes - int(W * p.bytes_per_pixel * H)) / (launch_ms / 1e3) / 1e9,
                                        "frac": (abytes - int(W * p.bytes_per_pixel * H)) / (launch_ms / 1e3) / 1e9 / peak},
-                         "frac_of_nominal_8000": achieved / 8000.0,
                          "pipeline_achieved": abytes * fps_value / world / 1e9, "pipeline_frac": abytes * fps_value / world / 1e9 / peak,
                          "kernel": "warp_kernel_x2 (trusted path, filtered pre-pass: main + tail launch), timed alone on one stream with CUDA events: %d frames per step" % FRAMES_PER_STEP,
-                         "note": "kernel is FP32-issue bound in bit-exact (-fmad=false) mode, not HBM bound; traffic is the DRAM bytes of ONE cold launch under ncu (output stays in L2), not a steady-state figure; see DESIGN.md"},
+                         "note": "kernel is FP32-issue bound in bit-exact (-fmad=false) mode, not HBM bound; see DESIGN.md"},
             "cpu_baseline": cpu,
         }
         print(json.dumps(out))
@@ -491,7 +513,10 @@ def main():
     ap.add_argument("--digital", default=None, help="override the config's digital lens (side measurement), e.g. gopro_superview, digital_stretch, gopro_warp")
     ap.add_argument("--planes", type=int, default=1, help="planes of this geometry per frame, rendered by one gf_cuda_undistort_planes_dev call (side measurement)")
     ap.add_argument("--interp", default="Bilinear", help="Bilinear (BASELINE), Bicubic, Lanczos4, 'EWA: Robidoux', ... (side measurement)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write a seeded sample of the frames the last timed step rendered to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1: ap.error("--steps must be at least 1")
     select_config(args.config)
     global INTERP, LENS, WORKLOAD
     INTERP = args.interp
@@ -593,6 +618,10 @@ def main():
     torch.cuda.synchronize()
     clocks.mark_end()
     if world > 1: dist.barrier()
+    if args.dump_outputs and rank == 0:
+        last = [(args.steps - 1) * FRAMES_PER_STEP + j for j in range(FRAMES_PER_STEP)][-RING:]
+        dump_outputs(args.dump_outputs, [frames_out[(i % RING) * NPL + k] for i in last for k in range(NPL)],
+                     [i * world + rank for i in last for k in range(NPL)], p, torch)
     total_ms = sum(a.elapsed_time(b) for a, b in ev)
     launches = ctx.launch_count - l0
     if clocks.proc and clocks.samples_inside() < 3:   # a very short timed region: keep the same load running (untimed) until the sampler has seen it
@@ -650,7 +679,7 @@ def main():
         peaks = {}
         try: peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception: pass
-        peak = float(peaks.get("hbm_gbs", 6650.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0)); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         abytes = algorithmic_bytes(p, rows, mesh_np.size if mesh_np is not None else 0, NPL)
         launch_ms = total_ms / max(args.steps * FRAMES_PER_STEP, 1)      # per frame: one launch for the headline config; coordinate + sampling passes otherwise
         achieved = abytes / (launch_ms / 1e3) / 1e9
@@ -673,8 +702,7 @@ def main():
                     "h2d_bytes_per_frame": h2d_frame, "d2h_bytes_per_frame": d2h_frame, "frames_per_step": FRAMES_PER_STEP * world, "steps": e2e_steps,
                     "sync_call_value": sync_fps * world,
                     "note": "pinned host frame + tables H2D, kernel, D2H per frame; value = %d-deep pipeline over gf_cuda_undistort_image_async, sync_call_value = strictly sequential gf_cuda_undistort_image; %d frames, wall clock" % (DEPTH, e2e_frames)},
-            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": NCU_TRAFFIC.get((args.config, INTERP)),
-                         "traffic_source": NCU_TRAFFIC_SOURCE if (args.config, INTERP) in NCU_TRAFFIC else None,
+            "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "algorithmic_bytes_per_launch": abytes, "launch_ms": launch_ms, "peak_source": peak_src,
                          "note": "kernel is FP32-issue bound in bit-exact (-fmad=false) mode; see DESIGN.md"},
             "cpu_baseline": cpu,

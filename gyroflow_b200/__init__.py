@@ -1,4 +1,4 @@
-"""gyroflow_b200 — B200 (sm_100a) backend for Gyroflow's per-pixel stabilization warp.
+"""gyroflow_b200 — H100 (sm_90a) backend for Gyroflow's per-pixel stabilization warp.
 
 Product code = gyroflow_b200/csrc (CUDA kernels + extern "C" ABI, built into libgyroflow_cuda.so).
 This package is the thin host-side mirror used by tests and bench.py.

@@ -1,6 +1,6 @@
 """ctypes mirror of include/gyroflow_cuda.h and loader of the product library.
 
-The library is the hand-written sm_100a backend (gyroflow_b200/libgyroflow_cuda.so, built in-tree by
+The library is the hand-written sm_90a backend (gyroflow_b200/libgyroflow_cuda.so, built in-tree by
 `make -C gyroflow_b200/csrc` / `__graft_entry__.build()`).  Loading fails loudly when it is missing:
 there is no Python, PyTorch or CPU fallback for the warp.
 """

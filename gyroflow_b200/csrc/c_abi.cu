@@ -45,7 +45,7 @@ struct gf_cuda_ctx {
     int width = 0, height = 0, output_width = 0, output_height = 0;    // Stabilization.size / output_size
     KernelFn fn = nullptr;        // general instantiation (run-time feature tests)
     KernelFn fn_lean = nullptr;   // rare features compiled out
-    KernelFn fn_x2 = nullptr;     // lean + two pixels per thread on the packed f32x2 pipe; trusted / guarded path picked from a device word
+    KernelFn fn_x2 = nullptr;     // lean + two pixels per thread (f32x2.cuh pair arithmetic); trusted / guarded path picked from a device word
     KernelFn fn_x2c = nullptr;    // the packed kernel writing a coordinate map (pass 1 of the two-pass path)
     uint32_t* d_const_flags = nullptr;   // two device words {0, 1}: the verdict of the host scan of host tables, as the kernel wants it
     uint32_t* d_vflags = nullptr;        // scratch verdict word of gf_cuda_validate_tables_dev
@@ -54,6 +54,7 @@ struct gf_cuda_ctx {
     uint32_t* d_defer_q = nullptr; unsigned* d_defer_count = nullptr; uint32_t defer_cap = 0; unsigned long long filter_frames = 0;
     bool no_filter = false;
     int block_y = GF_BLOCK_Y, x2_block_y = 4;   // tuning knobs GF_BLOCK_Y / GF_X2_BLOCK_Y, read once per context at creation
+    int sm_count = 1;                            // the device's multiprocessors (sizes the filtered pre-pass's tail launch)
     // preview overlays (overlay.cu), off unless gf_cuda_set_overlays: device copy of the drawing buffer, private copy of a DEVICE input
     int overlays = 0;
     uint8_t* h_drawing = nullptr; uint8_t* d_drawing = nullptr; size_t drawing_cap = 0;
@@ -363,7 +364,7 @@ GF_API int gf_cuda_supports(const gf_buffer_desc* in, const gf_buffer_desc* out)
     return (i && o) ? 1 : 0;
 }
 
-GF_API const char* gf_cuda_version(void) { return "gyroflow-b200 0.1 (sm_100a)"; }
+GF_API const char* gf_cuda_version(void) { return "gyroflow-b200 0.1 (sm_90a)"; }
 GF_API size_t gf_abi_struct_size(int which) {
     switch (which) {
     case 0: return sizeof(gf_kernel_params);  case 1: return sizeof(gf_buffer_desc);    case 2: return sizeof(gf_compute_params);
@@ -413,6 +414,8 @@ GF_API int gf_cuda_create(gf_cuda_ctx** out_ctx, int device, const gf_kernel_par
 
     cudaError_t e = cudaSetDevice(device);
     if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaSetDevice"); return bail(GF_ERR_CUDA); }
+    e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
+    if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaDeviceGetAttribute(multiprocessor count)"); return bail(GF_ERR_CUDA); }
     e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaStreamCreate"); return bail(GF_ERR_CUDA); }
     // matrices: 14 * max(W, H) f32 (rows = height, or width for horizontal rolling shutter) — opencl.rs:268, wgpu.rs:260
@@ -660,7 +663,7 @@ static int run_warp(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_
     // touches memory, so the dependency itself is unchanged and only the kernel-to-kernel launch gap disappears.
     auto launch_pdl = [&](KernelFn fn, dim3 g, dim3 b, const WarpArgs& args) -> cudaError_t {
         cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = 0; cfg.stream = st;      // 0 bytes: f32x2.cuh's opaque zero depends on it
+        cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = 0; cfg.stream = st;
         cudaLaunchAttribute attr[1];
         attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
@@ -692,7 +695,7 @@ static int run_warp(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_
             A.flt.tail = 1;                                            // the deferred pairs, exact pre-pass; also re-arms the other counter
             // one thread per deferred pair for up to 2 % of a 4K frame's pairs in a single wave of tiny blocks (idle blocks exit at once);
             // more entries than threads are covered by the grid-stride loop
-            CK(launch_pdl(x2, dim3(148 * 16, 1), block2, A));
+            CK(launch_pdl(x2, dim3(ctx->sm_count * 16, 1), block2, A));
             ctx->launches++;
         } else {
             CK(launch_pdl(x2, grid2, block2, A)); ctx->x2_launches++;

@@ -135,7 +135,7 @@ GF_API int gf_cuda_checksum_dev(const void* ptr_dev, size_t len, uint64_t* out_d
     cudaStream_t st = (cudaStream_t)cu_stream;
     if (cudaMemsetAsync(out_dev, 0, sizeof(uint64_t), st) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     const size_t n = len / 4;
-    if (n) checksum_kernel<<<148 * 4, 256, 0, st>>>(reinterpret_cast<const uint32_t*>(ptr_dev), n, reinterpret_cast<unsigned long long*>(out_dev));
+    if (n) checksum_kernel<<<132 * 4, 256, 0, st>>>(reinterpret_cast<const uint32_t*>(ptr_dev), n, reinterpret_cast<unsigned long long*>(out_dev));
     if (cudaGetLastError() != cudaSuccess) return GF_ERR_CUDA;
     return GF_OK;
 }

@@ -204,7 +204,7 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
     }
     cudaMemcpy(d_cfg, cfgs.data(), cfgs.size() * sizeof(FilterCfg), cudaMemcpyHostToDevice);
     cudaMemset(d_out, 0, 4 * sizeof(unsigned long long));
-    filter_check_kernel<<<dim3(148, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg, n_cfg, step, 0x1p-17f, d_out);
+    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg, n_cfg, step, 0x1p-17f, d_out);
     e = cudaDeviceSynchronize();
     if (e == cudaSuccess) e = cudaMemcpy(out4, d_out, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
     cudaFree(d_cfg); cudaFree(d_out);
@@ -219,8 +219,8 @@ extern "C" GF_API int gf_cuda_selftest_exhaustive(int device, unsigned long long
     unsigned long long* d = nullptr;
     if (cudaMalloc(&d, 2 * sizeof(unsigned long long)) != cudaSuccess) return GF_ERR_CUDA;
     cudaMemset(d, 0, 2 * sizeof(unsigned long long));
-    sweep_kernel<<<148 * 16, 256>>>(__float_as_uint_host(0x1p-28f), __float_as_uint_host(0x1p24f), 0, d);
-    sweep_kernel<<<148 * 16, 256>>>(__float_as_uint_host(0x1p-56f), __float_as_uint_host(0x1p48f), 1, d + 1);
+    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-28f), __float_as_uint_host(0x1p24f), 0, d);
+    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-56f), __float_as_uint_host(0x1p48f), 1, d + 1);
     cudaError_t e = cudaDeviceSynchronize();
     if (e == cudaSuccess) e = cudaMemcpy(out2, d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
     cudaFree(d);
@@ -236,7 +236,7 @@ extern "C" GF_API int gf_cuda_selftest(int device, unsigned long long n, unsigne
     cudaMemset(d, 0, 4 * sizeof(unsigned long long));
     uint32_t* dbg = nullptr;
     if (getenv("GF_SELFTEST_DEBUG")) { cudaMalloc(&dbg, 65 * 4); cudaMemset(dbg, 0, 65 * 4); }
-    selftest_kernel<<<148 * 8, 256>>>(n, seed, d, dbg);
+    selftest_kernel<<<132 * 8, 256>>>(n, seed, d, dbg);
     cudaError_t e = cudaDeviceSynchronize();
     if (e == cudaSuccess) e = cudaMemcpy(out4, d, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
     if (dbg) {

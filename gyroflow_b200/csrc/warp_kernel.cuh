@@ -666,7 +666,7 @@ static __device__ __noinline__ void sample_generic(int sx0, int sy0, const WarpA
 #define GF_HI_UNROLL 2               // rows of the 16 / 64-tap loop per iteration (full unrolling stalled on instruction fetch)
 #endif
 #ifndef GF_SHADE_MINB
-#define GF_SHADE_MINB 5              // 48 registers: measured best of {none (57-64 regs), 4, 5} x unroll {1, 2}, profiles/README.md
+#define GF_SHADE_MINB 5              // 48 registers (unbounded, the kernel takes 57-64)
 #endif
 #ifdef GF_SHADE_MINB
 #define GF_SHADE_BOUNDS __launch_bounds__(GF_BLOCK_X * GF_BLOCK_Y, GF_SHADE_MINB)
@@ -747,8 +747,8 @@ GF_DEV void sample_interior(int sx0, int sy0, const WarpArgs& A, float (&sum)[PI
     } else {
         // 16 / 64 taps.  Same operations in the same order (xsum += px * cx[xp] along a row, sum += xsum * cy[yp] down the rows);
         // the schedule differs: rows are a rolled loop (the fully unrolled 64-tap body stalled on instruction fetch) with cy[yp]
-        // read from the table, and with an even channel count the multiply/add stream runs on register pairs (FFMA2), halving
-        // its issue slots.  Integer taps are widened by PRMT into m = 2^23 + raw (exact), and the product is taken as
+        // read from the table, and with an even channel count the multiply/add stream is written on register pairs (f32x2.cuh).
+        // Integer taps are widened by PRMT into m = 2^23 + raw (exact), and the product is taken as
         // fma(m, cx, -2^23*cx): -2^23*cx is exact (a power-of-two scale), so the FMA rounds the exact real raw*cx once —
         // the same value as float(raw) * cx — and the separate subtraction of 2^23 disappears.  (A zero tap yields +0 where
         // the plain product yields sign(cx)*0; the running sum starts at +0 and x + (+-0) == x, so sums are identical; and since
@@ -860,7 +860,7 @@ template <int C> GF_DEV void remap_colorrange(float (&px)[C], bool is_y) {      
 // Bicubic (I = 4) and Lanczos4 (I = 8) — cpu_undistort.rs:370-418 with offset 1 / 3 (:372-376).  Only the coordinate-map shading
 // kernel reaches these (one instantiation per pixel format), through a uniform run-time branch on the resampler, and they are
 // inlined into it: as an out-of-line function the sampler saw the kernel parameters through a generic pointer (LD.E + R2UR per
-// access instead of constant-bank operands), which cost 12-18 % of the two-pass frame rate (profiles/README.md, r02n).
+// access instead of constant-bank operands).
 template <int I, class PIX>
 GF_DEV void sample_input_at_hi(float uvx, float uvy, const WarpArgs& A, float (&sum)[PIX::COUNT]) {
     const float offset = I == 4 ? 1.0f : 3.0f;

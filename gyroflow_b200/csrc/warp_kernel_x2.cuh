@@ -1,15 +1,15 @@
-// warp_kernel_x2.cuh — the warp with two output pixels per thread on Blackwell's packed f32x2 pipe.
+// warp_kernel_x2.cuh — the warp with two output pixels per thread (pair arithmetic of f32x2.cuh).
 //
 // Same arithmetic, same rounding, same results as warp_kernel.cuh (the scalar kernel remains the general
 // implementation and the exact fallback).  What changes is the schedule:
 //   * a thread owns the vertically adjacent pixels (x, y) and (x, y + 1); every FP32 multiply/add of the
-//     undistort -> rotate -> redistort chain is issued once for both (FFMA2, see f32x2.cuh);
+//     undistort -> rotate -> redistort chain is written once for both (f32x2.cuh);
 //   * the hot path is BRANCH-FREE: divisions, square roots and atanf run their exact fast sequences unconditionally
 //     while a handful of integer tests accumulate one `bad` predicate (an operand outside the magnitude window in which
 //     those sequences are the correctly rounded result, a scanline with IBIS data, ...).  Only if `bad` is set — in
 //     practice never — the pair is re-evaluated with the scalar kernel's code (cold, out of line).  No convergence
 //     barriers, no slow-path stubs inside the arithmetic, so the scheduler can overlap the two lens evaluations' loads,
-//     MUFU ops and FFMA2 chains;
+//     MUFU ops and FP32 chains;
 //   * `TRUSTED` tables: the producer of the table (host scan, gf_cuda_scan_tables_dev, or the on-device FrameTransform producer)
 //     has established that every matrix entry is zero or of moderate magnitude and that no row carries IBIS data, and left that
 //     verdict in a device word the kernel reads at entry; it removes the per-pixel numerator / IBIS tests.
@@ -523,9 +523,8 @@ GF_DEV int round_away_i32(float t) {
 // what the reference gives) or treat every negative / huge result as "not interior" and recompute exactly out of line.
 template <bool BOUNDED = false>     // BOUNDED: the caller guarantees |a2| < 2^23 (no NaN), the max() is not needed
 GF_DEV void round_half_away_w(f2 a2, int& wa, int& wb) {
-    float sa, sb;
-    asm("{ .reg .b64 t, m, r; mov.b64 t, {%2, %3}; mov.b64 m, {%4, %4}; add.rz.f32x2 r, t, m; mov.b64 {%0, %1}, r; }"
-        : "=f"(sa), "=f"(sb) : "f"(BOUNDED ? a2.x : fmaxf(a2.x, -4.0f)), "f"(BOUNDED ? a2.y : fmaxf(a2.y, -4.0f)), "f"(8388608.0f));
+    const float sa = __fadd_rz(BOUNDED ? a2.x : fmaxf(a2.x, -4.0f), 8388608.0f);
+    const float sb = __fadd_rz(BOUNDED ? a2.y : fmaxf(a2.y, -4.0f), 8388608.0f);
     wa = __float_as_int(sa) - 0x4affffff; wb = __float_as_int(sb) - 0x4affffff;
 }
 // max(min(round(t) as i32, lim), 0) for both lanes, 0 <= lim < 2^22

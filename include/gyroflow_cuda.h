@@ -1,4 +1,4 @@
-/* gyroflow_cuda.h — C ABI of the B200 (sm_100a) backend for Gyroflow's per-pixel warp.
+/* gyroflow_cuda.h — C ABI of the H100 (sm_90a) backend for Gyroflow's per-pixel warp.
  *
  * This header is the drop-in boundary.  Every entry point replaces one method of the
  * reference's backend-wrapper convention (there is no C ABI in the reference; the
@@ -199,7 +199,7 @@ typedef struct gf_cuda_ctx gf_cuda_ctx;   /* opaque; one per host thread / strea
 
 /* ---- capability probe: OclWrapper::list_devices opencl.rs:60, wgpu.rs:77,99,113 ---------- */
 GF_API int         gf_cuda_device_count(void);
-GF_API int         gf_cuda_device_name(int device, char* buf, size_t buf_len);   /* "[CUDA] NVIDIA B200" style name */
+GF_API int         gf_cuda_device_name(int device, char* buf, size_t buf_len);   /* "[CUDA] NVIDIA H100 80GB HBM3" style name */
 GF_API int         gf_cuda_supports(const gf_buffer_desc* in, const gf_buffer_desc* out); /* is_buffer_supported opencl.rs:451 */
 GF_API const char* gf_cuda_version(void);
 /* sizeof() of the structs that cross this ABI, for binding generators and their tests: 0 gf_kernel_params, 1 gf_buffer_desc,

@@ -1,6 +1,6 @@
 """GPU parity: the CUDA path (through the C ABI) against the CPU oracle, bit-exact.
 
-Every test here needs a real B200 (`-m gpu`).  A missing GPU or a missing libgyroflow_cuda.so is a FAILURE,
+Every test here needs a real H100 (`-m gpu`).  A missing GPU or a missing libgyroflow_cuda.so is a FAILURE,
 never a skip: there is no fallback path to test instead.
 """
 import os

@@ -4,7 +4,7 @@
 //   C) four tex2Dgather<uchar4> (one per channel: the four taps of that channel in one fetch)
 // over a 3840x2160 RGBA8 frame with a warp-like coordinate field (smooth, ~1 degree of roll + barrel curvature, 1/32-pixel steps).
 // Hardware bilinear filtering is not an option: its 8-bit weights and internal rounding are not the reference's arithmetic.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo tools/bench_tex_gather.cu -o /tmp/bench_tex_gather ; run on the GPU.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo tools/bench_tex_gather.cu -o /tmp/bench_tex_gather ; run on the GPU.
 // Static instruction counts: cuobjdump -sass /tmp/bench_tex_gather | grep -c ... (recorded in DESIGN.md §4).
 #include <cuda_runtime.h>
 #include <cstdio>

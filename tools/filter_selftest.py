@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Run gf_cuda_selftest_filter (the certificate of the filtered rolling-shutter pre-pass, on the real MUFU units) for several seeds and
-print what it measured.  GPU box only; output kept as profiles/r02_filter_selftest.txt."""
+print what it measured.  Needs a GPU."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import gyroflow_b200 as g
