@@ -5,6 +5,24 @@
 #include <cstdint>
 #include "../../include/gyroflow_cuda.h"
 
+namespace gf {
+
+// Trust verdict of a matrix table (rows of GF_MATRIX_STRIDE floats), as the packed warp kernel wants it: 0 = trusted, TBL_WILD = an
+// entry of columns 0-8 is not tame (below), TBL_IBIS = an entry of columns 9-13 (IBIS / OIS shifts) is non-zero.
+enum : uint32_t { TBL_WILD = 1u, TBL_IBIS = 2u };
+// "tame": zero, or 2^-40 <= |v| <= 2^40 — the magnitudes for which the packed kernel's unguarded numerators are safe
+__host__ __device__ __forceinline__ bool tame(float v) { const float a = fabsf(v); return v == 0.0f || (a >= 0x1p-40f && a <= 0x1p40f); }
+__host__ __device__ __forceinline__ uint32_t table_entry_verdict(unsigned col, float v) {
+    return col < 9u ? (tame(v) ? 0u : TBL_WILD) : (v == 0.0f ? 0u : TBL_IBIS);
+}
+__host__ __device__ __forceinline__ uint32_t table_row_verdict(const float* r) {
+    uint32_t f = 0;
+    for (unsigned i = 0; i < GF_MATRIX_STRIDE; ++i) f |= table_entry_verdict(i, r[i]);
+    return f;
+}
+
+} // namespace gf
+
 // One frame through the warp with a DEVICE matrix table + verdict word, never synchronising: HOST image buffers (page-locked) are
 // copied on `cu_stream` before / after the kernel.  `checksum_dev` (nullable): the output buffer's checksum is accumulated into it
 // on the same stream, between the kernel and the device-to-host copy.  Used by the render queue.

@@ -16,6 +16,7 @@
 #include <string>
 #include <vector>
 #include "../../include/gyroflow_cuda.h"
+#include "c_abi_internal.h"
 #include "quat_track.cuh"
 
 #define GF_FT_HD __host__ __device__ __forceinline__
@@ -94,14 +95,6 @@ GF_FT_HD void frame_row(const RowCtx& C, size_t y, float* out14) {
     out14[9] = (float)sx; out14[10] = (float)sy; out14[11] = (float)ra; out14[12] = (float)ox; out14[13] = (float)oy;
 }
 
-// the trust verdict of one row, as the packed warp kernel wants it (c_abi.cu: TBL_WILD = 1, TBL_IBIS = 2)
-GF_FT_HD unsigned row_verdict(const float* r) {
-    unsigned f = 0;
-    for (int i = 0; i < 9; ++i) { const float v = r[i], a = fabsf(v); if (!(v == 0.0f || (a >= 0x1p-40f && a <= 0x1p40f))) f |= 1u; }
-    for (int i = 9; i < 14; ++i) if (!(r[i] == 0.0f)) f |= 2u;
-    return f;
-}
-
 // One thread per scanline.  The table's trust verdict (see warp_kernel_x2) is produced with it: every block ORs its rows into an
 // accumulator, the last block to finish publishes the word and re-arms the accumulator and the ticket for the next launch, so no
 // memset is needed and the verdict is ordered with the table on the producer's stream.
@@ -112,7 +105,7 @@ __global__ void frame_rows_kernel(const __grid_constant__ RowCtx C, size_t rows,
     if (y < rows) {
         float row[14];
         frame_row(C, y, row);
-        f = row_verdict(row);
+        f = table_row_verdict(row);
         float2* o = reinterpret_cast<float2*>(out + y * GF_MATRIX_STRIDE);
         #pragma unroll
         for (int t = 0; t < 7; ++t) o[t] = make_float2(row[2 * t], row[2 * t + 1]);
@@ -335,7 +328,7 @@ GF_API int gf_frame_transform_at_timestamp(const gf_compute_params* cp, double t
 // Host-side form of the table verdict (what gf_cuda_frame_transform_dev leaves in table_flags_dev): 0 = tame and IBIS-free.
 GF_API uint32_t gf_table_flags_host(const float* matrices, size_t rows) {
     uint32_t f = 0;
-    if (matrices) for (size_t r = 0; r < rows; ++r) f |= row_verdict(matrices + r * GF_MATRIX_STRIDE);
+    if (matrices) for (size_t r = 0; r < rows; ++r) f |= table_row_verdict(matrices + r * GF_MATRIX_STRIDE);
     return f;
 }
 

@@ -1001,7 +1001,6 @@ template <class PIX, bool GEN, bool HI>
 GF_DEV void finish_pixel(bool have_uv, float u, float v, float4 jac, const WarpArgs& A, uint8_t* __restrict__ out) {
     const gf_kernel_params& P = A.p;
     constexpr int C = PIX::COUNT;
-    constexpr int I = 2;
     const uint32_t feat = A.feat;
     const bool dvec = has<GEN>(feat, F_DST_VEC);
     float pixel[C];
@@ -1023,8 +1022,8 @@ GF_DEV void finish_pixel(bool have_uv, float u, float v, float4 jac, const WarpA
             u   = map_apply(u,   A.smap_x); v   = map_apply(v,   A.smap_y);
             p2x = map_apply(p2x, A.smap_x); p2y = map_apply(p2y, A.smap_y);
             float c1[C], c2[C];
-            sample_input_at<I, PIX, GEN, HI>(u, v, A, c1, jac);
-            sample_input_at<I, PIX, GEN, HI>(p2x, p2y, A, c2, jac);          // (the reference notes jac should be adjusted for pt2; it is not)
+            sample_input_at<2, PIX, GEN, HI>(u, v, A, c1, jac);
+            sample_input_at<2, PIX, GEN, HI>(p2x, p2y, A, c2, jac);          // (the reference notes jac should be adjusted for pt2; it is not)
             #pragma unroll
             for (int ch = 0; ch < C; ++ch) pixel[ch] = c1[ch] * alpha + c2[ch] * (1.0f - alpha);
         } else {
@@ -1041,9 +1040,9 @@ GF_DEV void finish_pixel(bool have_uv, float u, float v, float4 jac, const WarpA
                     PIX::store_scalars(out, dvec, s);
                     return;
                 }
-                sample_generic<I, PIX>(sx0, sy0, A, pixel);
+                sample_generic<2, PIX>(sx0, sy0, A, pixel);
             } else {
-                sample_input_at<I, PIX, GEN, HI>(u, v, A, pixel, jac);                                           // :615
+                sample_input_at<2, PIX, GEN, HI>(u, v, A, pixel, jac);                                           // :615
             }
         }
     }
@@ -1051,7 +1050,7 @@ GF_DEV void finish_pixel(bool have_uv, float u, float v, float4 jac, const WarpA
     PIX::store(out, dvec, pixel);                                                                                // :611 / :622
 }
 
-template <int LENS, int DIGITAL, class PIX, int I, bool GEN>
+template <int LENS, int DIGITAL, class PIX, bool GEN>
 __global__ void __launch_bounds__(GF_BLOCK_X * GF_BLOCK_Y)
 warp_kernel(const __grid_constant__ WarpArgs A) {
     const gf_kernel_params& P = A.p;

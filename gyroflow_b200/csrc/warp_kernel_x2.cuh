@@ -728,7 +728,7 @@ warp_kernel_x2(const __grid_constant__ WarpArgs A) {
         return;
     }
     const int x = blockIdx.x * GF_BLOCK_X + threadIdx.x;
-    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * 2;          // blockDim.y: the host may launch flatter blocks (GF_X2_BLOCK_Y)
+    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * 2;          // blockDim.y: the host launches flatter blocks than the bounds allow (32 x 4)
     if (trusted) warp_x2_body<LENS, DIGITAL, PIX, true, COORD>(A, x, y0, !(kFilter && (A.feat & F_FILTER)));
     else         warp_x2_body<LENS, DIGITAL, PIX, false, COORD>(A, x, y0, true);
 }

@@ -86,3 +86,52 @@ def test_overlays_match_oracle(case, scale):
         n = int((got != want).sum())
         assert n == 0, (n, device_buffers)
         w.close()
+
+
+@pytest.mark.gpu
+def test_host_planes_around_an_overlay_frame():
+    """One HOST context renders the planes of a frame, then (overlays on) a frame whose drawing buffer makes the context allocate its
+    drawing copies, then the planes again: growing the drawing buffers leaves the planes' staging buffers alone."""
+    case = dict(w=320, h=180, pix="Luma16")
+    built = [cases.build(dict(case, frame=i)) for i in range(2)]
+    p0, src0, m, mesh, dst0, pix, lens, digital = built[0]
+    mesh_data = mesh if mesh is not None else np.zeros(0, np.float32)
+    params, wants = [], []
+    for i, (p, src, _, _, d0, _, _, _) in enumerate(built):
+        p = p.copy(); p.plane_index = i
+        want = d0.copy()
+        assert oracle_lib.undistort_image(src, want, p, pix, lens, digital, m, mesh) == 0
+        params.append(p); wants.append(want)
+
+    def buffers(p, src, dst):
+        return g.Buffers(g.BufferDescription((case["w"], case["h"], p.stride), src), g.BufferDescription((case["w"], case["h"], p.output_stride), dst))
+
+    def planes():
+        gots = [b[4].copy() for b in built]
+        w.undistort_planes([buffers(p, b[1], got) for p, b, got in zip(params, built, gots)], params,
+                           g.FrameTransform(matrices=m, kernel_params=params[0], mesh_data=mesh_data))
+        for i, (got, want) in enumerate(zip(gots, wants)):
+            assert np.array_equal(got, want), i
+
+    # the overlay frame and its restatement: input-stage entries, the CPU warp, output-stage entries + safe area
+    po = p0.copy()
+    po.flags |= abi.FLAG_DRAWING_ENABLED; po.canvas_scale = 1.0
+    po.safe_area_rect[:] = [case["w"] * 0.12, case["h"] * 0.1, case["w"] * 0.88, case["h"] * 0.9]
+    d = _drawing(po, 1.0, 5)
+    src2 = src0.copy()
+    oracle_lib.draw_overlays(src2, case["w"], case["h"], po.stride, po, pix, True, d)
+    want = dst0.copy()
+    assert oracle_lib.undistort_image(src2, want, po, pix, lens, digital, m, mesh) == 0
+    oracle_lib.draw_overlays(want, case["w"], case["h"], po.output_stride, po, pix, False, d)
+
+    w = g.CudaWrapper.new(params[0], pix, lens, digital, buffers(params[0], src0, dst0.copy()))
+    try:
+        planes()
+        w.set_overlays(True)
+        got = dst0.copy()
+        w.undistort_image(buffers(po, src0, got), g.FrameTransform(matrices=m, kernel_params=po, mesh_data=mesh_data), drawing_buffer=d)
+        w.synchronize()
+        assert np.array_equal(got, want)
+        planes()
+    finally:
+        w.close()
