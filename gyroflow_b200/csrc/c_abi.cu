@@ -58,7 +58,9 @@ constexpr LayoutInfo kLayouts[LAY_COUNT] = {
 
 // What the uniforms and the kernel choice of a frame depend on besides the frame: lens, digital lens, layout, and the compiled kernels
 // by variant.  GF_DISABLE_X2 (no packed kernel) and GF_DISABLE_FILTER (no filtered pre-pass) take a fast path out of service for A/B
-// comparisons; they are read whenever a combo is made: once per context, and on every gf_cuda_plan / gf_combo_supported query.
+// comparisons; GF_DISABLE_LEAN (no lean and no packed kernel) makes every frame run the general kernel, so that its instantiations can
+// be checked on plain frames.  They are read whenever a combo is made: once per context, and on every gf_cuda_plan /
+// gf_combo_supported query.
 struct Combo {
     int lens = 0, digital = 0, layout = 0;
     KernelFn kernels[KV_COUNT] = {};     // nullptr where not compiled (or switched off)
@@ -132,9 +134,11 @@ KernelFn find_kernel(const Combo& c, int interp, KernelVariant v) {
 
 bool make_combo(int pixel_type, int lens, int digital, int interp, Combo* c) {
     c->layout = pix_layout(pixel_type); c->lens = lens; c->digital = digital;
-    const bool no_packed = getenv("GF_DISABLE_X2") != nullptr;
+    const bool no_lean = getenv("GF_DISABLE_LEAN") != nullptr;
+    const bool no_packed = no_lean || getenv("GF_DISABLE_X2") != nullptr;
     c->no_filter = getenv("GF_DISABLE_FILTER") != nullptr;
-    for (int v = 0; v < KV_COUNT; ++v) c->kernels[v] = (no_packed && v >= KV_PACKED) ? nullptr : find_kernel(*c, interp, (KernelVariant)v);
+    for (int v = 0; v < KV_COUNT; ++v)
+        c->kernels[v] = ((no_packed && v >= KV_PACKED) || (no_lean && v == KV_LEAN)) ? nullptr : find_kernel(*c, interp, (KernelVariant)v);
     return c->layout >= 0;                                 // false: unknown pixel type
 }
 
@@ -379,8 +383,9 @@ Plan plan_frame(const Combo& c, const WarpArgs& A, uint32_t table_flags, const F
     const int interp = A.p.interpolation;
     pl.two_pass = s.more_planes > 0 || s.coord_only || interp != GF_INTERP_BILINEAR;
     pl.n_maps = (interp > 8 && !s.coord_only) ? 3 : 1;
-    // lean instantiation iff no general-only feature is on, vector access is legal, and the digital-lens flag matches the template
-    const bool lean_ok = (A.feat & F_GENERAL_ONLY) == 0 && (A.feat & F_LEAN_REQUIRED) == F_LEAN_REQUIRED &&
+    // lean instantiation iff it is in service (GF_DISABLE_LEAN), no general-only feature is on, vector access is legal, and the
+    // digital-lens flag matches the template
+    const bool lean_ok = c.kernels[KV_LEAN] && (A.feat & F_GENERAL_ONLY) == 0 && (A.feat & F_LEAN_REQUIRED) == F_LEAN_REQUIRED &&
                          (((A.feat & F_DIGITAL) != 0) == (c.digital != GF_LENS_NONE));
     // packed kernel: magnitudes its fast paths assume (F_WILD clear); two-pass: the coordinate-writing variant, except for EWA whose
     // probe positions only the scalar kernels evaluate

@@ -144,7 +144,12 @@ template <int COUNT_, int SCALAR_> struct Pix {
     }
     static GF_DEV uint32_t float_to_scalar(float v) {        // PixelType::from_float: Rust `as` casts
         if (SCALAR == SC_F32) return __float_as_uint(v);
-        if (SCALAR == SC_F16) return (uint32_t)__half_as_ushort(__float2half_rn(v));
+        if (SCALAR == SC_F16) {
+            // half::f16::from_f32 keeps a NaN's sign and the top of its payload, with the quiet bit set; cvt.rn.f16.f32 does not
+            const uint32_t b = __float_as_uint(v);
+            if (v != v) return ((b >> 16) & 0x8000u) | 0x7e00u | ((b & 0x7fffffu) >> 13);
+            return (uint32_t)__half_as_ushort(__float2half_rn(v));
+        }
         int i = __float2int_rz(v);                           // trunc, saturating, NaN -> 0
         const int hi = SCALAR == SC_U8 ? 255 : 65535;
         i = i < 0 ? 0 : (i > hi ? hi : i);
@@ -1047,6 +1052,13 @@ GF_DEV void finish_pixel(bool have_uv, float u, float v, float4 jac, const WarpA
         }
     }
     if (has<GEN>(feat, F_FIXRANGE)) remap_colorrange<C>(pixel, (feat & F_IS_Y) != 0);                                     // :608-610 / :619-621
+    if ((PIX::SCALAR == SC_F32 || PIX::SCALAR == SC_F16) && have_uv && has<GEN>(feat, F_BG3)) {
+        // The samples are NaN-free (min against the limit), but the feather blend makes a NaN from -inf * 0 where a -inf sample meets
+        // alpha 1 or 0.  x86, which the reference runs on, produces its default NaN 0xffc00000 there and the range fix keeps it; the
+        // GPU's arithmetic produces 0x7fffffff.  Store what the CPU path stores.
+        #pragma unroll
+        for (int ch = 0; ch < C; ++ch) if (pixel[ch] != pixel[ch]) pixel[ch] = __uint_as_float(0xffc00000u);
+    }
     PIX::store(out, dvec, pixel);                                                                                // :611 / :622
 }
 

@@ -44,6 +44,56 @@ def synthetic_frame(width, height, pixel_type="RGBA8", frame=0, stride=None, see
     return buf
 
 
+# bit patterns of the special values edge_frame mixes in: NaNs with assorted signs and payloads (quiet and signalling), +-Inf
+_NAN_F32 = [0x7FC00000, 0xFFC00000, 0x7F800001, 0x7FA5A5A5, 0xFFFFFFFF, 0x7FFFFFFF]
+_NAN_F16 = [0x7E00, 0xFE00, 0x7C01, 0x7D55, 0xFFFF, 0x7FFF]
+
+
+def edge_frame(width, height, pixel_type, seed=0, stride=None):
+    """A frame at the edges of the format's value domain, as a (height, stride) uint8 array like synthetic_frame.
+
+    f32 / f16: ordinary values in [0, 1) mixed with HDR values (1 .. 1e4), values near f16's largest finite 65504 (f16 only),
+    negatives, subnormals, +-0, +-Inf and NaNs with assorted payloads.  The non-finite values sit in every fourth 8 x 8 tile only,
+    so that most footprints of the 16- and 64-tap resamplers still see finite content.
+    u8 / u16: 0 / max checkerboards (pixel parity, flipped per 8 x 8 tile and per channel), which make the bicubic and Lanczos
+    taps overshoot hardest."""
+    _, count, sdt = abi.PIXEL_TYPES[pixel_type]
+    dt = np.dtype(sdt)
+    bpp = count * dt.itemsize
+    if stride is None:
+        stride = (width * bpp + 255) // 256 * 256
+    rng = np.random.Generator(np.random.PCG64(seed))
+    y, x, c = np.meshgrid(np.arange(height), np.arange(width), np.arange(count), indexing="ij")
+    tile = rng.integers(0, 2, size=(height // 8 + 1, width // 8 + 1))[y // 8, x // 8]
+    if dt.kind == "u":
+        vals = np.where(((x + y + c + tile) & 1) == 1, np.iinfo(dt).max, 0).astype(dt)
+    else:
+        f16 = dt == np.dtype("f2")
+        shape = x.shape
+        v = rng.random(shape, dtype=np.float32)                                                  # ordinary
+        kind = rng.integers(0, 100, size=shape)
+        hdr = np.float32(10.0) ** rng.uniform(0.0, 4.0, shape).astype(np.float32)              # 1 .. 1e4
+        v = np.where(kind < 12, hdr, v)
+        v = np.where((kind >= 12) & (kind < 24), -v * np.float32(10.0) ** rng.integers(-2, 3, shape).astype(np.float32), v)   # negatives
+        tiny = (np.float32(2.0) ** -20 if f16 else np.float32(1e-40)) * rng.integers(1, 16, shape).astype(np.float32)          # subnormals
+        v = np.where((kind >= 24) & (kind < 30), np.where(rng.integers(0, 2, shape) == 1, -tiny, tiny), v)
+        v = np.where((kind >= 30) & (kind < 34), np.float32(0.0), v)
+        v = np.where((kind >= 34) & (kind < 38), np.float32(-0.0), v)
+        if f16:
+            near = rng.choice(np.array([65504.0, 65472.0, 65440.0, 60000.0, -65504.0], np.float32), size=shape)
+            v = np.where((kind >= 38) & (kind < 45), near, v)
+        vals = v.astype(dt)
+        bits = vals.view(np.uint16 if f16 else np.uint32)
+        nonfinite = ((y // 8 + x // 8) % 4 == 0) & (kind >= 88)
+        pos_inf, neg_inf = (0x7C00, 0xFC00) if f16 else (0x7F800000, 0xFF800000)
+        nans = np.array(_NAN_F16 if f16 else _NAN_F32, dtype=bits.dtype)
+        special = np.where(kind >= 96, nans[rng.integers(0, len(nans), shape)], np.where(kind >= 92, neg_inf, pos_inf)).astype(bits.dtype)
+        vals = np.where(nonfinite, special, bits).view(dt)
+    buf = np.zeros((height, stride), dtype=np.uint8)
+    buf[:, : width * bpp] = np.ascontiguousarray(vals).reshape(height, width * count).view(np.uint8).reshape(height, width * bpp)
+    return buf
+
+
 # ------------------------------------------------------------------------------------------ quaternions
 
 

@@ -17,7 +17,7 @@ def gyro(duration=4.0):
 
 
 def build(case):
-    """case keys: w,h [,ow,oh] pix lens [digital] [interp] [rs] [ts] [stride_pad] plus any KernelParams field override
+    """case keys: w,h [,ow,oh] pix lens [digital] [interp] [rs] [ts] [stride_pad] [edge_values] plus any KernelParams field override
     under 'params' and rects under 'in_rect'/'out_rect' (x,y,w,h) with 'in_size'/'out_size' = buffer (w,h)."""
     w, h = case["w"], case["h"]
     ow, oh = case.get("ow", w), case.get("oh", h)
@@ -33,7 +33,10 @@ def build(case):
     stride = bw * bpp + pad
     ostride = obw * bpp + case.get("out_stride_pad", pad)
     p = synth.base_kernel_params(w, h, ow, oh, pix, stride, ostride, lens, digital, case.get("interp", "Bilinear"), case.get("fov", 1.0))
-    src = synth.synthetic_frame(bw, bh, pix, frame=case.get("frame", 0), stride=stride)
+    if case.get("edge_values"):      # content at the edges of the value domain (synth.edge_frame)
+        src = synth.edge_frame(bw, bh, pix, seed=case.get("frame", 0), stride=stride)
+    else:
+        src = synth.synthetic_frame(bw, bh, pix, frame=case.get("frame", 0), stride=stride)
     if "in_rect" in case:
         p.source_rect[:] = list(case["in_rect"]); p.flags |= abi.FLAG_HAS_SOURCE_RECT
     else:
