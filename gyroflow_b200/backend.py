@@ -348,15 +348,16 @@ class DeviceGyro:
             raise GyroflowCoreError(rc, "gf_cuda_gyro_upload")
         self._h = h
 
-    def frame_transform(self, timestamp_ms, matrices_dev: int, max_rows: int, frame=0, stream=0, table_flags_dev: int = 0):
+    def frame_transform(self, timestamp_ms, matrices_dev: int, max_rows: int, frame=0, stream=0, table_flags_dev: int = 0, with_fov=False):
         """FrameTransform::at_timestamp on the device.  table_flags_dev: device word that receives the table's trust verdict.
-        stream = 0: the call waits for the kernel before returning; otherwise it only enqueues (give the warp the same stream)."""
+        stream = 0: the call waits for the kernel before returning; otherwise it only enqueues (give the warp the same stream).
+        Returns (KernelParams fields it sets, rows), or with_fov=True (KernelParams, rows, fov, minimal_fov) like ComputeParams.at_timestamp."""
         kp = abi.KernelParams(); rows = C.c_size_t(); fov = C.c_double(); mfov = C.c_double()
         rc = self._lib.gf_cuda_frame_transform_dev_flagged(self._h, C.byref(self.cp.c), timestamp_ms, frame, C.byref(kp), matrices_dev, max_rows,
                                                            table_flags_dev or None, C.byref(rows), C.byref(fov), C.byref(mfov), stream or None)
         if rc != 0:
             raise GyroflowCoreError(rc, "gf_cuda_frame_transform_dev")
-        return kp, rows.value
+        return (kp, rows.value, fov.value, mfov.value) if with_fov else (kp, rows.value)
 
     def find_fovs(self, distortion_model: str, digital_lens, timestamps_ms, margin=2.0, stream=0):
         """FovIterative::compute on the device: per-frame minimal FOV (zooming/fov_iterative.rs:31-134)."""

@@ -290,6 +290,12 @@ size_t prepare(const gf_compute_params* cp, double timestamp_ms, size_t frame, c
     return rows;
 }
 
+// One spline of a camera_stab entry.  A null position or value pointer means no points, whatever the count says: the host producer
+// and the device upload read an entry the same way.
+Spline3 stab_spline(const double* pos, const double* xyz, size_t n) {
+    return Spline3{ pos, xyz, (pos && xyz) ? n : 0 };
+}
+
 SyncOffsets host_offsets_of(const gf_compute_params* cp) {
     return SyncOffsets{ cp->sync_offset_ts_us, cp->sync_offset_ms, (cp->sync_offset_ts_us && cp->sync_offset_ms) ? cp->n_sync_offsets : 0, cp->gyro_offset_ms };
 }
@@ -316,7 +322,7 @@ GF_API int gf_frame_transform_at_timestamp(const gf_compute_params* cp, double t
     StabPoints sp; memset(&sp, 0, sizeof(sp));
     if (cp->camera_stab && frame < cp->n_camera_stab) {
         const gf_camera_stab& is = cp->camera_stab[frame];
-        sp.ibis = Spline3{ is.ibis_pos, is.ibis_xyz, is.n_ibis }; sp.ois = Spline3{ is.ois_pos, is.ois_xyz, is.n_ois };
+        sp.ibis = stab_spline(is.ibis_pos, is.ibis_xyz, is.n_ibis); sp.ois = stab_spline(is.ois_pos, is.ois_xyz, is.n_ois);
     }
     const size_t rows = prepare(cp, timestamp_ms, frame, org, sm, host_offsets_of(cp), &sp, C, out_params, out_fov, out_minimal_fov);
     if (out_rows) *out_rows = rows;
@@ -360,7 +366,7 @@ GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_
         for (size_t f = 0; f < cp->n_camera_stab; ++f) {
             const gf_camera_stab& is = cp->camera_stab[f];
             gf_cuda_gyro::StabIndex& ix = g->stab_index[f];
-            ix.n_ibis = is.ibis_pos && is.ibis_xyz ? is.n_ibis : 0; ix.n_ois = is.ois_pos && is.ois_xyz ? is.n_ois : 0;
+            ix.n_ibis = stab_spline(is.ibis_pos, is.ibis_xyz, is.n_ibis).n; ix.n_ois = stab_spline(is.ois_pos, is.ois_xyz, is.n_ois).n;
             ix.ibis_pos = flat.size(); flat.insert(flat.end(), is.ibis_pos, is.ibis_pos + ix.n_ibis);
             ix.ibis_val = flat.size(); flat.insert(flat.end(), is.ibis_xyz, is.ibis_xyz + 3 * ix.n_ibis);
             ix.ois_pos = flat.size();  flat.insert(flat.end(), is.ois_pos, is.ois_pos + ix.n_ois);

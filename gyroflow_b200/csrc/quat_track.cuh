@@ -38,7 +38,7 @@ GF_QT_HD Quat qslerp(const Quat& a, Quat b, double t) {
 // offsets / offsets_adjusted: BTreeMap<i64 us, f64 ms> as sorted arrays.  n == 0: the scalar fallback (a single sync point).
 struct SyncOffsets { const int64_t* ts; const double* ms; size_t n; double scalar_ms; };
 
-// gyro_source/mod.rs:884-909 — 0 points: 0; 1 point: its value; else linear interpolation between the neighbours of
+// gyro_source/mod.rs:884-909 — 0 points: the scalar offset (gyro_offset_ms); 1 point: its value; else linear interpolation between the neighbours of
 // clamp(ts, first + 1, last - 1), with the fraction taken from the UNclamped timestamp (so it extrapolates outside the range).
 GF_QT_HD double sync_offset_at(const SyncOffsets& o, double timestamp_ms) {
     if (o.n == 0) return o.scalar_ms;

@@ -43,10 +43,11 @@ def q_to_matrix(q):
 
 
 
-def offset_at_timestamp(offsets, timestamp_ms):
-    """GyroSource::offset_at_timestamp — gyro_source/mod.rs:884-909.  offsets: {timestamp_us: offset_ms}."""
+def offset_at_timestamp(offsets, timestamp_ms, scalar_ms=0.0):
+    """GyroSource::offset_at_timestamp — gyro_source/mod.rs:884-909.  offsets: {timestamp_us: offset_ms}; with no points the
+    scalar offset (gyro_offset_ms) applies."""
     if not offsets:
-        return 0.0
+        return scalar_ms
     ks = sorted(offsets)
     if len(ks) == 1:
         return offsets[ks[0]]
@@ -65,12 +66,13 @@ def offset_at_timestamp(offsets, timestamp_ms):
     return offsets[k1] + (offsets[k2] - offsets[k1]) * fract
 
 
-def quat_at_timestamp(track, timestamp_ms, offsets=None):
-    """gyro_source/mod.rs:857-879; vectorised over timestamp_ms.  offsets: {timestamp_us: offset_ms} or None."""
+def quat_at_timestamp(track, timestamp_ms, offsets=None, scalar_offset_ms=0.0):
+    """gyro_source/mod.rs:857-879; vectorised over timestamp_ms.  offsets: {timestamp_us: offset_ms} or None (then the scalar
+    scalar_offset_ms applies)."""
     self = track
     t = np.atleast_1d(np.asarray(timestamp_ms, dtype=np.float64))
-    if offsets:
-        t = t - np.array([offset_at_timestamp(offsets, float(v)) for v in t])
+    if offsets or scalar_offset_ms != 0.0:
+        t = t - np.array([offset_at_timestamp(offsets, float(v), scalar_offset_ms) for v in t])
     us = t * 1000.0
     lookup = np.clip((np.sign(us) * np.floor(np.abs(us) + 0.5)).astype(np.int64), self.ts[0], self.ts[-1])   # f64::round: half away from zero
     i1 = np.searchsorted(self.ts, lookup, side="right") - 1          # last key <= lookup
@@ -114,21 +116,32 @@ def stab_row(stab, y, width, height, framebuffer_inverted):
     if framebuffer_inverted:
         y_sensor = float(stab["sensor_size"][1]) - y_sensor
     z = np.zeros(3)
-    s = catmull_rom(np.asarray(stab["ibis"][0], float), np.asarray(stab["ibis"][1], float), y_sensor + stab["offset"])
-    o = catmull_rom(np.asarray(stab["ois"][0], float), np.asarray(stab["ois"][1], float), y_sensor + stab["offset"])
+    none = (np.zeros(0), np.zeros((0, 3)))                                 # an entry without a spline has no points
+    ibis, ois = stab.get("ibis", none), stab.get("ois", none)
+    s = catmull_rom(np.asarray(ibis[0], float), np.asarray(ibis[1], float).reshape(-1, 3), y_sensor + stab.get("offset", 0.0))
+    o = catmull_rom(np.asarray(ois[0], float), np.asarray(ois[1], float).reshape(-1, 3), y_sensor + stab.get("offset", 0.0))
     s = z if s is None else s; o = z if o is None else o
     ra = s[2] / 1000.0 * (-1.0 if framebuffer_inverted else 1.0)
     return (s[0] * sc[0], s[1] * sc[1], ra * (math.pi / 180.0), o[0] * sc[0], o[1] * sc[1])
 
 
 def frame_matrices(p, org, smoothed, timestamp_ms, frame_readout_time_ms=16.0, video_rotation_deg=0.0,
-                   horizontal=False, framebuffer_inverted=False, ibis=None, offsets=None, stab=None, fov_f64=None):
+                   horizontal=False, framebuffer_inverted=False, ibis=None, offsets=None, stab=None, fov_f64=None,
+                   gyro_offset_ms=0.0, suppress_rotation=False, camera_stab=None, frame=0, camera_matrix=None):
     """FrameTransform::at_timestamp rows — frame_transform.rs:221-308 (f64 -> f32).
 
-    ibis: optional callable row -> (sx, sy, ra_rad, ox, oy) filling m[9..13] (synthetic stand-in for the IBIS/OIS splines)."""
-    fx, fy, cx, cy = float(p.f[0]), float(p.f[1]), float(p.c[0]), float(p.c[1])
+    frame_readout_time_ms: the signed, scaled get_frame_readout_time (:22-36).
+    ibis: optional callable row -> (sx, sy, ra_rad, ox, oy) filling m[9..13] (synthetic stand-in for the IBIS/OIS splines).
+    offsets: multi-point sync offsets {timestamp_us: offset_ms}; without points gyro_offset_ms applies.
+    camera_stab: the per-frame CameraStabData list; frame `frame` is used, a frame past its end has none (:227).
+    camera_matrix: the frame's K (9 values, row-major) when it is not the KernelParams' f / c."""
+    if camera_matrix is None:
+        camera_matrix = [float(p.f[0]), 0.0, float(p.c[0]), 0.0, float(p.f[1]), float(p.c[1]), 0.0, 0.0, 1.0]
+    K = [float(v) for v in camera_matrix]
     fov = float(p.fov) if fov_f64 is None else float(fov_f64)      # the reference keeps fov in f64 until KernelParams (:191, :329)
-    new_k = np.array([[fx / fov, 0.0, p.output_width / 2.0], [0.0, fy / fov, p.output_height / 2.0], [0.0, 0.0, 1.0]])   # get_new_k :37-51
+    new_k = np.array([[K[0] / fov, K[1], p.output_width / 2.0], [K[3], K[4] / fov, p.output_height / 2.0], [K[6], K[7], K[8]]])   # get_new_k :37-51
+    if camera_stab is not None:
+        stab = camera_stab[frame] if frame < len(camera_stab) else None
     frt = frame_readout_time_ms
     n = (p.width if horizontal else p.height)
     rows = n if abs(frt) > 0.0 else 1
@@ -136,15 +149,17 @@ def frame_matrices(p, org, smoothed, timestamp_ms, frame_readout_time_ms=16.0, v
     start_ts = timestamp_ms - frt / 2.0
     a = math.radians(video_rotation_deg)
     image_rotation = np.array([[math.cos(a), -math.sin(a), 0.0], [math.sin(a), math.cos(a), 0.0], [0.0, 0.0, 1.0]])
-    quat1 = q_inv(quat_at_timestamp(org, timestamp_ms, offsets)[0])
-    sq1 = quat_at_timestamp(smoothed, timestamp_ms, offsets)[0]
+    quat1 = q_inv(quat_at_timestamp(org, timestamp_ms, offsets, gyro_offset_ms)[0])
+    sq1 = quat_at_timestamp(smoothed, timestamp_ms, offsets, gyro_offset_ms)[0]
     qt = start_ts + row_readout_time * np.arange(rows) if abs(frt) > 0.0 else np.array([start_ts])
-    quat = q_mul(q_mul(sq1[None, :], quat1[None, :]), quat_at_timestamp(org, qt, offsets))
+    quat = q_mul(q_mul(sq1[None, :], quat1[None, :]), quat_at_timestamp(org, qt, offsets, gyro_offset_ms))
     r = image_rotation[None] @ q_to_matrix(quat)
     if framebuffer_inverted:
         r[:, 0, 2] *= -1; r[:, 1, 2] *= -1; r[:, 2, 0] *= -1; r[:, 2, 1] *= -1
     else:
         r[:, 0, 1] *= -1; r[:, 0, 2] *= -1; r[:, 1, 0] *= -1; r[:, 2, 0] *= -1
+    if suppress_rotation:                                             # :289-290
+        r[:] = np.eye(3)
     i_r = np.linalg.pinv(new_k[None] @ r, rcond=1e-6)
     m = np.zeros((rows, 14), dtype=np.float32)
     m[:, :9] = i_r.reshape(rows, 9).astype(np.float32)
@@ -154,6 +169,8 @@ def frame_matrices(p, org, smoothed, timestamp_ms, frame_readout_time_ms=16.0, v
     if stab is not None:
         for y in range(rows):
             m[y, 9:14] = np.asarray(stab_row(stab, y, p.width, p.height, framebuffer_inverted), dtype=np.float32)
+    if suppress_rotation and frt == 0.0:                              # :289-293: no rotation and no rolling shutter, no shifts either
+        m[:, 9:14] = 0.0
     return m
 
 

@@ -2,8 +2,10 @@
 sync, FrameTransform::at_timestamp (producer kernel + trust verdict) -> warp; `depth` frames in flight; results in submission order.
 
 Parity: every frame's bytes (and the queue's device-side checksum) against the oracle run on the table the device producer wrote
-for that timestamp (read back through gf_cuda_frame_transform_dev, the same deterministic kernel).  The 2-rank test renders frames
-`rank::2` of one job on two processes and gathers the per-frame checksums in frame order — over NCCL when the box has two GPUs,
+for that timestamp (read back through gf_cuda_frame_transform_dev, the same deterministic kernel).  That table is itself checked
+against the host producer (gf_frame_transform_at_timestamp: IBIS / OIS columns bit-identical, the rest within 1 f32 ulp), and
+tests/test_device_producer.py checks the host producer against the numpy restatement, so a wrong device table cannot pass as its
+own reference.  The 2-rank test renders frames `rank::2` of one job on two processes and gathers the per-frame checksums in frame order — over NCCL when the box has two GPUs,
 over gloo with both ranks on GPU 0 otherwise (the data path has no collective either way)."""
 import os
 import socket
@@ -13,7 +15,7 @@ import pytest
 
 import gyroflow_b200 as g
 from gyroflow_b200 import abi, render_queue, synth
-from tests import cases, oracle_lib
+from tests import cases, oracle_lib, producer_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -31,8 +33,11 @@ def _job(pix="RGBA8", lens="opencv_fisheye", digital=None, w=W, h=H, **cpkw):
 def _expected(p, cp, st, dg, mats_dev, ts, frame, src, pix, lens, digital, bufs, mesh=None):
     """The frame as the reference would render it from the table the device producer writes for (ts, frame)."""
     kp, rows = dg.frame_transform(ts, mats_dev.data_ptr(), max(p.width, p.height), frame=frame)     # stream = 0: synchronous
-    g.get_frame_transform_at(st, cp, bufs, kp, mesh=mesh, frame=frame)
     table = mats_dev.cpu().numpy()[:rows].copy()
+    kp_h, table_h, _, _ = cp.at_timestamp(ts, frame)              # the host producer: same KernelParams, the same table to the bars
+    assert bytes(kp) == bytes(kp_h)                               # of tests/test_device_producer.py
+    producer_cases.compare_tables(table, table_h)
+    g.get_frame_transform_at(st, cp, bufs, kp, mesh=mesh, frame=frame)
     want = np.zeros((p.output_height, p.output_stride), np.uint8)
     assert oracle_lib.undistort_image(src, want, kp, pix, lens, digital, table, mesh) == 0
     return want
@@ -71,13 +76,17 @@ def test_queue_device_buffers_every_frame_matches_oracle():
     ("RGBA8", "opencv_fisheye", None, {}),
     ("Luma16", "opencv_fisheye", "gopro_superview", {}),
     ("RGBAf", "sony", None, dict(stab=True, mesh=True)),          # IBIS rows from the spline producer + per-frame mesh: guarded / general kernel
+    ("RGBA8", "opencv_fisheye", None, dict(stab="alternate")),     # packed kernel, consecutive slots alternate between verdicts 2 and 0
 ])
 def test_queue_host_buffers_pipelined(pix, lens, digital, extra):
     import torch
     from tests.test_frame_transform import _stab
     n = 9
     kw = {}
-    if extra.get("stab"):
+    if extra.get("stab") == "alternate":      # spline points on even frames (counts differ), none on odd ones, frames 7 and 8 past the end
+        stab = producer_cases.spline_stab([12, 0, 31, 0, 6, 0, 19], seed=8)
+        kw = dict(camera_stab=stab, sync_offsets={500_000: 3.0, 800_000: -1.5, 1_200_000: 2.5})
+    elif extra.get("stab"):
         kw = dict(camera_stab=_stab(n, H), per_frame_time_offsets=[0.25 * i for i in range(n)], sync_offsets={0: 1.0, 2_000_000: -2.0, 4_000_000: 0.5})
     p, cp, st = _job(pix, lens, digital, **kw)
     mesh = synth.synthetic_mesh(W, H) if extra.get("mesh") else None
@@ -94,8 +103,12 @@ def test_queue_host_buffers_pipelined(pix, lens, digital, extra):
         want = _expected(p, cp, st, dg, mats, ts_of(f), f, srcs[f % 3].numpy(), pix, lens, digital, bufs[f], mesh)
         assert np.array_equal(outs[f].numpy(), want), "frame %d" % f
         assert sums[f] == render_queue.checksum_host(want)
-    if extra.get("stab"):
+    if extra.get("stab") is True:
         assert np.abs(mats.cpu().numpy()[:H, 9:]).max() > 1.0       # the IBIS columns really were exercised
+    if extra.get("stab") == "alternate":      # the verdict each slot's producer gave: IBIS rows on even frames up to 6, nothing else
+        for f in range(n):
+            _, table, _, _ = cp.at_timestamp(ts_of(f), f)
+            assert producer_cases.table_flags_host(table) == (2 if f % 2 == 0 and f < 7 else 0), f
     dg.close()
 
 
