@@ -224,17 +224,6 @@ __global__ void __launch_bounds__(1024) scan_tables_kernel(const float* __restri
     }
 }
 
-bool lens_noop(int lens, const gf_kernel_params* p) {
-    const float* k = p->k;
-    switch (lens) {
-    case GF_LENS_OPENCV_FISHEYE:
-    case GF_LENS_SONY:               return k[0] == 0.0f && k[1] == 0.0f && k[2] == 0.0f && k[3] == 0.0f;
-    case GF_LENS_GENERIC_POLYNOMIAL: { for (int i = 0; i < 12; ++i) if (!(k[i] == 0.0f)) return false; return true; }
-    case GF_LENS_GOPRO:              return k[1] == 0.0f;
-    default: return false;
-    }
-}
-
 // Everything the reference recomputes per pixel from per-frame constants (cpu_undistort.rs:421-528), computed once, on the
 // host, with the same IEEE float operations (this TU is built with -ffp-contract=off; sin/cos come from gf_math.cuh, the
 // same code the device runs).
@@ -264,7 +253,7 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     if (p->background_mode == 3) f |= F_BG3;
     if ((p->flags & 1) == 1) f |= F_FIXRANGE;
     if ((p->flags & 4) == 4) f |= F_FILLBG;
-    if (lens_noop(c.lens, p)) f |= F_LENS_NOOP;
+    if (lens_noop(c.lens, p->k)) f |= F_LENS_NOOP;
     if ((reinterpret_cast<uintptr_t>(src) % (uintptr_t)align) == 0 && (p->stride % align) == 0) f |= F_SRC_VEC;
     if ((f & F_SRC_VEC) && (reinterpret_cast<uintptr_t>(src) % 8u) == 0 && (p->stride % 8) == 0 && (A.src_len % 8ull) == 0) f |= F_SRC_VEC8;
     if ((reinterpret_cast<uintptr_t>(dst) % (uintptr_t)align) == 0 && (p->output_stride % align) == 0) f |= F_DST_VEC;
@@ -664,6 +653,16 @@ int gf_internal_run_frame(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_b
     return run_warp(ctx, job);
 }
 
+bool gf::lens_noop(int lens, const float* k) {
+    switch (lens) {
+    case GF_LENS_OPENCV_FISHEYE:
+    case GF_LENS_SONY:               return k[0] == 0.0f && k[1] == 0.0f && k[2] == 0.0f && k[3] == 0.0f;
+    case GF_LENS_GENERIC_POLYNOMIAL: { for (int i = 0; i < 12; ++i) if (!(k[i] == 0.0f)) return false; return true; }
+    case GF_LENS_GOPRO:              return k[1] == 0.0f;
+    default: return false;
+    }
+}
+
 extern "C" {
 
 GF_API int gf_cuda_device_count(void) {
@@ -848,18 +847,8 @@ GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_u
     cp.fov_scale = 1.0; cp.output_width = width; cp.output_height = height;                  // :44-46
 
     // bbox of the undistorted frame edge: points_around_rect(width, height, 31, 31) with fov_algorithm_margin = 0 (:58-60, fov_iterative.rs:154-175)
-    std::vector<float> rect, und;
-    {
-        const float w = (float)width, h = (float)height;
-        const int wcnt = 30, hcnt = 30;
-        const float wstep = w / (float)wcnt, hstep = h / (float)hcnt;
-        for (int i = 0; i < wcnt; ++i) { rect.push_back((float)i * wstep); rect.push_back(0.0f); }
-        for (int i = 0; i < hcnt; ++i) { rect.push_back(w); rect.push_back((float)i * hstep); }
-        for (int i = 0; i < wcnt; ++i) { rect.push_back((float)(wcnt - i) * wstep); rect.push_back(h); }
-        for (int i = 0; i < hcnt; ++i) { rect.push_back(0.0f); rect.push_back((float)(hcnt - i) * hstep); }
-        for (float& v : rect) v += 0.0f;
-    }
-    und.resize(rect.size());
+    std::vector<float> rect(2 * RECT_POINTS), und(2 * RECT_POINTS);
+    for (int k = 0; k < RECT_POINTS; ++k) rect_point((float)width, (float)height, 0.0f, k, rect[2 * k], rect[2 * k + 1]);
     int rc = gf_cuda_undistort_points(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, 0, 1.0, rect.data(), rect.size() / 2, und.data(), cu_stream);
     if (rc != GF_OK) return fail(nullptr, rc, "gf_cuda_undistort_points failed");
     float min_x = 0.0f, min_y = 0.0f, max_x = 0.0f, max_y = 0.0f;                             // :62-71 (f32::min / max ignore NaN)

@@ -4,6 +4,7 @@
 #include <cstddef>
 #include <cstdint>
 #include "../../include/gyroflow_cuda.h"
+#include "frame_geometry.cuh"
 
 namespace gf {
 
@@ -20,6 +21,27 @@ __host__ __device__ __forceinline__ uint32_t table_row_verdict(const float* r) {
     for (unsigned i = 0; i < GF_MATRIX_STRIDE; ++i) f |= table_entry_verdict(i, r[i]);
     return f;
 }
+
+// The host half of the per-frame geometry (frame_transform.cu), shared by the matrix producer (at_timestamp) and the point path
+// (at_timestamp_for_points).
+// `params.keyframes.value_at_video_timestamp(typ, ts).unwrap_or(dflt)`
+double keyframed(const gf_compute_params* cp, int typ, double timestamp_ms, double dflt);
+// get_fov (frame_transform.rs:52-58) without its last line, `fov *= width / output_width.max(1)`, which the callers apply: the producer in
+// that order, the point path as (fov * width) / output_width, like the oracle's transcription of at_timestamp_for_points.
+double fov_unscaled(const gf_compute_params* cp, size_t frame, bool use_fovs, double timestamp_ms, bool for_ui);
+// get_new_k — frame_transform.rs:37-51
+void get_new_k(const gf_compute_params* cp, const double* camera_matrix, double fov, double (&new_k)[9]);
+// Readout timing and base rotation of one frame — frame_transform.rs:221-225,243-244 (at_timestamp), :376-388 (at_timestamp_for_points)
+struct FrameTiming {
+    double frame_readout_time;            // get_frame_readout_time(can_invert): signed and scaled
+    double row_readout_time, start_ts;    // start_ts includes the frame's per_frame_time_offsets entry
+    Quat q0;                              // smoothed(ts) * org(ts)^-1 through the host tracks and sync offsets
+};
+FrameTiming frame_timing(const gf_compute_params* cp, size_t frame, double timestamp_ms, bool can_invert);
+// camera_stab[frame] with `splines` as its spline points; absent when the frame has no entry or `splines` is null
+CameraStab camera_stab_at(const gf_compute_params* cp, size_t frame, bool framebuffer_inverted, const StabSplines* splines);
+// the lens model is the identity for these coefficients (c_abi.cu)
+bool lens_noop(int lens, const float* k);
 
 } // namespace gf
 

@@ -4,7 +4,9 @@
 // (:22-36), get_new_k (:37-51), get_fov (:52-58), focal_length_fov_compensation (:70-80), the IBIS / OIS row fill (:227-287 with
 // CatmullRom::interpolate, gyro_source/splines.rs:22-83), per_frame_time_offsets (:224), GyroSource::quat_at_timestamp with
 // multi-point sync offsets (src/core/gyro_source/mod.rs:857-909); quaternion algebra as nalgebra 0.34.2's UnitQuaternion<f64>
-// (slerp, product, to_rotation_matrix) in quat_track.cuh.  All f64, narrowed to f32 at the very end (:300).
+// (slerp, product, to_rotation_matrix) in quat_track.cuh; the rotation and shift of one row in frame_geometry.cuh.  All f64, narrowed to
+// f32 at the very end (:300).  The per-frame host setup (keyframes, fov, K_new, readout timing, camera_stab) is shared with the point
+// path of zoom_kernel.cu through c_abi_internal.h.
 // Not evaluated here (they stay in Rust, see INTEGRATION.md "what stays on the Rust side"): keyframe curves (the caller passes
 // the per-timestamp values in gf_compute_params), lens-profile interpolation (get_lens_data_at_timestamp: the caller passes the
 // resulting camera matrix / coefficients), and mesh extraction from metadata (the caller passes mesh_data to the warp).
@@ -17,7 +19,7 @@
 #include <vector>
 #include "../../include/gyroflow_cuda.h"
 #include "c_abi_internal.h"
-#include "quat_track.cuh"
+#include "frame_geometry.cuh"
 
 #define GF_FT_HD __host__ __device__ __forceinline__
 
@@ -26,11 +28,6 @@ using namespace gf;
 namespace {
 
 // everything per-frame-uniform the row function needs
-struct StabRow {                  // camera_stab_data[frame] resolved for the row function (:227-236, :269-287)
-    int present;
-    double offset, sensor_h, crop_y, crop_h, scale_x, scale_y, height;
-    Spline3 ibis, ois;
-};
 struct RowCtx {
     Track org;
     SyncOffsets offsets;
@@ -40,32 +37,16 @@ struct RowCtx {
     double new_k[9];              // :37-51
     double start_ts, row_readout_time;
     int rs_on, framebuffer_inverted, suppress_rotation, zero_shifts;
-    StabRow stab;
+    CameraStab stab;
 };
-
-GF_FT_HD void mat3_mul(const double* a, const double* b, double* o) {
-    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) o[r * 3 + c] = a[r * 3 + 0] * b[0 * 3 + c] + a[r * 3 + 1] * b[1 * 3 + c] + a[r * 3 + 2] * b[2 * 3 + c];
-}
 
 // one scanline: frame_transform.rs:249-308
 GF_FT_HD void frame_row(const RowCtx& C, size_t y, float* out14) {
     const double quat_time = C.rs_on ? C.start_ts + C.row_readout_time * (double)y : C.start_ts;       // :250-254
     const Quat qy = quat_at_timestamp(C.org, C.duration_ms, C.offsets, quat_time);
     const Quat q = qmul(C.q0, qy);                                                                     // :255-257
-    // UnitQuaternion::to_rotation_matrix
-    const double ww = q.w * q.w, ii = q.i * q.i, jj = q.j * q.j, kk = q.k * q.k;
-    const double ij = q.i * q.j * 2.0, wk = q.w * q.k * 2.0, wj = q.w * q.j * 2.0, ik = q.i * q.k * 2.0, jk = q.j * q.k * 2.0, wi = q.w * q.i * 2.0;
-    const double rq[9] = { ww + ii - jj - kk, ij - wk, wj + ik,
-                           wk + ij, ww - ii + jj - kk, jk - wi,
-                           ik - wj, wi + jk, ww - ii - jj + kk };
-    const double rz[9] = { C.rot_c, -C.rot_s, 0.0, C.rot_s, C.rot_c, 0.0, 0.0, 0.0, 1.0 };
-    double r[9];
-    mat3_mul(rz, rq, r);                                                                               // :260
-    if (C.framebuffer_inverted) { r[2] *= -1.0; r[5] *= -1.0; r[6] *= -1.0; r[7] *= -1.0; }            // :261-264
-    else                        { r[1] *= -1.0; r[2] *= -1.0; r[3] *= -1.0; r[6] *= -1.0; }            // :265-266
-    if (C.suppress_rotation) { for (int t = 0; t < 9; ++t) r[t] = (t % 4 == 0) ? 1.0 : 0.0; }          // :289-290
     double m[9];
-    mat3_mul(C.new_k, r, m);
+    frame_rotation(q, C.rot_c, C.rot_s, C.new_k, C.framebuffer_inverted, C.suppress_rotation, m);      // :258-266,289-291
     // pinv(m): m is invertible (K_new has a positive focal length, r is a rotation up to sign flips) -> inverse via cofactors
     const double c00 = m[4] * m[8] - m[5] * m[7], c01 = m[5] * m[6] - m[3] * m[8], c02 = m[3] * m[7] - m[4] * m[6];
     const double det = m[0] * c00 + m[1] * c01 + m[2] * c02;
@@ -77,22 +58,10 @@ GF_FT_HD void frame_row(const RowCtx& C, size_t y, float* out14) {
         inv[6] = c02 * id;                          inv[7] = (m[1] * m[6] - m[0] * m[7]) * id; inv[8] = (m[0] * m[4] - m[1] * m[3]) * id;
     }
     for (int t = 0; t < 9; ++t) out14[t] = (float)inv[t];                                              // :300-304
-    double sx = 0.0, sy = 0.0, ra = 0.0, ox = 0.0, oy = 0.0;                                           // :286
-    if (C.stab.present) {                                                                              // :269-285
-        const StabRow& S = C.stab;
-        double y_sensor = ((double)y - 0.0) * ((S.crop_y + S.crop_h) - S.crop_y) / (S.height - 0.0) + S.crop_y;   // map_coord, util.rs:144-147
-        if (C.framebuffer_inverted) y_sensor = S.sensor_h - y_sensor;
-        double v[3] = { 0.0, 0.0, 0.0 };
-        if (!catmull_rom3(S.ibis, y_sensor + S.offset, v)) { v[0] = v[1] = v[2] = 0.0; }               // unwrap_or_default
-        sx = v[0] * S.scale_x; sy = v[1] * S.scale_y;
-        ra = v[2] / 1000.0 * (C.framebuffer_inverted ? -1.0 : 1.0);
-        ra = ra * (3.14159265358979323846 / 180.0);                                                    // f64::to_radians
-        double o[3] = { 0.0, 0.0, 0.0 };
-        if (!catmull_rom3(S.ois, y_sensor + S.offset, o)) { o[0] = o[1] = o[2] = 0.0; }
-        ox = o[0] * S.scale_x; oy = o[1] * S.scale_y;
-    }
-    if (C.zero_shifts) { sx = sy = ra = ox = oy = 0.0; }                                               // :289-293 (suppress_rotation without rolling shutter)
-    out14[9] = (float)sx; out14[10] = (float)sy; out14[11] = (float)ra; out14[12] = (float)ox; out14[13] = (float)oy;
+    double sh[5] = { 0.0, 0.0, 0.0, 0.0, 0.0 };                                                        // :286
+    if (C.stab.present) stab_shift(C.stab, (double)y, C.framebuffer_inverted, sh);                     // :269-285
+    if (C.zero_shifts) { sh[0] = sh[1] = sh[2] = sh[3] = sh[4] = 0.0; }                                // :289-293 (suppress_rotation without rolling shutter)
+    for (int t = 0; t < 5; ++t) out14[9 + t] = (float)sh[t];
 }
 
 // One thread per scanline.  The table's trust verdict (see warp_kernel_x2) is produced with it: every block ORs its rows into an
@@ -159,27 +128,76 @@ bool keyframe_value(const gf_keyframe_track& t, double timestamp_ms, double scal
     *out = t.value[i1] * (1.0 - x) + t.value[i2] * x;
     return true;
 }
-// `params.keyframes.value_at_video_timestamp(typ, ts).unwrap_or(default)`
-double keyframed(const gf_compute_params* cp, int typ, double timestamp_ms, double dflt) {
+// get_frame_readout_time — frame_transform.rs:22-36 (`scale` = capture_area_size.1 / sensor_size_px.1 of the closest lens_params
+// entry, resolved by the caller into cp->readout_time_scale; 0 = no entry = 1.0)
+double get_frame_readout_time(const gf_compute_params* cp, bool can_invert) {
+    double t = fabs(cp->frame_readout_time);
+    const double scale = cp->readout_time_scale != 0.0 ? cp->readout_time_scale : 1.0;
+    if (can_invert && cp->framebuffer_inverted && !cp->readout_horizontal) t *= -1.0;
+    if (cp->readout_inverted) t *= -1.0;
+    return t * scale;
+}
+
+SyncOffsets host_offsets_of(const gf_compute_params* cp) {
+    return SyncOffsets{ cp->sync_offset_ts_us, cp->sync_offset_ms, (cp->sync_offset_ts_us && cp->sync_offset_ms) ? cp->n_sync_offsets : 0, cp->gyro_offset_ms };
+}
+
+} // namespace
+
+double gf::keyframed(const gf_compute_params* cp, int typ, double timestamp_ms, double dflt) {
     double v;
     return keyframe_value(cp->keyframes[typ], timestamp_ms, cp->keyframe_timestamp_scale, &v) ? v : dflt;
 }
 
-// get_fov — frame_transform.rs:52-58
-double get_fov(const gf_compute_params* cp, size_t frame, bool use_fovs, double timestamp_ms, bool for_ui) {
+double gf::fov_unscaled(const gf_compute_params* cp, size_t frame, bool use_fovs, double timestamp_ms, bool for_ui) {
     double fov_scale = keyframed(cp, GF_KF_FOV, timestamp_ms, cp->fov_scale);
     fov_scale += (cp->fov_overview && use_fovs && !for_ui) ? 1.0 : 0.0;
     double fov = 1.0;
     if (use_fovs) {
         double f = 1.0;
-        if (frame < cp->n_fovs) f = cp->fovs[frame];
-        else if (cp->n_fovs > 1) f = cp->fovs[cp->n_fovs - 1];
+        if (cp->fovs && frame < cp->n_fovs) f = cp->fovs[frame];
+        else if (cp->fovs && cp->n_fovs > 1) f = cp->fovs[cp->n_fovs - 1];
         fov = f * fov_scale;
     }
-    fov = fmax(fov, 0.001);
-    fov *= (double)cp->width / (double)(cp->output_width > 1 ? cp->output_width : 1);
-    return fov;
+    return fmax(fov, 0.001);
 }
+
+void gf::get_new_k(const gf_compute_params* cp, const double* camera_matrix, double fov, double (&new_k)[9]) {
+    const double hr = cp->input_horizontal_stretch > 0.01 ? cp->input_horizontal_stretch : 1.0;     // :38 reads params.lens, the base profile
+    const double img_dim_ratio = 1.0 / hr;
+    memcpy(new_k, camera_matrix, sizeof(new_k));
+    new_k[0] = new_k[0] * img_dim_ratio / fov; new_k[4] = new_k[4] * img_dim_ratio / fov;                   // :46-47
+    new_k[2] = (double)cp->output_width / 2.0; new_k[5] = (double)cp->output_height / 2.0;                  // :48-49
+}
+
+gf::FrameTiming gf::frame_timing(const gf_compute_params* cp, size_t frame, double timestamp_ms, bool can_invert) {
+    FrameTiming t;
+    t.frame_readout_time = get_frame_readout_time(cp, can_invert);
+    t.row_readout_time = t.frame_readout_time / (double)(cp->readout_horizontal ? cp->width : cp->height);
+    if (cp->per_frame_time_offsets && frame < cp->n_per_frame_time_offsets) timestamp_ms += cp->per_frame_time_offsets[frame];
+    t.start_ts = timestamp_ms - t.frame_readout_time / 2.0;
+    const Track org{ cp->org.ts_us, cp->org.quats, cp->org.n }, sm{ cp->smoothed.ts_us, cp->smoothed.quats, cp->smoothed.n };
+    const SyncOffsets ho = host_offsets_of(cp);
+    const Quat quat1 = qinv(quat_at_timestamp(org, cp->duration_ms, ho, timestamp_ms));
+    t.q0 = qmul(quat_at_timestamp(sm, cp->duration_ms, ho, timestamp_ms), quat1);
+    return t;
+}
+
+gf::CameraStab gf::camera_stab_at(const gf_compute_params* cp, size_t frame, bool framebuffer_inverted, const StabSplines* splines) {
+    CameraStab s; memset(&s, 0, sizeof(s));
+    if (!cp->camera_stab || frame >= cp->n_camera_stab || !splines) return s;
+    const gf_camera_stab& is = cp->camera_stab[frame];
+    s.present = 1;
+    s.offset = is.offset; s.sensor_h = (double)is.sensor_size[1];
+    s.crop_y = (double)is.crop_area[1]; s.crop_h = (double)is.crop_area[3];
+    s.height = (double)cp->height;
+    s.scale_x = (double)cp->width  / (double)is.crop_area[2] / (double)is.pixel_pitch[0];
+    s.scale_y = (double)cp->height / (double)is.crop_area[3] / (double)is.pixel_pitch[1] * (framebuffer_inverted ? -1.0 : 1.0);
+    s.ibis = splines->ibis; s.ois = splines->ois;
+    return s;
+}
+
+namespace {
 
 // focal_length_fov_compensation — frame_transform.rs:70-80.  None is encoded as NaN (or any non-positive value, which the
 // reference maps to 1.0 as well).
@@ -191,22 +209,10 @@ double focal_length_fov_compensation(const gf_compute_params* cp, size_t frame) 
     return 1.0;
 }
 
-// get_frame_readout_time — frame_transform.rs:22-36 (`scale` = capture_area_size.1 / sensor_size_px.1 of the closest lens_params
-// entry, resolved by the caller into cp->readout_time_scale; 0 = no entry = 1.0)
-double get_frame_readout_time(const gf_compute_params* cp, bool can_invert) {
-    double t = fabs(cp->frame_readout_time);
-    const double scale = cp->readout_time_scale != 0.0 ? cp->readout_time_scale : 1.0;
-    if (can_invert && cp->framebuffer_inverted && !cp->readout_horizontal) t *= -1.0;
-    if (cp->readout_inverted) t *= -1.0;
-    return t * scale;
-}
-
-// the per-frame-uniform part of at_timestamp: fills RowCtx + KernelParams, returns the number of rows.
-// `stab_dev`: the frame's spline points as the row function will address them (host pointers for the host producer, the uploaded
-// copies for the device producer).
-struct StabPoints { Spline3 ibis, ois; };
-size_t prepare(const gf_compute_params* cp, double timestamp_ms, size_t frame, const Track& org, const Track& smoothed_host,
-               const SyncOffsets& host_offsets, const StabPoints* stab_points,
+// the per-frame-uniform part of at_timestamp: fills RowCtx (with the host tracks and sync offsets) + KernelParams, returns the number
+// of rows.  `stab_splines`: the frame's spline points as the row function will address them (host pointers for the host producer, the
+// uploaded copies for the device producer), or null when there are none.
+size_t prepare(const gf_compute_params* cp, double timestamp_ms, size_t frame, const StabSplines* stab_splines,
                RowCtx& C, gf_kernel_params* kp, double* out_fov, double* out_minimal_fov) {
     // ----------- Keyframes :167-174 (evaluated at the frame's own timestamp, before per_frame_time_offsets) -----------
     const double video_rotation = keyframed(cp, GF_KF_VIDEO_ROTATION, timestamp_ms, cp->video_rotation);
@@ -217,8 +223,9 @@ size_t prepare(const gf_compute_params* cp, double timestamp_ms, size_t frame, c
     const double zoom_center_y = keyframed(cp, GF_KF_ZOOMING_CENTER_Y, timestamp_ms, cp->adaptive_zoom_center_offset[1]);
     const double light_refraction_coefficient = keyframed(cp, GF_KF_LIGHT_REFRACTION_COEFF, timestamp_ms, cp->light_refraction_coefficient);
     const double fl_compensation = focal_length_fov_compensation(cp, frame);                                              // :190
-    double fov = get_fov(cp, frame, true, timestamp_ms, false) * fl_compensation;                                         // :191
-    double ui_fov = get_fov(cp, frame, true, timestamp_ms, true);
+    const double size_ratio = (double)cp->width / (double)(cp->output_width > 1 ? cp->output_width : 1);                  // get_fov :56
+    double fov = fov_unscaled(cp, frame, true, timestamp_ms, false) * size_ratio * fl_compensation;                       // :191
+    double ui_fov = fov_unscaled(cp, frame, true, timestamp_ms, true) * size_ratio;
     if (cp->has_optimal_fov) { if (cp->n_fovs == 0) fov *= cp->lens_optimal_fov; else ui_fov /= cp->lens_optimal_fov; }   // :193-199
     // ----------- Lens :183-188: this frame's get_lens_data_at_timestamp result when the caller supplies one per frame -----------
     const gf_lens_data* lens = (cp->lens_per_frame && frame < cp->n_lens_per_frame) ? &cp->lens_per_frame[frame] : nullptr;
@@ -228,41 +235,21 @@ size_t prepare(const gf_compute_params* cp, double timestamp_ms, size_t frame, c
     const double ihs = lens ? lens->input_horizontal_stretch : cp->input_horizontal_stretch;
     const double ivs = lens ? lens->input_vertical_stretch : cp->input_vertical_stretch;
     const double hr_frame = ihs > 0.01 ? ihs : 1.0;                                                                     // :146 (the lens of this timestamp)
-    const double hr = cp->input_horizontal_stretch > 0.01 ? cp->input_horizontal_stretch : 1.0;                         // :38 get_new_k reads params.lens, the base profile
-    const double img_dim_ratio = 1.0 / hr;
-    double new_k[9]; memcpy(new_k, K, sizeof(new_k));
-    new_k[0] = new_k[0] * img_dim_ratio / fov; new_k[4] = new_k[4] * img_dim_ratio / fov;                                 // :46-47
-    new_k[2] = (double)cp->output_width / 2.0; new_k[5] = (double)cp->output_height / 2.0;                                // :48-49
 
-    const double frame_readout_time = get_frame_readout_time(cp, true);                                                   // :221
+    const FrameTiming t = frame_timing(cp, frame, timestamp_ms, true);                                                   // :221-225,243-244
     const size_t n = (size_t)(cp->readout_horizontal ? cp->width : cp->height);
-    const double row_readout_time = frame_readout_time / (double)n;                                                       // :223
-    if (cp->per_frame_time_offsets && frame < cp->n_per_frame_time_offsets) timestamp_ms += cp->per_frame_time_offsets[frame];   // :224
-    const double start_ts = timestamp_ms - frame_readout_time / 2.0;                                                      // :225
-    const size_t rows = fabs(frame_readout_time) > 0.0 ? n : 1;                                                           // :247
+    const size_t rows = fabs(t.frame_readout_time) > 0.0 ? n : 1;                                                         // :247
 
     const double a = video_rotation * (M_PI / 180.0);
-    const Quat quat1 = qinv(quat_at_timestamp(org, cp->duration_ms, host_offsets, timestamp_ms));                         // :243
-    const Quat sq1 = quat_at_timestamp(smoothed_host, cp->duration_ms, host_offsets, timestamp_ms);                       // :244
-    C.org = org; C.duration_ms = cp->duration_ms; C.offsets = host_offsets;
-    C.q0 = qmul(sq1, quat1);
+    C.org = Track{ cp->org.ts_us, cp->org.quats, cp->org.n }; C.duration_ms = cp->duration_ms; C.offsets = host_offsets_of(cp);
+    C.q0 = t.q0;
     C.rot_c = cos(a); C.rot_s = sin(a);
-    memcpy(C.new_k, new_k, sizeof(new_k));
-    C.start_ts = start_ts; C.row_readout_time = row_readout_time;
-    C.rs_on = fabs(frame_readout_time) > 0.0 ? 1 : 0;
+    get_new_k(cp, K, fov, C.new_k);
+    C.start_ts = t.start_ts; C.row_readout_time = t.row_readout_time;
+    C.rs_on = fabs(t.frame_readout_time) > 0.0 ? 1 : 0;
     C.framebuffer_inverted = cp->framebuffer_inverted; C.suppress_rotation = cp->suppress_rotation;
     C.zero_shifts = (cp->suppress_rotation && cp->frame_readout_time == 0.0) ? 1 : 0;                                     // :289-293
-    memset(&C.stab, 0, sizeof(C.stab));
-    if (cp->camera_stab && frame < cp->n_camera_stab && stab_points) {                                                    // :227-236
-        const gf_camera_stab& is = cp->camera_stab[frame];
-        C.stab.present = 1;
-        C.stab.offset = is.offset; C.stab.sensor_h = (double)is.sensor_size[1];
-        C.stab.crop_y = (double)is.crop_area[1]; C.stab.crop_h = (double)is.crop_area[3];
-        C.stab.height = (double)cp->height;
-        C.stab.scale_x = (double)cp->width  / (double)is.crop_area[2] / (double)is.pixel_pitch[0];
-        C.stab.scale_y = (double)cp->height / (double)is.crop_area[3] / (double)is.pixel_pitch[1] * (cp->framebuffer_inverted ? -1.0 : 1.0);
-        C.stab.ibis = stab_points->ibis; C.stab.ois = stab_points->ois;
-    }
+    C.stab = camera_stab_at(cp, frame, cp->framebuffer_inverted, stab_splines);                                           // :227-236
 
     if (kp) {                                                                                                             // :322-340
         memset(kp, 0, sizeof(*kp));
@@ -296,10 +283,6 @@ Spline3 stab_spline(const double* pos, const double* xyz, size_t n) {
     return Spline3{ pos, xyz, (pos && xyz) ? n : 0 };
 }
 
-SyncOffsets host_offsets_of(const gf_compute_params* cp) {
-    return SyncOffsets{ cp->sync_offset_ts_us, cp->sync_offset_ms, (cp->sync_offset_ts_us && cp->sync_offset_ms) ? cp->n_sync_offsets : 0, cp->gyro_offset_ms };
-}
-
 } // namespace
 
 #include "gyro_dev.h"
@@ -318,13 +301,12 @@ GF_API int gf_frame_transform_at_timestamp(const gf_compute_params* cp, double t
                                            size_t* out_rows, double* out_fov, double* out_minimal_fov) {
     if (!cp || !out_matrices) return GF_ERR_BAD_PARAMS;
     RowCtx C;
-    const Track org{cp->org.ts_us, cp->org.quats, cp->org.n}, sm{cp->smoothed.ts_us, cp->smoothed.quats, cp->smoothed.n};
-    StabPoints sp; memset(&sp, 0, sizeof(sp));
+    StabSplines sp; memset(&sp, 0, sizeof(sp));
     if (cp->camera_stab && frame < cp->n_camera_stab) {
         const gf_camera_stab& is = cp->camera_stab[frame];
         sp.ibis = stab_spline(is.ibis_pos, is.ibis_xyz, is.n_ibis); sp.ois = stab_spline(is.ois_pos, is.ois_xyz, is.n_ois);
     }
-    const size_t rows = prepare(cp, timestamp_ms, frame, org, sm, host_offsets_of(cp), &sp, C, out_params, out_fov, out_minimal_fov);
+    const size_t rows = prepare(cp, timestamp_ms, frame, &sp, C, out_params, out_fov, out_minimal_fov);
     if (out_rows) *out_rows = rows;
     if (rows > max_rows) return GF_ERR_BUFFER_TOO_SMALL;
     for (size_t y = 0; y < rows; ++y) frame_row(C, y, out_matrices + y * GF_MATRIX_STRIDE);       // rayon par_iter in the reference (:249)
@@ -421,19 +403,13 @@ GF_API int gf_cuda_frame_transform_dev_flagged(gf_cuda_gyro* g, const gf_compute
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     RowCtx C;
     // the two per-frame lookups (org(ts), smoothed(ts)) stay on the host: O(log n) each; the per-row ones run on the device
-    const Track org{cp->org.ts_us, cp->org.quats, cp->org.n}, sm{cp->smoothed.ts_us, cp->smoothed.quats, cp->smoothed.n};
-    StabPoints sp; memset(&sp, 0, sizeof(sp));
-    const bool has_stab = cp->camera_stab && frame < cp->n_camera_stab && frame < g->stab_index.size();
-    if (has_stab) {
-        const gf_cuda_gyro::StabIndex& ix = g->stab_index[frame];
-        sp.ibis = Spline3{ g->d_stab + ix.ibis_pos, g->d_stab + ix.ibis_val, ix.n_ibis };
-        sp.ois  = Spline3{ g->d_stab + ix.ois_pos,  g->d_stab + ix.ois_val,  ix.n_ois };
-    }
-    const size_t rows = prepare(cp, timestamp_ms, frame, org, sm, host_offsets_of(cp), has_stab ? &sp : nullptr, C, out_params, out_fov, out_minimal_fov);
+    StabSplines sp;
+    const bool has_stab = g->frame_splines(frame, sp);
+    const size_t rows = prepare(cp, timestamp_ms, frame, has_stab ? &sp : nullptr, C, out_params, out_fov, out_minimal_fov);
     if (out_rows) *out_rows = rows;
     if (rows > max_rows) return GF_ERR_BUFFER_TOO_SMALL;
-    C.org = Track{g->d_org_ts, g->d_org_q, g->n_org};
-    C.offsets = SyncOffsets{ g->d_off_ts, g->d_off_ms, g->n_offsets, cp->gyro_offset_ms };
+    C.org = g->org_track();
+    C.offsets = g->sync_offsets(cp->gyro_offset_ms);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     unsigned* scratch = g->d_scratch + 2u * (g->next_scratch++ % gf_cuda_gyro::kScratchPairs);     // self-cleaning: the last block re-arms it
     frame_rows_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(C, rows, matrices_dev, table_flags_dev, scratch);

@@ -4,6 +4,7 @@
 #include <cstdint>
 #include <cstddef>
 #include <vector>
+#include "frame_geometry.cuh"
 
 struct gf_cuda_gyro {
     int device = 0;
@@ -20,4 +21,23 @@ struct gf_cuda_gyro {
     static constexpr unsigned kScratchPairs = 64;
     unsigned* d_scratch = nullptr; unsigned next_scratch = 0;
     cudaStream_t stream = nullptr;
+
+    gf::Track org_track() const { return gf::Track{ d_org_ts, d_org_q, n_org }; }
+    // the uploaded multi-point sync offsets; `scalar_ms` (gyro_offset_ms) applies when there are none
+    gf::SyncOffsets sync_offsets(double scalar_ms) const { return gf::SyncOffsets{ d_off_ts, d_off_ms, n_offsets, scalar_ms }; }
+    // this frame's IBIS / OIS spline points; false when the upload had no camera_stab entry for it
+    bool frame_splines(size_t frame, gf::StabSplines& s) const {
+        if (frame >= stab_index.size()) return false;
+        const StabIndex& ix = stab_index[frame];
+        s.ibis = gf::Spline3{ d_stab + ix.ibis_pos, d_stab + ix.ibis_val, ix.n_ibis };
+        s.ois  = gf::Spline3{ d_stab + ix.ois_pos,  d_stab + ix.ois_val,  ix.n_ois };
+        return true;
+    }
+    // this frame's distorting mesh (mesh_correction[frame].0) and its length, or nullptr when it has none of more than 9 values
+    const double* frame_mesh(size_t frame, uint32_t& len) const {
+        len = 0;
+        if (!d_mesh || frame >= mesh_index.size() || mesh_index[frame].len <= 9) return nullptr;
+        len = (uint32_t)mesh_index[frame].len;
+        return d_mesh + mesh_index[frame].off;
+    }
 };

@@ -1,6 +1,6 @@
 // quat_track.cuh — quaternion tracks (TimeQuat = BTreeMap<i64 us, UnitQuaternion<f64>>, src/core/gyro_source/mod.rs:34) as sorted
 // arrays, and the lookups the per-frame producers need.  Shared by frame_transform.cu (FrameTransform::at_timestamp) and
-// zoom_kernel.cu (at_timestamp_for_points); host and device compile the same functions.
+// zoom_kernel.cu (at_timestamp_for_points) through frame_geometry.cuh; host and device compile the same functions.
 //
 //   qslerp             nalgebra 0.34.2 UnitQuaternion::slerp (shortest arc; `a` when the quaternions coincide)
 //   sync_offset_at     GyroSource::offset_at_timestamp         gyro_source/mod.rs:884-909

@@ -16,27 +16,19 @@
 #include <vector>
 #include "lens_models.cuh"
 #include "warp_kernel.cuh"      // MeshView + mesh_bivariate (the f64 bivariate spline, splines.rs:141-176)
-#include "quat_track.cuh"
+#include "frame_geometry.cuh"
 #include "gyro_dev.h"
+#include "c_abi_internal.h"
 
 using namespace gf;
 
 namespace {
 
-// quaternion tracks, slerp and the sync-offset lookup are shared with frame_transform.cu (quat_track.cuh)
-typedef Quat ZQuat;
-typedef Track ZTrack;
-__host__ __device__ inline ZQuat zq_mul(const ZQuat& a, const ZQuat& b) { return qmul(a, b); }
-
-struct ZoomStab {               // camera_stab_data[frame] as at_timestamp_for_points uses it (frame_transform.rs:412-431); spline points in HBM
-    int present;
-    double offset, crop_y, crop_h, scale_x, scale_y, height;
-    Spline3 ibis, ois;
-};
 struct ZoomFrame {              // per-frame uniforms (host, f64)
-    ZQuat q0;                   // smoothed(ts) * org(ts)^-1
-    double start_ts;
-    ZoomStab stab;
+    Quat q0;                    // smoothed(ts) * org(ts)^-1
+    double start_ts, row_readout_time;
+    int rs_on;                  // rolling-shutter correction: frame readout time != 0
+    CameraStab stab;            // spline points in HBM; absent when at_timestamp_for_points has no shifts (:412, :432-434)
     const double* mesh; uint32_t mesh_len;      // this frame's distorting mesh in HBM (mesh_correction[frame].0), or nullptr
     // keyframed values of this frame (fov_iterative.rs:44-46, frame_transform.rs:354, cpu_undistort.rs:661); `keyed` = some track exists
     int keyed;
@@ -46,11 +38,11 @@ struct ZoomFrame {              // per-frame uniforms (host, f64)
 };
 struct ZoomArgs {
     gf_kernel_params kp;        // as built by undistort_points (:671-683)
-    ZTrack org;                 // device-resident track
+    Track org;                  // device-resident track
     double duration_ms;
     SyncOffsets offsets;        // device-resident multi-point sync offsets (or the scalar)
-    double new_k[9], rot_c, rot_s, row_readout_time;
-    int rs_on, horizontal, suppress_rotation, lens_noop;
+    double new_k[9], rot_c, rot_s;
+    int horizontal, suppress_rotation, lens_noop;
     float fx, fy, cx, cy;
     float hstretch, vstretch;   // 0 = do not apply (:702-703)
     float in_w, in_h, out_w, inv_aspect, margin;
@@ -59,37 +51,37 @@ struct ZoomArgs {
     int lc; float amount, factor, out_cx, out_cy, out_fx, out_fy, fov;
 };
 
-// K_new * R for one point — frame_transform.rs:391-410 (f64), narrowed to f32 like cpu_undistort.rs:764
+// K_new * R for one point — frame_transform.rs:391-410 (f64, no inverted-framebuffer flips), narrowed to f32 like cpu_undistort.rs:764
 __device__ void point_rotation(const ZoomArgs& A, const ZoomFrame& F, float px, float py, float (&rot)[9]) {
-    const double quat_time = A.rs_on ? F.start_ts + A.row_readout_time * (double)(A.horizontal ? px : py) : F.start_ts;
-    const ZQuat q = zq_mul(F.q0, quat_at_timestamp(A.org, A.duration_ms, A.offsets, quat_time));
-    const double ww = q.w*q.w, ii = q.i*q.i, jj = q.j*q.j, kk = q.k*q.k;
-    const double ij = q.i*q.j*2.0, wk = q.w*q.k*2.0, wj = q.w*q.j*2.0, ik = q.i*q.k*2.0, jk = q.j*q.k*2.0, wi = q.w*q.i*2.0;
-    const double rq[9] = { ww+ii-jj-kk, ij-wk, wj+ik, wk+ij, ww-ii+jj-kk, jk-wi, ik-wj, wi+jk, ww-ii-jj+kk };
-    const double rz[9] = { A.rot_c, -A.rot_s, 0.0, A.rot_s, A.rot_c, 0.0, 0.0, 0.0, 1.0 };
-    double r[9], m[9];
-    for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) r[a*3+b] = rz[a*3]*rq[b] + rz[a*3+1]*rq[3+b] + rz[a*3+2]*rq[6+b];
-    r[1] *= -1.0; r[2] *= -1.0; r[3] *= -1.0; r[6] *= -1.0;
-    if (A.suppress_rotation) { for (int t = 0; t < 9; ++t) r[t] = (t % 4 == 0) ? 1.0 : 0.0; }
-    for (int a = 0; a < 3; ++a) for (int b = 0; b < 3; ++b) m[a*3+b] = A.new_k[a*3]*r[b] + A.new_k[a*3+1]*r[3+b] + A.new_k[a*3+2]*r[6+b];
+    const double quat_time = F.rs_on ? F.start_ts + F.row_readout_time * (double)(A.horizontal ? px : py) : F.start_ts;
+    const Quat q = qmul(F.q0, quat_at_timestamp(A.org, A.duration_ms, A.offsets, quat_time));
+    double m[9];
+    frame_rotation(q, A.rot_c, A.rot_s, A.new_k, false, A.suppress_rotation, m);
     for (int t = 0; t < 9; ++t) rot[t] = (float)m[t];
 }
 
 // The IBIS / OIS shift of point `index` — frame_transform.rs:412-431.  points_iter is the point list when rolling-shutter correction is
 // on and the single point (0, 0) otherwise, so with correction off only index 0 has an entry (cpu_undistort.rs:748 `v.get(index)`).
-__device__ bool point_shift(const ZoomArgs& A, const ZoomFrame& F, float py, size_t index, float (&sh)[5]) {
-    const ZoomStab& S = F.stab;
-    if (!S.present) return false;
-    if (!A.rs_on && index != 0) return false;
-    const double yy = A.rs_on ? (double)py : 0.0;
-    const double y = (yy - 0.0) * ((S.crop_y + S.crop_h) - S.crop_y) / (S.height - 0.0) + S.crop_y;       // map_coord (util.rs:144-147), f64
-    double s[3], o[3];
-    if (!catmull_rom3(S.ibis, y + S.offset, s)) { s[0] = 0.0; s[1] = 0.0; s[2] = 0.0; }                  // .unwrap_or_default()
-    if (!catmull_rom3(S.ois,  y + S.offset, o)) { o[0] = 0.0; o[1] = 0.0; o[2] = 0.0; }
-    const double ra = s[2] / 1000.0;
-    sh[0] = (float)(s[0] * S.scale_x); sh[1] = (float)(s[1] * S.scale_y); sh[2] = (float)(ra * (M_PI / 180.0));
-    sh[3] = (float)(o[0] * S.scale_x); sh[4] = (float)(o[1] * S.scale_y);
+__device__ bool point_shift(const ZoomFrame& F, float py, size_t index, float (&sh)[5]) {
+    if (!F.stab.present) return false;
+    if (!F.rs_on && index != 0) return false;
+    double s[5];
+    stab_shift(F.stab, F.rs_on ? (double)py : 0.0, false, s);
+    for (int t = 0; t < 5; ++t) sh[t] = (float)s[t];
     return true;
+}
+
+// light refraction — cpu_undistort.rs:767-776, :805-814
+__device__ __forceinline__ void refract(float lrc, float& x, float& y) {
+    if (lrc != 1.0f && lrc > 0.0f) {
+        const float r = sqrtf(x * x + y * y);
+        if (r != 0.0f) {
+            const float sin_theta_d = (r / sqrtf(1.0f + r * r)) / lrc;
+            const float r_d = sin_theta_d / sqrtf(1.0f - sin_theta_d * sin_theta_d);
+            const float s = r_d / r;
+            x = x * s; y = y * s;
+        }
+    }
 }
 
 // map_coord (util.rs:144-147) in f32, IEEE division
@@ -147,16 +139,7 @@ __device__ void lc_r_of(const ZoomArgs& A, float ox, float oy, float& rx, float&
     }
     float nx = (qx - A.out_cx) / A.out_fx, ny = (qy - A.out_cy) / A.out_fy;
     { float dx, dy; if (Lens<LENS>::undistort(nx, ny, P, A.lens_noop != 0, dx, dy)) { nx = dx; ny = dy; } }
-    const float lrc = P.light_refraction_coefficient;
-    if (lrc != 1.0f && lrc > 0.0f) {
-        const float r = sqrtf(nx * nx + ny * ny);
-        if (r != 0.0f) {
-            const float sin_theta_d = (r / sqrtf(1.0f + r * r)) / lrc;
-            const float r_d = sin_theta_d / sqrtf(1.0f - sin_theta_d * sin_theta_d);
-            const float s = r_d / r;
-            nx = nx * s; ny = ny * s;
-        }
-    }
+    refract(P.light_refraction_coefficient, nx, ny);
     rx = (nx * A.out_fx) + A.out_cx; ry = (ny * A.out_fy) + A.out_cy;
 }
 
@@ -172,7 +155,7 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     if (DIGITAL != GF_LENS_NONE) { float tx, ty; if (Lens<DIGITAL>::undistort(x, y, P, false, tx, ty)) { x = tx; y = ty; } }
     if (F.mesh && F.mesh_len > 9) point_mesh(A, F, x, y);          // cpu_undistort.rs:712-746
     float sh[5];
-    if (point_shift(A, F, py, index, sh)) {             // cpu_undistort.rs:748-757 (sic: y is rotated with the already rotated x)
+    if (point_shift(F, py, index, sh)) {             // cpu_undistort.rs:748-757 (sic: y is rotated with the already rotated x)
         const float cos_a = gf_cosf(sh[2]), sin_a = gf_sinf(sh[2]);
         x = x - A.cx - sh[3] + sh[0];
         y = y - A.cy - sh[4] + sh[1];
@@ -182,16 +165,7 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     const float pwx = (x - A.cx) / A.fx, pwy = (y - A.cy) / A.fy;
     float ptx, pty;
     if (!Lens<LENS>::undistort(pwx, pwy, P, A.lens_noop != 0, ptx, pty)) { outx = -1000000.0f; outy = -1000000.0f; return; }
-    const float lrc = P.light_refraction_coefficient;
-    if (lrc != 1.0f && lrc > 0.0f) {
-        const float r = sqrtf(ptx * ptx + pty * pty);
-        if (r != 0.0f) {
-            const float sin_theta_d = (r / sqrtf(1.0f + r * r)) / lrc;
-            const float r_d = sin_theta_d / sqrtf(1.0f - sin_theta_d * sin_theta_d);
-            const float f2 = r_d / r;
-            ptx *= f2; pty *= f2;
-        }
-    }
+    refract(P.light_refraction_coefficient, ptx, pty);
     const float pr0 = rot[0] * ptx + rot[1] * pty + rot[2] * 1.0f;
     const float pr1 = rot[3] * ptx + rot[4] * pty + rot[5] * 1.0f;
     const float pr2 = rot[6] * ptx + rot[7] * pty + rot[8] * 1.0f;
@@ -230,20 +204,7 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     outx = ptx; outy = pty;
 }
 
-// points_around_rect(w, h, 31, 31) — fov_iterative.rs:154-175, point k
-__device__ void rect_point(const ZoomArgs& A, int k, float& x, float& y) {
-    float w = A.in_w, h = A.in_h;
-    w -= A.margin * 2.0f; h -= A.margin * 2.0f;
-    const int wcnt = 30, hcnt = 30;
-    const float wstep = w / (float)wcnt, hstep = h / (float)hcnt;
-    if (k < wcnt)                    { x = (float)k * wstep;                          y = 0.0f; }
-    else if (k < wcnt + hcnt)        { x = w;                                         y = (float)(k - wcnt) * hstep; }
-    else if (k < 2 * wcnt + hcnt)    { x = (float)(wcnt - (k - wcnt - hcnt)) * wstep; y = h; }
-    else                             { x = 0.0f;                                      y = (float)(hcnt - (k - 2 * wcnt - hcnt)) * hstep; }
-    x += A.margin; y += A.margin;
-}
-
-constexpr int ZOOM_RECT_LEN = 120;
+constexpr int ZOOM_RECT_LEN = RECT_POINTS;
 constexpr int ZOOM_INTERP_LEN = 63;       // (30 + 1) * 3 - 30
 
 template <int LENS, int DIGITAL>
@@ -265,7 +226,7 @@ __global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ Z
     const ZoomArgs& A = F.keyed ? SA : A0;
     const float cx = A.in_w / 2.0f, cy = A.in_h / 2.0f;
     if (tid < ZOOM_RECT_LEN) {
-        float x, y; rect_point(A, tid, x, y);
+        float x, y; rect_point(A.in_w, A.in_h, A.margin, tid, x, y);
         rect[2 * tid] = x; rect[2 * tid + 1] = y;
         float ux, uy; undistort_point_rs<LENS, DIGITAL>(A, F, x, y, (size_t)tid, ux, uy);
         poly[2 * tid] = ux - A.zc_x; poly[2 * tid + 1] = uy - A.zc_y;
@@ -317,33 +278,6 @@ __global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ Z
     if (tid == 0) out[blockIdx.x] = (double)(sw * 2.0f / A.out_w);      // :133
 }
 
-typedef void (*ZoomFn)(const ZoomArgs, const ZoomFrame*, double*);
-template <int LENS> ZoomFn pick_digital(int digital) {
-    switch (digital) {
-    case GF_LENS_NONE:             return find_fov_kernel<LENS, GF_LENS_NONE>;
-    case GF_LENS_DIGITAL_STRETCH:  return find_fov_kernel<LENS, GF_LENS_DIGITAL_STRETCH>;
-    case GF_LENS_GOPRO_SUPERVIEW:  return LENS == GF_LENS_OPENCV_FISHEYE ? find_fov_kernel<LENS, GF_LENS_GOPRO_SUPERVIEW> : nullptr;
-    case GF_LENS_GOPRO6_SUPERVIEW: return LENS == GF_LENS_OPENCV_FISHEYE ? find_fov_kernel<LENS, GF_LENS_GOPRO6_SUPERVIEW> : nullptr;
-    case GF_LENS_GOPRO_HYPERVIEW:  return LENS == GF_LENS_OPENCV_FISHEYE ? find_fov_kernel<LENS, GF_LENS_GOPRO_HYPERVIEW> : nullptr;
-    case GF_LENS_GOPRO_WARP:       return LENS == GF_LENS_GOPRO ? find_fov_kernel<LENS, GF_LENS_GOPRO_WARP> : nullptr;
-    default: return nullptr;
-    }
-}
-ZoomFn pick_zoom(int lens, int digital) {
-    switch (lens) {
-    case GF_LENS_OPENCV_FISHEYE:     return pick_digital<GF_LENS_OPENCV_FISHEYE>(digital);
-    case GF_LENS_OPENCV_STANDARD:    return pick_digital<GF_LENS_OPENCV_STANDARD>(digital);
-    case GF_LENS_POLY3:              return pick_digital<GF_LENS_POLY3>(digital);
-    case GF_LENS_POLY5:              return pick_digital<GF_LENS_POLY5>(digital);
-    case GF_LENS_PTLENS:             return pick_digital<GF_LENS_PTLENS>(digital);
-    case GF_LENS_INSTA360:           return pick_digital<GF_LENS_INSTA360>(digital);
-    case GF_LENS_SONY:               return pick_digital<GF_LENS_SONY>(digital);
-    case GF_LENS_GENERIC_POLYNOMIAL: return pick_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
-    case GF_LENS_GOPRO:              return pick_digital<GF_LENS_GOPRO>(digital);
-    default: return nullptr;
-    }
-}
-
 // undistort_points over an explicit point list (pts != nullptr: out = n x (x, y)) or over every pixel centre of a w x h grid
 // (pts == nullptr: out = w*h x RGB, the ST-map encoding of stmap.rs:131-135: x / w, 1 - y / h, 0).
 template <int LENS, int DIGITAL>
@@ -358,76 +292,60 @@ __global__ void __launch_bounds__(128) points_kernel(const ZoomArgs A, const Zoo
     if (pts) { out[2 * i] = ox; out[2 * i + 1] = oy; }
     else     { out[3 * i] = ox / (float)grid_w; out[3 * i + 1] = 1.0f - (oy / (float)grid_h); out[3 * i + 2] = 0.0f; }
 }
-typedef void (*PointsFn)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
-template <int LENS> PointsFn pick_points_digital(int digital) {
+// Both kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye
+// model, GoPro warp the GoPro model).
+struct ZoomKernels {
+    void (*find_fov)(const ZoomArgs, const ZoomFrame*, double*);
+    void (*points)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
+};
+template <int LENS, int DIGITAL> ZoomKernels kernels_of() { return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL> }; }
+template <int LENS> ZoomKernels pick_digital(int digital) {
     switch (digital) {
-    case GF_LENS_NONE:             return points_kernel<LENS, GF_LENS_NONE>;
-    case GF_LENS_DIGITAL_STRETCH:  return points_kernel<LENS, GF_LENS_DIGITAL_STRETCH>;
-    case GF_LENS_GOPRO_SUPERVIEW:  return LENS == GF_LENS_OPENCV_FISHEYE ? points_kernel<LENS, GF_LENS_GOPRO_SUPERVIEW> : nullptr;
-    case GF_LENS_GOPRO6_SUPERVIEW: return LENS == GF_LENS_OPENCV_FISHEYE ? points_kernel<LENS, GF_LENS_GOPRO6_SUPERVIEW> : nullptr;
-    case GF_LENS_GOPRO_HYPERVIEW:  return LENS == GF_LENS_OPENCV_FISHEYE ? points_kernel<LENS, GF_LENS_GOPRO_HYPERVIEW> : nullptr;
-    case GF_LENS_GOPRO_WARP:       return LENS == GF_LENS_GOPRO ? points_kernel<LENS, GF_LENS_GOPRO_WARP> : nullptr;
-    default: return nullptr;
+    case GF_LENS_NONE:             return kernels_of<LENS, GF_LENS_NONE>();
+    case GF_LENS_DIGITAL_STRETCH:  return kernels_of<LENS, GF_LENS_DIGITAL_STRETCH>();
+    case GF_LENS_GOPRO_SUPERVIEW:  if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_SUPERVIEW>();  break;
+    case GF_LENS_GOPRO6_SUPERVIEW: if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO6_SUPERVIEW>(); break;
+    case GF_LENS_GOPRO_HYPERVIEW:  if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_HYPERVIEW>();  break;
+    case GF_LENS_GOPRO_WARP:       if (LENS == GF_LENS_GOPRO) return kernels_of<LENS, GF_LENS_GOPRO_WARP>();                break;
+    default: break;
     }
+    return { nullptr, nullptr };
 }
-PointsFn pick_points(int lens, int digital) {
+ZoomKernels pick_kernels(int lens, int digital) {
     switch (lens) {
-    case GF_LENS_OPENCV_FISHEYE:     return pick_points_digital<GF_LENS_OPENCV_FISHEYE>(digital);
-    case GF_LENS_OPENCV_STANDARD:    return pick_points_digital<GF_LENS_OPENCV_STANDARD>(digital);
-    case GF_LENS_POLY3:              return pick_points_digital<GF_LENS_POLY3>(digital);
-    case GF_LENS_POLY5:              return pick_points_digital<GF_LENS_POLY5>(digital);
-    case GF_LENS_PTLENS:             return pick_points_digital<GF_LENS_PTLENS>(digital);
-    case GF_LENS_INSTA360:           return pick_points_digital<GF_LENS_INSTA360>(digital);
-    case GF_LENS_SONY:               return pick_points_digital<GF_LENS_SONY>(digital);
-    case GF_LENS_GENERIC_POLYNOMIAL: return pick_points_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
-    case GF_LENS_GOPRO:              return pick_points_digital<GF_LENS_GOPRO>(digital);
-    default: return nullptr;
-    }
-}
-
-bool zoom_lens_noop(int lens, const float* k) {
-    switch (lens) {
-    case GF_LENS_OPENCV_FISHEYE: case GF_LENS_SONY: return k[0] == 0.0f && k[1] == 0.0f && k[2] == 0.0f && k[3] == 0.0f;
-    case GF_LENS_GENERIC_POLYNOMIAL: { for (int i = 0; i < 12; ++i) if (!(k[i] == 0.0f)) return false; return true; }
-    case GF_LENS_GOPRO: return k[1] == 0.0f;
-    default: return false;
+    case GF_LENS_OPENCV_FISHEYE:     return pick_digital<GF_LENS_OPENCV_FISHEYE>(digital);
+    case GF_LENS_OPENCV_STANDARD:    return pick_digital<GF_LENS_OPENCV_STANDARD>(digital);
+    case GF_LENS_POLY3:              return pick_digital<GF_LENS_POLY3>(digital);
+    case GF_LENS_POLY5:              return pick_digital<GF_LENS_POLY5>(digital);
+    case GF_LENS_PTLENS:             return pick_digital<GF_LENS_PTLENS>(digital);
+    case GF_LENS_INSTA360:           return pick_digital<GF_LENS_INSTA360>(digital);
+    case GF_LENS_SONY:               return pick_digital<GF_LENS_SONY>(digital);
+    case GF_LENS_GENERIC_POLYNOMIAL: return pick_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
+    case GF_LENS_GOPRO:              return pick_digital<GF_LENS_GOPRO>(digital);
+    default: return { nullptr, nullptr };
     }
 }
 
 } // namespace
 
-// FrameTransform::get_fov — frame_transform.rs:52-58 (callers pass a ComputeParams whose fov_scale is already the Fov keyframe value)
-static double gf_points_fov(const gf_compute_params* cp, size_t frame, int use_fovs) {
-    double fov_scale = cp->fov_scale;
-    if (cp->fov_overview && use_fovs) fov_scale += 1.0;
-    double fov = 1.0;
-    if (use_fovs) {
-        double f = 1.0;
-        if (cp->fovs && frame < cp->n_fovs) f = cp->fovs[frame]; else if (cp->fovs && cp->n_fovs > 1) f = cp->fovs[cp->n_fovs - 1];
-        fov = f * fov_scale;
-    }
-    fov = fmax(fov, 0.001);
-    return fov * (double)cp->width / (double)(cp->output_width > 1 ? cp->output_width : 1);
+// at_timestamp_for_points' fov without focal-length compensation (frame_transform.rs:360-362): get_fov, scaled by the output size as
+// (fov * width) / output_width
+static double points_fov(const gf_compute_params* cp, size_t frame, bool use_fovs, double timestamp_ms) {
+    return fov_unscaled(cp, frame, use_fovs, timestamp_ms, false) * (double)cp->width / (double)(cp->output_width > 1 ? cp->output_width : 1);
 }
 
 // Everything undistort_points (cpu_undistort.rs:652-698) and at_timestamp_for_points (frame_transform.rs:352-410) derive from
-// ComputeParams for one call: kernel params, K_new, readout timing.  Returns the signed frame readout time.
-static double setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, double fov, double lens_correction_amount, ZoomArgs& A) {
+// ComputeParams for one call: kernel params, K_new.
+static void setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, double fov, double lens_correction_amount, ZoomArgs& A) {
     memset(&A, 0, sizeof(A));
     const double* K = cp.camera_matrix;
-    const double hr = cp.input_horizontal_stretch > 0.01 ? cp.input_horizontal_stretch : 1.0;
-    memcpy(A.new_k, K, sizeof(A.new_k));
-    A.new_k[0] = A.new_k[0] * (1.0 / hr) / fov; A.new_k[4] = A.new_k[4] * (1.0 / hr) / fov;
-    A.new_k[2] = (double)cp.output_width / 2.0; A.new_k[5] = (double)cp.output_height / 2.0;
-    double frt = fabs(cp.frame_readout_time); if (cp.readout_inverted) frt *= -1.0;        // get_frame_readout_time(can_invert = false)
-    if (cp.readout_time_scale != 0.0) frt *= cp.readout_time_scale;                         // capture_area / sensor height of the closest lens_params entry (:26-29)
-    A.row_readout_time = frt / (double)(cp.readout_horizontal ? cp.width : cp.height);
-    A.rs_on = fabs(frt) > 0.0 ? 1 : 0; A.horizontal = cp.readout_horizontal; A.suppress_rotation = cp.suppress_rotation;
+    get_new_k(&cp, K, fov, A.new_k);
+    A.horizontal = cp.readout_horizontal; A.suppress_rotation = cp.suppress_rotation;
     const double a = cp.video_rotation * (M_PI / 180.0);
     A.rot_c = cos(a); A.rot_s = sin(a);
-    A.org = ZTrack{ g->d_org_ts, g->d_org_q, g->n_org };
+    A.org = g->org_track();
     A.duration_ms = cp.duration_ms;
-    A.offsets = SyncOffsets{ g->d_off_ts, g->d_off_ms, g->n_offsets, cp.gyro_offset_ms };
+    A.offsets = g->sync_offsets(cp.gyro_offset_ms);
     gf_kernel_params& kp = A.kp;                                                            // cpu_undistort.rs:671-683
     kp.width = cp.width; kp.height = cp.height; kp.output_width = cp.output_width; kp.output_height = cp.output_height;
     A.fx = (float)K[0]; A.fy = (float)K[4]; A.cx = (float)K[2]; A.cy = (float)K[5];
@@ -435,7 +353,7 @@ static double setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& 
     for (int i = 0; i < 12; ++i) kp.k[i] = (float)cp.distortion_coeffs[i];
     for (int i = 0; i < 16 && i < cp.n_digital_lens_params; ++i) kp.digital_lens_params[i] = (float)cp.digital_lens_params[i];
     kp.light_refraction_coefficient = (float)cp.light_refraction_coefficient;
-    A.lens_noop = zoom_lens_noop(distortion_model, kp.k) ? 1 : 0;
+    A.lens_noop = lens_noop(distortion_model, kp.k) ? 1 : 0;
     A.hstretch = cp.input_horizontal_stretch > 0.001 ? (float)cp.input_horizontal_stretch : 0.0f;
     A.vstretch = cp.input_vertical_stretch   > 0.001 ? (float)cp.input_vertical_stretch   : 0.0f;
     A.lc = lens_correction_amount < 1.0 ? 1 : 0;
@@ -444,40 +362,19 @@ static double setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& 
         A.amount = (float)lens_correction_amount; A.factor = fmaxf(1.0f - A.amount, 0.001f);
         A.out_fx = A.fx / (float)fov / A.factor; A.out_fy = A.fy / (float)fov / A.factor; A.fov = (float)fov;
     }
-    return frt;
 }
-// smoothed(ts) * org(ts)^-1 and the readout start time of one frame — frame_transform.rs:376-388
-static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& cp, double ts, double frt, size_t frame) {
-    if (cp.per_frame_time_offsets && frame < cp.n_per_frame_time_offsets) ts += cp.per_frame_time_offsets[frame];     // frame_transform.rs:384
-    const ZTrack horg{ cp.org.ts_us, cp.org.quats, cp.org.n }, hsm{ cp.smoothed.ts_us, cp.smoothed.quats, cp.smoothed.n };
+// readout timing, smoothed(ts) * org(ts)^-1, shifts and distorting mesh of one frame — frame_transform.rs:366-388,412-434
+static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& cp, double ts, size_t frame) {
     ZoomFrame f;
-    const SyncOffsets ho{ cp.sync_offset_ts_us, cp.sync_offset_ms, (cp.sync_offset_ts_us && cp.sync_offset_ms) ? cp.n_sync_offsets : 0, cp.gyro_offset_ms };
-    const ZQuat q1 = qinv(quat_at_timestamp(horg, cp.duration_ms, ho, ts));
-    f.q0 = zq_mul(quat_at_timestamp(hsm, cp.duration_ms, ho, ts), q1);
-    f.start_ts = ts - frt / 2.0;
+    const FrameTiming t = frame_timing(&cp, frame, ts, false);
+    f.q0 = t.q0; f.start_ts = t.start_ts; f.row_readout_time = t.row_readout_time;
+    f.rs_on = fabs(t.frame_readout_time) > 0.0 ? 1 : 0;
     f.keyed = 0;
-    memset(&f.stab, 0, sizeof(f.stab));
-    f.mesh = nullptr; f.mesh_len = 0;
-    if (g->d_mesh && frame < g->mesh_index.size() && g->mesh_index[frame].len > 9) {                 // mesh_correction.get(frame) (:369-373)
-        f.mesh = g->d_mesh + g->mesh_index[frame].off; f.mesh_len = (uint32_t)g->mesh_index[frame].len;
-    }
-    if (cp.camera_stab && frame < cp.n_camera_stab && frame < g->stab_index.size() && !(cp.suppress_rotation && cp.frame_readout_time == 0.0)) {   // :412, :432-434
-        const gf_camera_stab& is = cp.camera_stab[frame];
-        const gf_cuda_gyro::StabIndex& ix = g->stab_index[frame];
-        f.stab.present = 1;
-        f.stab.offset = is.offset; f.stab.crop_y = (double)is.crop_area[1]; f.stab.crop_h = (double)is.crop_area[3]; f.stab.height = (double)cp.height;
-        f.stab.scale_x = (double)cp.width  / (double)is.crop_area[2] / (double)is.pixel_pitch[0];
-        f.stab.scale_y = (double)cp.height / (double)is.crop_area[3] / (double)is.pixel_pitch[1];
-        f.stab.ibis = Spline3{ g->d_stab + ix.ibis_pos, g->d_stab + ix.ibis_val, ix.n_ibis };
-        f.stab.ois  = Spline3{ g->d_stab + ix.ois_pos,  g->d_stab + ix.ois_val,  ix.n_ois };
-    }
+    f.mesh = g->frame_mesh(frame, f.mesh_len);
+    StabSplines sp;
+    const bool shifts = !(cp.suppress_rotation && cp.frame_readout_time == 0.0) && g->frame_splines(frame, sp);       // :432-434
+    f.stab = camera_stab_at(&cp, frame, false, shifts ? &sp : nullptr);
     return f;
-}
-// KeyframeManager::value_at_video_timestamp(...).unwrap_or(default) for one of the tracks in gf_compute_params
-static double zoom_keyframed(const gf_compute_params& cp, int typ, double ts, double dflt) {
-    double v = dflt;
-    (void)gf_keyframe_value_at(&cp.keyframes[typ], ts, cp.keyframe_timestamp_scale, &v);
-    return v;
 }
 // at_timestamp_for_points / undistort_points for ONE timestamp: the tracks they read become the constants of a private copy
 static gf_compute_params resolve_point_keyframes(const gf_compute_params& cp, double ts, size_t frame) {
@@ -487,9 +384,8 @@ static gf_compute_params resolve_point_keyframes(const gf_compute_params& cp, do
         memcpy(r.camera_matrix, L.camera_matrix, sizeof(r.camera_matrix)); memcpy(r.distortion_coeffs, L.distortion_coeffs, sizeof(r.distortion_coeffs));
         r.radial_distortion_limit = L.radial_distortion_limit;
     }
-    r.video_rotation = zoom_keyframed(cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation);                                  // frame_transform.rs:354
-    r.light_refraction_coefficient = zoom_keyframed(cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);   // cpu_undistort.rs:661
-    r.fov_scale = zoom_keyframed(cp, GF_KF_FOV, ts, cp.fov_scale);                                                       // get_fov :53
+    r.video_rotation = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation);                                  // frame_transform.rs:354
+    r.light_refraction_coefficient = keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);   // cpu_undistort.rs:661
     return r;
 }
 static bool zoom_any_keyframes(const gf_compute_params& cp) {
@@ -502,15 +398,15 @@ static bool zoom_any_keyframes(const gf_compute_params& cp) {
 // `lens_correction_default` = what the caller would have used without a track).
 static void fill_keyed(ZoomFrame& f, const gf_compute_params& cp, const ZoomArgs& A, double ts, double fov, double lens_correction_default, bool zoom_center) {
     f.keyed = 1;
-    const double a = zoom_keyframed(cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation) * (M_PI / 180.0);
+    const double a = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation) * (M_PI / 180.0);
     f.rot_c = cos(a); f.rot_s = sin(a);
-    f.lrc = (float)zoom_keyframed(cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);
+    f.lrc = (float)keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);
     f.zc_x = A.zc_x; f.zc_y = A.zc_y;
     if (zoom_center) {
-        f.zc_x = (float)zoom_keyframed(cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * A.in_w;
-        f.zc_y = (float)zoom_keyframed(cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * A.in_h;
+        f.zc_x = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * A.in_w;
+        f.zc_y = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * A.in_h;
     }
-    const double lca = zoom_center ? zoom_keyframed(cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, lens_correction_default) : lens_correction_default;
+    const double lca = zoom_center ? keyframed(&cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, lens_correction_default) : lens_correction_default;
     f.lc = lca < 1.0 ? 1 : 0;
     f.amount = (float)lca; f.factor = fmaxf(1.0f - f.amount, 0.001f);
     f.out_fx = A.fx / (float)fov / f.factor; f.out_fy = A.fy / (float)fov / f.factor;
@@ -527,17 +423,16 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
                              const double* timestamps_ms, size_t n, float fov_algorithm_margin, double* out_fov_minimal, void* cu_stream) {
     if (!g || !cp_user || !timestamps_ms || !out_fov_minimal) return GF_ERR_BAD_PARAMS;
     if (n == 0) return GF_OK;
-    ZoomFn fn = pick_zoom(distortion_model, digital_lens);
-    if (!fn) return GF_ERR_UNSUPPORTED_COMBO;
+    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
+    if (!k.find_fov) return GF_ERR_UNSUPPORTED_COMBO;
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     gf_compute_params cp = *cp_user;
     const int org_ow = cp.output_width, org_oh = cp.output_height;
     cp.fov_scale = 1.0; cp.n_fovs = 0; cp.n_minimal_fovs = 0; cp.output_width = cp.width; cp.output_height = cp.height;
 
     ZoomArgs A;
-    // at_timestamp_for_points with use_fovs = false: fov = max(1, 0.001) * width / output_width (= 1 after the adjustments)
-    const double fov = fmax(1.0, 0.001) * (double)cp.width / (double)(cp.output_width > 1 ? cp.output_width : 1);
-    const double frt = setup_points_args(g, cp, distortion_model, fov, cp.lens_correction_amount, A);
+    const double fov = points_fov(&cp, 0, false, 0.0);            // use_fovs = false: 1 after the adjustments
+    setup_points_args(g, cp, distortion_model, fov, cp.lens_correction_amount, A);
     const float ratio = (float)cp.width / (float)(org_ow > 1 ? org_ow : 1);                // FovIterative::new :78-89
     A.in_w = (float)cp.width; A.in_h = (float)cp.height;
     A.out_w = (float)org_ow * ratio; const float out_h = (float)org_oh * ratio;
@@ -550,7 +445,7 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
         A.out_cx = (float)cp.output_width / 2.0f; A.out_cy = (float)cp.output_height / 2.0f; A.fov = (float)fov;
     }
     for (size_t i = 0; i < n; ++i) {
-        hf[i] = frame_uniforms(g, cp, timestamps_ms[i], frt, i);
+        hf[i] = frame_uniforms(g, cp, timestamps_ms[i], i);
         if (keyed) fill_keyed(hf[i], cp, A, timestamps_ms[i], fov, cp.lens_correction_amount, true);
     }
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
@@ -560,7 +455,7 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
         if (d_frames) cudaFree(d_frames); (void)cudaGetLastError(); return GF_ERR_CUDA;
     }
     e = cudaMemcpyAsync(d_frames, hf.data(), n * sizeof(ZoomFrame), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) { fn<<<(unsigned)n, 128, 0, st>>>(A, d_frames, d_out); e = cudaGetLastError(); }
+    if (e == cudaSuccess) { k.find_fov<<<(unsigned)n, 128, 0, st>>>(A, d_frames, d_out); e = cudaGetLastError(); }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_fov_minimal, d_out, n * sizeof(double), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     cudaFree(d_frames); cudaFree(d_out);
@@ -574,15 +469,15 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
                                     const float* points_xy, size_t n, float* out_xy, void* cu_stream) {
     if (!g || !cp_user || !points_xy || !out_xy) return GF_ERR_BAD_PARAMS;
     if (n == 0) return GF_OK;
-    PointsFn fn = pick_points(distortion_model, digital_lens);
-    if (!fn) return GF_ERR_UNSUPPORTED_COMBO;
+    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
+    if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     ZoomArgs A;
-    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // video rotation, refraction, Fov at this timestamp
+    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // lens, video rotation and refraction at this timestamp
     const gf_compute_params* cp = &rcp;
-    const double fov = gf_points_fov(cp, frame, use_fovs);
-    const double frt = setup_points_args(g, *cp, distortion_model, fov, lens_correction_amount, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frt, frame);
+    const double fov = points_fov(cp, frame, use_fovs != 0, timestamp_ms);
+    setup_points_args(g, *cp, distortion_model, fov, lens_correction_amount, A);
+    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frame);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     float2* d_in = nullptr; float* d_out = nullptr;
     cudaError_t e;
@@ -590,7 +485,7 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
         if (d_in) cudaFree(d_in); (void)cudaGetLastError(); return GF_ERR_CUDA;
     }
     e = cudaMemcpyAsync(d_in, points_xy, n * sizeof(float2), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) { fn<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, d_in, n, 0, 0, d_out); e = cudaGetLastError(); }
+    if (e == cudaSuccess) { k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, d_in, n, 0, 0, d_out); e = cudaGetLastError(); }
     if (e == cudaSuccess) e = cudaMemcpyAsync(out_xy, d_out, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     cudaFree(d_in); cudaFree(d_out);
@@ -603,19 +498,19 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
 GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
                                      double timestamp_ms, size_t frame, float* out_rgb_dev, void* cu_stream) {
     if (!g || !cp_user || !out_rgb_dev) return GF_ERR_BAD_PARAMS;
-    PointsFn fn = pick_points(distortion_model, digital_lens);
-    if (!fn) return GF_ERR_UNSUPPORTED_COMBO;
-    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // video rotation, refraction, Fov at this timestamp
+    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
+    if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
+    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // lens, video rotation and refraction at this timestamp
     const gf_compute_params* cp = &rcp;
     if (cp->width < 1 || cp->height < 1) return GF_ERR_BAD_PARAMS;
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     ZoomArgs A;
-    const double fov = gf_points_fov(cp, frame, 1);
-    const double frt = setup_points_args(g, *cp, distortion_model, fov, 1.0, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frt, frame);
+    const double fov = points_fov(cp, frame, true, timestamp_ms);
+    setup_points_args(g, *cp, distortion_model, fov, 1.0, A);
+    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frame);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     const size_t n = (size_t)cp->width * (size_t)cp->height;
-    fn<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);
+    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);
     if (cudaGetLastError() != cudaSuccess) return GF_ERR_CUDA;
     return GF_OK;
 }
