@@ -131,6 +131,16 @@ class StabConfig(C.Structure):
     ]
 
 
+class ZoomParams(C.Structure):
+    """gf_zoom_params: the ComputeParams fields zooming::calculate_fovs reads besides find_fov's inputs (compute_params.rs:33-53)."""
+    _fields_ = [
+        ("adaptive_zoom_window", C.c_double), ("adaptive_zoom_method", C.c_int32), ("video_speed_affects_zooming", C.c_int32),
+        ("scaled_fps", C.c_double), ("video_speed", C.c_double),
+        ("zooming_speed", KeyframeTrack), ("video_speed_track", KeyframeTrack), ("keyframe_timestamp_scale", C.c_double),
+        ("trim_ranges", C.POINTER(C.c_double)), ("n_trim_ranges", C.c_size_t), ("fov_algorithm_margin", C.c_float),
+    ]
+
+
 class QueueConfig(C.Structure):
     _fields_ = [
         ("device", C.c_int32), ("distortion_model", C.c_int32), ("digital_lens", C.c_int32), ("depth", C.c_int32),
@@ -207,6 +217,9 @@ EXPORTS = [
                                               _P(C.c_size_t), _P(C.c_double), _P(C.c_double), C.c_void_p]),
     ("gf_cuda_find_fovs", C.c_int, [C.c_void_p, _P(ComputeParams), C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_float, C.c_void_p, C.c_void_p]),
     ("gf_zoom_dynamic_compute", C.c_int, [C.c_void_p, C.c_size_t, C.c_double, C.c_double, C.c_int, C.c_void_p]),
+    ("gf_zoom_fovs", C.c_int, [_P(ZoomParams), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("gf_cuda_calculate_fovs", C.c_int, [C.c_void_p, _P(ComputeParams), _P(ZoomParams), C.c_int, C.c_int, C.c_void_p, C.c_size_t,
+                                         C.c_void_p, C.c_void_p, C.c_void_p]),
     ("gf_cuda_scan_tables_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("gf_cuda_undistort_image_dev_flagged", C.c_int, [C.c_void_p, _P(BufferDesc), _P(BufferDesc), _P(KernelParams),
                                                       C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),

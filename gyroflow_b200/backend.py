@@ -222,13 +222,23 @@ class CudaWrapper:
 # ------------------------------------------------------------------------------------------ per-frame transform producer
 
 
+def _fill_keyframe_track(t: abi.KeyframeTrack, keys, keep: list):
+    """Flatten [(timestamp_us, value, easing name)] (any order; easing defaults to EaseInOut) into `t`; the arrays go into `keep`."""
+    keys = sorted(keys)
+    ts = np.asarray([k[0] for k in keys], dtype=np.int64); val = np.asarray([k[1] for k in keys], dtype=np.float64)
+    ea = np.asarray([abi.EASING[k[2]] if len(k) > 2 else abi.EASING["EaseInOut"] for k in keys], dtype=np.uint8)
+    keep += [ts, val, ea]
+    t.ts_us = ts.ctypes.data_as(C.POINTER(C.c_int64)); t.value = val.ctypes.data_as(C.POINTER(C.c_double))
+    t.easing = ea.ctypes.data_as(C.POINTER(C.c_uint8)); t.n = len(keys)
+
+
 class ComputeParams:
     """Owns a gf_compute_params plus the numpy arrays it points to (quaternion tracks, fovs)."""
 
     def __init__(self, kernel_params: abi.KernelParams, org, smoothed, frame_readout_time_ms=16.0, fovs=None, video_rotation=0.0,
                  horizontal=False, inverted=False, framebuffer_inverted=False, fov_scale=1.0, sync_offsets=None,
                  per_frame_time_offsets=None, focal_lengths=None, smoothed_focal_lengths=None, readout_time_scale=0.0, camera_stab=None,
-                 gyro_offset_ms=0.0, keyframes=None, keyframe_timestamp_scale=0.0, lens_per_frame=None, distorting_meshes=None):
+                 gyro_offset_ms=0.0, keyframes=None, keyframe_timestamp_scale=0.0, lens_per_frame=None, distorting_meshes=None, minimal_fovs=None):
         """sync_offsets: {timestamp_us: offset_ms} (GyroSource::offsets_adjusted); camera_stab: list (one per frame) of dicts with
         offset, sensor_size, crop_area, pixel_pitch, ibis=(pos[n], xyz[n,3]), ois=(pos[n], xyz[n,3]) (CameraStabData);
         keyframes: {KeyframeType name: [(timestamp_us, value, easing name), ...]} for the types at_timestamp reads (abi.KEYFRAME_TYPES)."""
@@ -244,6 +254,9 @@ class ComputeParams:
         self._fovs = np.ascontiguousarray(fovs if fovs is not None else [], dtype=np.float64)
         if self._fovs.size:
             c.fovs = self._fovs.ctypes.data_as(C.POINTER(C.c_double)); c.n_fovs = self._fovs.size
+        self._minimal_fovs = np.ascontiguousarray(minimal_fovs if minimal_fovs is not None else [], dtype=np.float64)
+        if self._minimal_fovs.size:
+            c.minimal_fovs = self._minimal_fovs.ctypes.data_as(C.POINTER(C.c_double)); c.n_minimal_fovs = self._minimal_fovs.size
         c.frame_readout_time = frame_readout_time_ms
         c.readout_horizontal, c.readout_inverted = int(horizontal), int(inverted)
         c.framebuffer_inverted = int(framebuffer_inverted)
@@ -286,13 +299,7 @@ class ComputeParams:
             c.lens_per_frame = C.cast(arr, C.c_void_p); c.n_lens_per_frame = len(lens_per_frame)
         self._kf_arrays = []
         for name, keys in (keyframes or {}).items():
-            keys = sorted(keys)
-            ts = np.asarray([k[0] for k in keys], dtype=np.int64); val = np.asarray([k[1] for k in keys], dtype=np.float64)
-            ea = np.asarray([abi.EASING[k[2]] if len(k) > 2 else abi.EASING["EaseInOut"] for k in keys], dtype=np.uint8)
-            self._kf_arrays += [ts, val, ea]
-            t = c.keyframes[abi.KEYFRAME_TYPES[name]]
-            t.ts_us = ts.ctypes.data_as(C.POINTER(C.c_int64)); t.value = val.ctypes.data_as(C.POINTER(C.c_double))
-            t.easing = ea.ctypes.data_as(C.POINTER(C.c_uint8)); t.n = len(keys)
+            _fill_keyframe_track(c.keyframes[abi.KEYFRAME_TYPES[name]], keys, self._kf_arrays)
         if distorting_meshes:     # one f64 mesh (or None) per frame: file_metadata.mesh_correction[frame].0
             arr = (abi.MeshF64 * len(distorting_meshes))()
             self._dmesh_arrays = []
@@ -336,6 +343,41 @@ class ComputeParams:
         return kp, m[: rows.value].copy(), fov.value, mfov.value
 
 
+class ZoomParams:
+    """Owns a gf_zoom_params plus the arrays it points to: the settings zooming::calculate_fovs reads besides find_fov's inputs.
+    method: 0 gaussian filter, 1 envelope follower; zooming_speed / video_speed_keys: [(timestamp_us, value, easing name)] tracks of
+    KeyframeType::ZoomingSpeed / VideoSpeed (empty = not keyframed); trim_ranges: [(start, end)] fractions of the clip."""
+
+    def __init__(self, adaptive_zoom_window, method=0, scaled_fps=30.0, video_speed=1.0, video_speed_affects_zooming=False,
+                 zooming_speed=(), video_speed_keys=(), keyframe_timestamp_scale=0.0, trim_ranges=(), fov_algorithm_margin=2.0):
+        z = abi.ZoomParams()
+        z.adaptive_zoom_window, z.adaptive_zoom_method, z.scaled_fps = adaptive_zoom_window, method, scaled_fps
+        z.video_speed, z.video_speed_affects_zooming = video_speed, int(video_speed_affects_zooming)
+        self._kf_arrays = []
+        if zooming_speed:
+            _fill_keyframe_track(z.zooming_speed, zooming_speed, self._kf_arrays)
+        if video_speed_keys:
+            _fill_keyframe_track(z.video_speed_track, video_speed_keys, self._kf_arrays)
+        z.keyframe_timestamp_scale = keyframe_timestamp_scale
+        self._trim = np.ascontiguousarray(np.asarray(trim_ranges, dtype=np.float64).reshape(-1, 2))
+        if self._trim.size:
+            z.trim_ranges = self._trim.ctypes.data_as(C.POINTER(C.c_double)); z.n_trim_ranges = self._trim.shape[0]
+        z.fov_algorithm_margin = fov_algorithm_margin
+        self.c = z
+
+
+def zoom_fovs(zp: ZoomParams, timestamps_ms, fov_values):
+    """calculate_fovs from the per-frame find_fov values on (trim ranges, zoom mode, zoom_dynamic) — host.  Returns (fovs, minimal_fovs)."""
+    ts = np.ascontiguousarray(timestamps_ms, dtype=np.float64)
+    v = np.ascontiguousarray(fov_values, dtype=np.float64)
+    assert ts.size == v.size
+    fovs, minimal = np.zeros_like(v), np.zeros_like(v)
+    rc = abi.load_library().gf_zoom_fovs(C.byref(zp.c), ts.ctypes.data, v.ctypes.data, v.size, fovs.ctypes.data, minimal.ctypes.data)
+    if rc != 0:
+        raise GyroflowCoreError(rc, "gf_zoom_fovs")
+    return fovs, minimal
+
+
 class DeviceGyro:
     """Quaternion tracks resident in HBM + the per-frame matrix kernel (gf_cuda_frame_transform_dev)."""
 
@@ -368,6 +410,17 @@ class DeviceGyro:
         if rc != 0:
             raise GyroflowCoreError(rc, "gf_cuda_find_fovs")
         return out
+
+    def calculate_fovs(self, distortion_model: str, digital_lens, zp: ZoomParams, timestamps_ms, stream=0):
+        """zooming::calculate_fovs (zooming/mod.rs:35-70): find_fovs on the device, then zoom_fovs.  Returns (fovs, minimal_fovs), the
+        arrays a render takes as ComputeParams(fovs=..., minimal_fovs=...)."""
+        ts = np.ascontiguousarray(timestamps_ms, dtype=np.float64)
+        fovs, minimal = np.zeros(ts.size, np.float64), np.zeros(ts.size, np.float64)
+        rc = self._lib.gf_cuda_calculate_fovs(self._h, C.byref(self.cp.c), C.byref(zp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
+                                              ts.ctypes.data, ts.size, fovs.ctypes.data, minimal.ctypes.data, stream or None)
+        if rc != 0:
+            raise GyroflowCoreError(rc, "gf_cuda_calculate_fovs")
+        return fovs, minimal
 
     def undistort_points(self, distortion_model: str, digital_lens, points_xy, timestamp_ms, frame=0, use_fovs=False, lens_correction_amount=1.0):
         """undistort_points_with_rolling_shutter (cpu_undistort.rs:636-641) on the device; points_xy: (n, 2) float32."""

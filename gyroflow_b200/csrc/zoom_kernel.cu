@@ -3,8 +3,8 @@
 // Behavioural source: FovIterative::find_fov / nearest_edge / points_around_rect / interpolate_points
 // (src/core/zooming/fov_iterative.rs:91-189), undistort_points_with_rolling_shutter + undistort_points
 // (src/core/stabilization/cpu_undistort.rs:636-858, with the IBIS / OIS shifts and the distorting mesh), FrameTransform::at_timestamp_for_points
-// (src/core/stabilization/frame_transform.rs:352-438), calculate_fovs (src/core/zooming/mod.rs:35-70) and the
-// static-window temporal filters of zoom_dynamic.rs:56-126,177-200.
+// (src/core/stabilization/frame_transform.rs:352-438), calculate_fovs (src/core/zooming/mod.rs:35-70) with the trim ranges of
+// fov_iterative.rs:59-69, and the temporal filters of zoom_dynamic.rs:15-189 (static and keyframed window).
 //
 // One CTA per frame: 120 edge points (then <= 4 rounds of 63 interpolated points) are pushed through the inverse lens
 // model with their own rolling-shutter rotation in parallel; the order-dependent nearest_edge fold runs on one thread.
@@ -412,6 +412,52 @@ static void fill_keyed(ZoomFrame& f, const gf_compute_params& cp, const ZoomArgs
     f.out_fx = A.fx / (float)fov / f.factor; f.out_fy = A.fy / (float)fov / f.factor;
 }
 
+// ---- the temporal filters of zoom_dynamic.rs, on the host like in the reference ----
+
+// Rust's `f64 as usize`: truncates, saturates, NaN -> 0
+static size_t as_usize(double x) {
+    if (!(x > 0.0)) return 0;
+    return x >= 18446744073709551616.0 ? SIZE_MAX : (size_t)x;
+}
+// KeyframeManager::is_keyframed for a flattened track (the custom provider is baked into the track by the caller)
+static bool track_keyed(const gf_keyframe_track& t) { return t.n > 0 && t.ts_us && t.value; }
+
+// envelope_follower (zoom_dynamic.rs:165-189): alphas[i] belongs to sample i in both passes
+static std::vector<double> envelope_follower(const std::vector<double>& a, const std::vector<double>& alphas) {
+    const size_t m = a.size(); std::vector<double> rev(m), res(m);
+    double q = a[m - 1];
+    for (size_t r = 0; r < m; ++r) { const size_t i = m - 1 - r; const double x = a[i], al = alphas[i]; q = fmin(x, x * al + q * (1.0 - al)); rev[r] = q; }
+    q = rev[m - 1];
+    for (size_t r = 0; r < m; ++r) { const double x = rev[m - 1 - r], al = alphas[r]; q = fmin(x, x * al + q * (1.0 - al)); res[r] = q; }
+    return res;
+}
+
+// Windows longer than this many frames are rejected instead of allocated (the reference would panic on the allocation).
+constexpr double kMaxWindowFrames = 1e8;
+
+// zoom_dynamic::compute's static-window branch (zoom_dynamic.rs:56-76) in place on v (non-empty).  False when the window is too long.
+static bool zoom_static_window(std::vector<double>& v, double window_s, double fps, int method) {
+    const size_t n = v.size();
+    if (method == 1) {
+        v = envelope_follower(v, std::vector<double>(n, 1.0 - exp(-(1.0 / fps) / window_s)));
+        v = envelope_follower(v, std::vector<double>(n, 1.0 - exp(-(1.0 / fps) / 0.2)));
+        return true;
+    }
+    const double frames_f = floor(window_s * fps);                  // get_frames_per_window :82-88
+    if (frames_f >= kMaxWindowFrames) return false;
+    size_t frames = as_usize(frames_f); if (frames % 2 == 0) frames += 1;
+    const size_t half = frames / 2;
+    auto pad = [&](const std::vector<double>& a) { std::vector<double> p(a.size() + 2 * half); for (size_t i = 0; i < p.size(); ++i) p[i] = i < half ? a.front() : (i >= half + a.size() ? a.back() : a[i - half]); return p; };
+    std::vector<double> p = pad(v), mn(n);
+    for (size_t i = 0; i < n; ++i) { double m = p[i]; for (size_t j = 1; j < frames; ++j) m = fmin(m, p[i + j]); mn[i] = m; }
+    p = pad(mn);
+    std::vector<double> gw(frames); const double sd = (double)frames / 6.0, sig2 = 2.0 * sd * sd; double sum = 0.0;
+    for (size_t i = 0; i < frames; ++i) { const long x = (long)i - (long)half; gw[i] = exp(-(double)(x * x) / sig2); sum += gw[i]; }
+    for (auto& w : gw) w /= sum;
+    for (size_t i = 0; i < n; ++i) { double s = 0.0; for (size_t j = 0; j < frames; ++j) s += p[i + j] * gw[j]; v[i] = s; }
+    return true;
+}
+
 
 extern "C" {
 
@@ -519,32 +565,75 @@ GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* c
 GF_API int gf_zoom_dynamic_compute(const double* fov_minimal, size_t n, double window_s, double fps, int method, double* out) {
     if (!fov_minimal || !out) return GF_ERR_BAD_PARAMS;
     if (n == 0) return GF_OK;
-    auto envelope = [](const std::vector<double>& a, double alpha) {                         // :177-200
-        const size_t m = a.size(); std::vector<double> rev(m), res(m);
-        double q = a[m - 1];
-        for (size_t r = 0; r < m; ++r) { const double x = a[m - 1 - r]; q = fmin(x, x * alpha + q * (1.0 - alpha)); rev[r] = q; }
-        q = rev[m - 1];
-        for (size_t r = 0; r < m; ++r) { const double x = rev[m - 1 - r]; q = fmin(x, x * alpha + q * (1.0 - alpha)); res[r] = q; }
-        return res;
-    };
     std::vector<double> v(fov_minimal, fov_minimal + n);
-    if (method == 1) {
-        v = envelope(v, 1.0 - exp(-(1.0 / fps) / window_s));
-        v = envelope(v, 1.0 - exp(-(1.0 / fps) / 0.2));
-    } else {
-        size_t frames = (size_t)floor(window_s * fps); if (frames % 2 == 0) frames += 1;     // :78-84
-        const size_t half = frames / 2;
-        auto pad = [&](const std::vector<double>& a) { std::vector<double> p(a.size() + 2 * half); for (size_t i = 0; i < p.size(); ++i) p[i] = i < half ? a.front() : (i >= half + a.size() ? a.back() : a[i - half]); return p; };
-        std::vector<double> p = pad(v), mn(n);
-        for (size_t i = 0; i < n; ++i) { double m = p[i]; for (size_t j = 1; j < frames; ++j) m = fmin(m, p[i + j]); mn[i] = m; }
-        p = pad(mn);
-        std::vector<double> gw(frames); const double sd = (double)frames / 6.0, sig2 = 2.0 * sd * sd; double sum = 0.0;
-        for (size_t i = 0; i < frames; ++i) { const long x = (long)i - (long)half; gw[i] = exp(-(double)(x * x) / sig2); sum += gw[i]; }
-        for (auto& w : gw) w /= sum;
-        for (size_t i = 0; i < n; ++i) { double s = 0.0; for (size_t j = 0; j < frames; ++j) s += p[i + j] * gw[j]; v[i] = s; }
-    }
+    if (!zoom_static_window(v, window_s, fps, method)) return GF_ERR_BAD_PARAMS;
     memcpy(out, v.data(), n * sizeof(double));
     return GF_OK;
+}
+
+GF_API int gf_zoom_fovs(const gf_zoom_params* zp, const double* timestamps_ms, const double* fov_values, size_t n,
+                        double* out_fovs, double* out_minimal_fovs) {
+    if (!zp) return GF_ERR_BAD_PARAMS;
+    if (n == 0) return GF_OK;                                        // calculate_fovs returns empty vectors (zooming/mod.rs:36-38)
+    if (!timestamps_ms || !fov_values || !out_fovs || !out_minimal_fovs || (zp->n_trim_ranges && !zp->trim_ranges)) return GF_ERR_BAD_PARAMS;
+    std::vector<double> v(fov_values, fov_values + n);
+    // Trim ranges (fov_iterative.rs:59-69) come before the mode branch, so the minimal FOVs of a trimmed clip carry the max-FOV fill.
+    if (zp->n_trim_ranges > 0) {
+        double max_fov = v[0];
+        for (size_t i = 1; i < n; ++i) max_fov = fmax(max_fov, v[i]);                      // reduce(f64::max)
+        const double l = (double)(n - 1);
+        for (size_t i = 0; i < n; ++i) {
+            bool within = false;
+            for (size_t r = 0; r < zp->n_trim_ranges && !within; ++r)
+                within = i >= as_usize(floor(l * zp->trim_ranges[2 * r])) && i <= as_usize(ceil(l * zp->trim_ranges[2 * r + 1]));
+            if (!within) v[i] = max_fov;
+        }
+    }
+    const std::vector<double> minimal = v;
+    const double window = zp->adaptive_zoom_window, fps = zp->scaled_fps;
+    const bool speed_keyed = track_keyed(zp->video_speed_track);
+    if (window < -0.9) {                                             // static zoom (zooming/mod.rs:55-61)
+        double m = v[0];
+        for (size_t i = 1; i < n; ++i) m = fmin(m, v[i]);                                  // reduce(f64::min)
+        v.assign(n, m);
+    } else if (!(window > 0.0001)) {                                 // zoom disabled (:65-67)
+        v.assign(n, 1.0);
+    } else if (track_keyed(zp->zooming_speed) || (zp->video_speed_affects_zooming && (zp->video_speed != 1.0 || speed_keyed))) {   // zoom_dynamic.rs:22
+        if (zp->adaptive_zoom_method == 1) {
+            // The first envelope pass uses each frame's window (:26-30, :171-173); the second always 0.2 s (:51).
+            std::vector<double> alphas(n);
+            for (size_t i = 0; i < n; ++i) {
+                double w = window, speed = zp->video_speed;
+                (void)gf_keyframe_value_at(&zp->zooming_speed, timestamps_ms[i], zp->keyframe_timestamp_scale, &w);
+                if (zp->video_speed_affects_zooming) {
+                    (void)gf_keyframe_value_at(&zp->video_speed_track, timestamps_ms[i], zp->keyframe_timestamp_scale, &speed);
+                    w *= fabs(speed);
+                }
+                alphas[i] = 1.0 - exp(-(1.0 / fps) / w);
+            }
+            v = envelope_follower(v, alphas);
+            v = envelope_follower(v, std::vector<double>(n, 1.0 - exp(-(1.0 / fps) / 0.2)));
+        } else {
+            // get_frames_per_window reads the global adaptive_zoom_window, not the frame's window (zoom_dynamic.rs:31): every frame has the
+            // static window, so min_rolling_dynamic / convolve_dynamic (:129-163) are the static min_rolling / convolve.
+            if (!zoom_static_window(v, window, fps, 0)) return GF_ERR_BAD_PARAMS;
+        }
+    } else if (!zoom_static_window(v, window, fps, zp->adaptive_zoom_method)) {                    // static window (zoom_dynamic.rs:56-76)
+        return GF_ERR_BAD_PARAMS;
+    }
+    memcpy(out_fovs, v.data(), n * sizeof(double));
+    memcpy(out_minimal_fovs, minimal.data(), n * sizeof(double));
+    return GF_OK;
+}
+
+GF_API int gf_cuda_calculate_fovs(gf_cuda_gyro* g, const gf_compute_params* cp, const gf_zoom_params* zp, int distortion_model, int digital_lens,
+                                  const double* timestamps_ms, size_t n, double* out_fovs, double* out_minimal_fovs, void* cu_stream) {
+    if (!g || !cp || !zp || !timestamps_ms || !out_fovs || !out_minimal_fovs) return GF_ERR_BAD_PARAMS;
+    if (n == 0) return GF_OK;
+    std::vector<double> fov_values(n);
+    const int rc = gf_cuda_find_fovs(g, cp, distortion_model, digital_lens, timestamps_ms, n, zp->fov_algorithm_margin, fov_values.data(), cu_stream);
+    if (rc != GF_OK) return rc;
+    return gf_zoom_fovs(zp, timestamps_ms, fov_values.data(), n, out_fovs, out_minimal_fovs);
 }
 
 } // extern "C"

@@ -203,7 +203,8 @@ GF_API int         gf_cuda_device_name(int device, char* buf, size_t buf_len);  
 GF_API int         gf_cuda_supports(const gf_buffer_desc* in, const gf_buffer_desc* out); /* is_buffer_supported opencl.rs:451 */
 GF_API const char* gf_cuda_version(void);
 /* sizeof() of the structs that cross this ABI, for binding generators and their tests: 0 gf_kernel_params, 1 gf_buffer_desc,
- * 2 gf_compute_params, 3 gf_camera_stab, 4 gf_keyframe_track, 5 gf_stab_config, 6 gf_queue_config, 7 gf_lens_data, 8 gf_mesh_f64; 0 for any other index. */
+ * 2 gf_compute_params, 3 gf_camera_stab, 4 gf_keyframe_track, 5 gf_stab_config, 6 gf_queue_config, 7 gf_lens_data, 8 gf_mesh_f64,
+ * 9 gf_zoom_params; 0 for any other index. */
 GF_API size_t gf_abi_struct_size(int which);
 
 /* ---- lens plugin surface: DistortionModel::from_name / id  distortion_models/mod.rs:79-90 -- */
@@ -473,6 +474,36 @@ GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp, 
                                   void* cu_stream);
 
 GF_API int gf_zoom_dynamic_compute(const double* fov_minimal, size_t n, double window_s, double fps, int method, double* out);
+
+/* ------------------------------------------------------------------------------------------
+ * zooming::calculate_fovs (src/core/zooming/mod.rs:35-70) — what the reference runs before a render (lib.rs:515-523).
+ * gf_zoom_params holds the ComputeParams fields it reads besides find_fov's inputs (compute_params.rs:33-53).
+ * gf_zoom_fovs takes the per-frame find_fov values and applies, in the reference's order:
+ *   1. trim ranges (fov_iterative.rs:59-69): frame i (its position in the timestamp list, l = n - 1) outside every
+ *      [floor(l * start), ceil(l * end)] gets the clip's largest FOV;
+ *   2. the zoom mode (zooming/mod.rs:55-68): adaptive_zoom_window < -0.9 static zoom (every frame gets the clip's minimum),
+ *      > 0.0001 dynamic zoom (zoom_dynamic::compute, zoom_dynamic.rs:15-80), otherwise disabled (fovs all 1.0);
+ *   3. dynamic zoom takes its keyframed-window branch (zoom_dynamic.rs:22-55) when ZoomingSpeed is keyframed, or
+ *      video_speed_affects_zooming is set and video_speed != 1 or VideoSpeed is keyframed.
+ * out_minimal_fovs are the values after step 1.  Host only, no CUDA call; n == 0 writes nothing. */
+typedef struct gf_zoom_params {
+    double  adaptive_zoom_window;              /* seconds; see the mode thresholds above */
+    int32_t adaptive_zoom_method;              /* 0 gaussian filter, 1 envelope follower (other values: gaussian, like ZoomMethod::from) */
+    int32_t video_speed_affects_zooming;
+    double  scaled_fps;
+    double  video_speed;                       /* used where video_speed_track has no key */
+    gf_keyframe_track zooming_speed;           /* KeyframeType::ZoomingSpeed, seconds; n == 0: not keyframed */
+    gf_keyframe_track video_speed_track;       /* KeyframeType::VideoSpeed; n == 0: not keyframed */
+    double  keyframe_timestamp_scale;          /* KeyframeManager::timestamp_scale; 0 = None (1.0) */
+    const double* trim_ranges; size_t n_trim_ranges;   /* n x (start, end) as fractions of the clip; n == 0: no trim */
+    float   fov_algorithm_margin;              /* pixels (2.0 in the reference) */
+} gf_zoom_params;
+GF_API int gf_zoom_fovs(const gf_zoom_params* zp, const double* timestamps_ms, const double* fov_values, size_t n,
+                        double* out_fovs, double* out_minimal_fovs);
+/* gf_cuda_find_fovs over n frames (frame index = position, as in recompute_adaptive_zoom_static, lib.rs:515-523; margin =
+ * zp->fov_algorithm_margin), then gf_zoom_fovs.  One kernel launch; synchronous. */
+GF_API int gf_cuda_calculate_fovs(gf_cuda_gyro* g, const gf_compute_params* cp, const gf_zoom_params* zp, int distortion_model, int digital_lens,
+                                  const double* timestamps_ms, size_t n, double* out_fovs, double* out_minimal_fovs, void* cu_stream);
 
 /* ------------------------------------------------------------------------------------------
  * Stabilization::get_frame_transform_at<T> — src/core/stabilization/mod.rs:253-326 (with get_kernel_flags :226-251 and
