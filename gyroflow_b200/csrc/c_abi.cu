@@ -173,40 +173,12 @@ int validate(gf_cuda_ctx* ctx, const gf_kernel_params* p, const gf_buffer_desc* 
     return GF_OK;
 }
 
-// map_coord's per-frame-uniform pieces (util.rs:144-147), same float operations as the reference evaluates per pixel.
-// max_abs_int_coord < 0: no identity shortcut (the map is not applied to integer-valued coordinates only).
-__host__ __device__ MapC make_map(float in_min, float in_max, float out_min, float out_max, float max_abs_int_coord) {
-    MapC m;
-    m.in_min = in_min;
-    m.mul = out_max - out_min;
-    m.div = in_max - in_min;
-    m.rcp = 1.0f / m.div;
-    m.add = out_min;
-    const float ad = fabsf(m.div);
-    m.fast_div = (isfinite(m.div) && ad >= 0x1p-40f && ad <= 0x1p40f) ? 1 : 0;
-    // integer-valued x: (x - in_min) and (x - in_min) * mul are exact below 2^24, and exact / div == (x - in_min) when mul == div
-    m.identity = (max_abs_int_coord >= 0.0f && m.mul == m.div && m.mul > 0.0f && in_min == truncf(in_min) &&
-                  (max_abs_int_coord + fabsf(in_min)) * m.mul < 16777216.0f) ? 1 : 0;
-    return m;
-}
-
 // f32 mesh -> f64 once per frame (cpu_undistort.rs:539) + the per-frame constants of MeshAux, all on the device so that
 // device-resident meshes never touch the host.  o has room for GF_MESH_MAX_LEN doubles followed by one MeshAux.
 __global__ void widen_mesh_kernel(const float* __restrict__ m, double* __restrict__ o, int n, float width_f, float height_f) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) o[i] = (double)m[i];
-    if (i == 0 && n >= 9) {
-        MeshAux* aux = reinterpret_cast<MeshAux*>(o + GF_MESH_MAX_LEN);
-        const double size_y = (double)m[4];
-        const double h = size_y / 8.0;
-        aux->h = h; aux->inv_h = 1.0 / h; aux->three_inv_h = 3.0 * aux->inv_h; aux->h_over_3 = h / 3.0; aux->inv_3h = 1.0 / (3.0 * h);
-        // `mesh[5] as f32` etc.: the f64 value is the widened f32, so the narrowing is the identity
-        const float origin_x = m[5], origin_y = m[6], crop_w = m[7], crop_h = m[8];
-        aux->to_crop_x  = make_map(0.0f, width_f,  origin_x, origin_x + crop_w, -1.0f);
-        aux->to_crop_y  = make_map(0.0f, height_f, origin_y, origin_y + crop_h, -1.0f);
-        aux->to_frame_x = make_map(origin_x, origin_x + crop_w, 0.0f, width_f, -1.0f);
-        aux->to_frame_y = make_map(origin_y, origin_y + crop_h, 0.0f, height_f, -1.0f);
-    }
+    if (i == 0 && n >= 9) make_mesh_aux(m, width_f, height_f, *reinterpret_cast<MeshAux*>(o + GF_MESH_MAX_LEN));
 }
 // one block: every thread ORs its rows, the block reduces, thread 0 WRITES the verdict (no prior memset, no atomics on the word)
 __global__ void __launch_bounds__(1024) scan_tables_kernel(const float* __restrict__ m, size_t rows, uint32_t* flags) {

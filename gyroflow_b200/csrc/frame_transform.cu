@@ -364,8 +364,10 @@ GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_
         g->mesh_index.resize(cp->n_distorting_mesh);
         for (size_t f = 0; f < cp->n_distorting_mesh; ++f) {
             const gf_mesh_f64& m = cp->distorting_mesh[f];
-            g->mesh_index[f].off = flat.size(); g->mesh_index[f].len = m.data ? m.len : 0;
+            gf_cuda_gyro::MeshIndex& ix = g->mesh_index[f];
+            ix.off = flat.size(); ix.len = m.data ? m.len : 0;
             if (m.data) flat.insert(flat.end(), m.data, m.data + m.len);
+            if (ix.len >= 9) memcpy(ix.header, m.data, sizeof(ix.header));
         }
         if (!flat.empty())
             ok = cudaMalloc(&g->d_mesh, flat.size() * sizeof(double)) == cudaSuccess &&

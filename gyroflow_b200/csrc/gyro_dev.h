@@ -14,7 +14,7 @@ struct gf_cuda_gyro {
     struct StabIndex { size_t ibis_pos, ibis_val, n_ibis, ois_pos, ois_val, n_ois; };
     std::vector<StabIndex> stab_index;                                              // offsets into d_stab per frame
     double* d_mesh = nullptr;                                                       // distorting meshes of every frame (point path), flat
-    struct MeshIndex { size_t off, len; };
+    struct MeshIndex { size_t off, len; double header[9]; };                       // header: host copy of the mesh's first 9 values
     std::vector<MeshIndex> mesh_index;
     // verdict accumulator + ticket of frame_rows_kernel: a pool of pairs handed out round-robin, so that producer launches that overlap
     // on different streams (the render queue's slots) never share one

@@ -25,6 +25,23 @@ struct MapC {
     int   identity;                     // integer-valued x only: ((x - in_min) * mul) / div == x - in_min exactly (products < 2^24, mul == div)
 };
 
+// map_coord's per-frame-uniform pieces (util.rs:144-147), same float operations as the reference evaluates per pixel.
+// max_abs_int_coord < 0: no identity shortcut (the map is not applied to integer-valued coordinates only).
+__host__ __device__ inline MapC make_map(float in_min, float in_max, float out_min, float out_max, float max_abs_int_coord) {
+    MapC m;
+    m.in_min = in_min;
+    m.mul = out_max - out_min;
+    m.div = in_max - in_min;
+    m.rcp = 1.0f / m.div;
+    m.add = out_min;
+    const float ad = fabsf(m.div);
+    m.fast_div = (isfinite(m.div) && ad >= 0x1p-40f && ad <= 0x1p40f) ? 1 : 0;
+    // integer-valued x: (x - in_min) and (x - in_min) * mul are exact below 2^24, and exact / div == (x - in_min) when mul == div
+    m.identity = (max_abs_int_coord >= 0.0f && m.mul == m.div && m.mul > 0.0f && in_min == truncf(in_min) &&
+                  (max_abs_int_coord + fabsf(in_min)) * m.mul < 16777216.0f) ? 1 : 0;
+    return m;
+}
+
 // feature bits, decided once per launch on the host (all per-frame uniform)
 enum : uint32_t {
     F_RS         = 1u << 0,   // matrix_count > 1
@@ -293,6 +310,17 @@ struct MeshAux {
     double h, inv_h, three_inv_h, h_over_3, inv_3h;      // size_y / 8, 1 / h, 3 * inv_h, h / 3, 1 / (3 h)
     MapC to_crop_x, to_crop_y, to_frame_x, to_frame_y;
 };
+// MeshAux of a mesh (its 9-value header `m`, f32 or f64) on a width_f x height_f frame
+template <class T> __host__ __device__ inline void make_mesh_aux(const T* m, float width_f, float height_f, MeshAux& aux) {
+    const double size_y = (double)m[4];
+    const double h = size_y / 8.0;
+    aux.h = h; aux.inv_h = 1.0 / h; aux.three_inv_h = 3.0 * aux.inv_h; aux.h_over_3 = h / 3.0; aux.inv_3h = 1.0 / (3.0 * h);
+    const float origin_x = (float)m[5], origin_y = (float)m[6], crop_w = (float)m[7], crop_h = (float)m[8];      // `mesh[5] as f32` etc.
+    aux.to_crop_x  = make_map(0.0f, width_f,  origin_x, origin_x + crop_w, -1.0f);
+    aux.to_crop_y  = make_map(0.0f, height_f, origin_y, origin_y + crop_h, -1.0f);
+    aux.to_frame_x = make_map(origin_x, origin_x + crop_w, 0.0f, width_f, -1.0f);
+    aux.to_frame_y = make_map(origin_y, origin_y + crop_h, 0.0f, height_f, -1.0f);
+}
 
 // BivariateSpline::interpolate for both maps (mesh_offset 0 and 1) of a grid with n_y == 9 rows — splines.rs:141-176.
 // Same operations in the same order as the general routine below, restricted to what the result depends on:
@@ -420,6 +448,40 @@ GF_DEV float map_apply(float x, const MapC& m) {
 }
 
 // ------------------------------------------------------------------------------------------
+// The mesh stages, shared by the warp (rotate_and_distort) and the adaptive-zoom point path (zoom_kernel.cu)
+// ------------------------------------------------------------------------------------------
+// The distorting mesh at a point (x, y) in mesh-crop coordinates, both maps (cpu_undistort.rs:169-185 / :735-745): the unrolled 9-row
+// spline where it applies, else the general one.  n_x, n_y, size_x, size_y: mesh[1..4]
+GF_DEV void mesh_spline(const MeshView mesh, const MeshAux& aux, uint32_t n_x, uint32_t n_y, double size_x, double size_y, double x, double y,
+                        double& nx, double& ny) {
+    if (n_y == 9 && n_x >= 2 && n_x <= 9) {
+        mesh_interpolate9(mesh, aux, n_x, size_x, size_y, x, y, nx, ny);
+    } else {
+        nx = mesh_bivariate(mesh, n_x, n_y, size_x, size_y, 0, x, y);
+        ny = mesh_bivariate(mesh, n_x, n_y, size_x, size_y, 1, x, y);
+    }
+}
+
+// Focal-plane distortion of a frame point through the block at mesh[o]: into the mesh crop, the shift of every stabilization band above
+// the point, back to the frame.  The warp subtracts the shift (cpu_undistort.rs:188-214), the point path adds it (:714-733).
+template <bool ADD>
+GF_DEV void focal_plane_shift(const MeshView mesh, const MeshAux& aux, uint32_t o, float& x, float& y) {
+    const double stblz_grid = aux.h;                                                                   // mesh_size_y / 8.0
+    x = map_apply(x, aux.to_crop_x);
+    y = map_apply(y, aux.to_crop_y);
+    const uint32_t idx = as_usize_small(fmin(fmax(floor((double)y / stblz_grid), 0.0), 7.0));        // f64::max / min ignore NaN: NaN -> 0
+    const double delta = (double)y - stblz_grid * (double)idx;
+    const float dx = (float)(mesh[o + 4 + idx * 2 + 0] * delta), dy = (float)(mesh[o + 4 + idx * 2 + 1] * delta);
+    if (ADD) { x += dx; y += dy; } else { x -= dx; y -= dy; }
+    for (uint32_t j = 0; j < idx; ++j) {
+        const float sx = (float)(mesh[o + 4 + j * 2 + 0] * stblz_grid), sy = (float)(mesh[o + 4 + j * 2 + 1] * stblz_grid);
+        if (ADD) { x += sx; y += sy; } else { x -= sx; y -= sy; }
+    }
+    x = map_apply(x, aux.to_frame_x);
+    y = map_apply(y, aux.to_frame_y);
+}
+
+// ------------------------------------------------------------------------------------------
 // rotate_and_distort — cpu_undistort.rs:133-228
 // ------------------------------------------------------------------------------------------
 template <int LENS, int DIGITAL, bool GEN>
@@ -472,12 +534,7 @@ GF_DEV bool rotate_and_distort(float px, float py, uint32_t idx, const WarpArgs&
             const uint32_t n_x = as_usize_small(mesh[1]), n_y = as_usize_small(mesh[2]);
             const double sx = mesh[3], sy = mesh[4];
             double nx, ny;
-            if (n_y == 9 && n_x >= 2 && n_x <= 9) {
-                mesh_interpolate9(mesh, aux, n_x, sx, sy, (double)ux, (double)uy, nx, ny);
-            } else {
-                nx = mesh_bivariate(mesh, n_x, n_y, sx, sy, 0, (double)ux, (double)uy);
-                ny = mesh_bivariate(mesh, n_x, n_y, sx, sy, 1, (double)ux, (double)uy);
-            }
+            mesh_spline(mesh, aux, n_x, n_y, sx, sy, (double)ux, (double)uy, nx, ny);
             ux = map_apply((float)nx, aux.to_frame_x);         // map_coord(nx, origin_x, origin_x + crop_w, 0, width_f)
             uy = map_apply((float)ny, aux.to_frame_y);
             if (inv) uy = A.height_f - uy;
@@ -485,20 +542,8 @@ GF_DEV bool rotate_and_distort(float px, float py, uint32_t idx, const WarpArgs&
         // FocalPlaneDistortion :188-214 (a missing FPD block means "none"; the reference would index out of bounds)
         const uint32_t o = as_usize_small(mesh0);
         if (mesh0 > 0.0 && o < (uint32_t)A.mesh_len && mesh[o] > 0.0) {
-            const double stblz_grid = aux.h;                                                           // mesh_size_y / 8.0
             if (inv) uy = A.height_f - uy;
-            ux = map_apply(ux, aux.to_crop_x);
-            uy = map_apply(uy, aux.to_crop_y);
-            const uint32_t idx2 = as_usize_small(fmin(fmax(floor((double)uy / stblz_grid), 0.0), 7.0));
-            const double delta = (double)uy - stblz_grid * (double)idx2;
-            ux -= (float)(mesh[o + 4 + idx2 * 2 + 0] * delta);
-            uy -= (float)(mesh[o + 4 + idx2 * 2 + 1] * delta);
-            for (uint32_t j = 0; j < idx2; ++j) {
-                ux -= (float)(mesh[o + 4 + j * 2 + 0] * stblz_grid);
-                uy -= (float)(mesh[o + 4 + j * 2 + 1] * stblz_grid);
-            }
-            ux = map_apply(ux, aux.to_frame_x);
-            uy = map_apply(uy, aux.to_frame_y);
+            focal_plane_shift<false>(mesh, aux, o, ux, uy);
             if (inv) uy = A.height_f - uy;
         }
     }
@@ -522,6 +567,39 @@ GF_DEV bool rotate_and_distort(float px, float py, uint32_t idx, const WarpArgs&
 GF_DEV void rotate_point(float px, float py, float ca, float sa, float ox, float oy, float o2x, float o2y, float& rx, float& ry) {
     rx = ca * (px - ox) - sa * (py - oy) + o2x;
     ry = sa * (px - ox) + ca * (py - oy) + o2y;
+}
+
+// The inverse light refraction of a normalised point (cpu_undistort.rs:449-456, :767-776, :805-814), for lrc != 1 && lrc > 0
+GF_DEV void refract_undistort(float& x, float& y, float lrc) {
+    const float r = sqrtf(x * x + y * y);
+    if (r != 0.0f) {
+        const float sin_theta_d = (r / sqrtf(1.0f + r * r)) / lrc;
+        const float r_d = sin_theta_d / sqrtf(1.0f - sin_theta_d * sin_theta_d);
+        const float factor = r_d / r;
+        x *= factor; y *= factor;
+    }
+}
+
+// The lens-correction undistort of an output point, the part before the blend (cpu_undistort.rs:429-457 / :794-815): the digital lens in
+// zoomed coordinates, normalise with the output centre (oc) and focal length (of), lens undistort, inverse refraction, de-normalise.
+// The point path's Newton solve (zoom_kernel.cu) calls it.  undistort_coord below writes the same operations in the same order inline:
+// calling this function (or refract_undistort) from there compiles the general warp kernels to different, if equivalent, machine code.
+// A change to one must be made to the other.
+template <int LENS, int DIGITAL>
+GF_DEV void lens_correction_undistort(float x, float y, const gf_kernel_params& P, float ocx, float ocy, float ofx, float ofy, float fov,
+                                      bool noop, bool digital, bool refract, float lrc, float& rx, float& ry) {
+    if (DIGITAL != GF_LENS_NONE && digital) {
+        const float uzx = (x - ocx) * fov + ocx, uzy = (y - ocy) * fov + ocy;
+        float tx, ty;
+        if (Lens<DIGITAL>::undistort(uzx, uzy, P, false, tx, ty)) {
+            x = (tx - ocx) / fov + ocx;
+            y = (ty - ocy) / fov + ocy;
+        }
+    }
+    x = (x - ocx) / ofx; y = (y - ocy) / ofy;
+    { float tx, ty; if (Lens<LENS>::undistort(x, y, P, noop, tx, ty)) { x = tx; y = ty; } }
+    if (refract) refract_undistort(x, y, lrc);
+    rx = (x * ofx) + ocx; ry = (y * ofy) + ocy;
 }
 
 // undistort_coord — cpu_undistort.rs:421-517.  (opx, opy) = out_pos after the output-rect mapping of :422-423.

@@ -15,7 +15,7 @@
 #include <cstring>
 #include <vector>
 #include "lens_models.cuh"
-#include "warp_kernel.cuh"      // MeshView + mesh_bivariate (the f64 bivariate spline, splines.rs:141-176)
+#include "warp_kernel.cuh"      // the warp's stage functions: lens correction, refraction, mesh
 #include "frame_geometry.cuh"
 #include "gyro_dev.h"
 #include "c_abi_internal.h"
@@ -30,25 +30,23 @@ struct ZoomFrame {              // per-frame uniforms (host, f64)
     int rs_on;                  // rolling-shutter correction: frame readout time != 0
     CameraStab stab;            // spline points in HBM; absent when at_timestamp_for_points has no shifts (:412, :432-434)
     const double* mesh; uint32_t mesh_len;      // this frame's distorting mesh in HBM (mesh_correction[frame].0), or nullptr
-    // keyframed values of this frame (fov_iterative.rs:44-46, frame_transform.rs:354, cpu_undistort.rs:661); `keyed` = some track exists
-    int keyed;
-    double rot_c, rot_s;
-    float zc_x, zc_y, lrc;
-    int lc; float amount, factor, out_fx, out_fy;
+    MeshAux mesh_aux;           // its crop maps and spline steps on the width x height frame
+    // the keyframed values at this frame's timestamp (fov_iterative.rs:44-46, frame_transform.rs:354, cpu_undistort.rs:661)
+    double rot_c, rot_s;        // video rotation
+    float zc_x, zc_y;           // adaptive_zoom_center_offset * input_dim (as f32 products, :100-101)
+    float lrc;                  // light refraction coefficient
+    int lc; float amount, factor, out_fx, out_fy;       // lens-correction blend (:686-694)
 };
-struct ZoomArgs {
+struct ZoomArgs {               // the call-wide values
     gf_kernel_params kp;        // as built by undistort_points (:671-683)
     Track org;                  // device-resident track
     double duration_ms;
     SyncOffsets offsets;        // device-resident multi-point sync offsets (or the scalar)
-    double new_k[9], rot_c, rot_s;
+    double new_k[9];
     int horizontal, suppress_rotation, lens_noop;
-    float fx, fy, cx, cy;
     float hstretch, vstretch;   // 0 = do not apply (:702-703)
     float in_w, in_h, out_w, inv_aspect, margin;
-    float zc_x, zc_y;           // adaptive_zoom_center_offset * input_dim (as f32 products, :100-101)
-    // lens-correction blend (:686-694)
-    int lc; float amount, factor, out_cx, out_cy, out_fx, out_fy, fov;
+    float out_cx, out_cy, fov;  // lens-correction blend (:686-694)
 };
 
 // K_new * R for one point — frame_transform.rs:391-410 (f64, no inverted-framebuffer flips), narrowed to f32 like cpu_undistort.rs:764
@@ -56,7 +54,7 @@ __device__ void point_rotation(const ZoomArgs& A, const ZoomFrame& F, float px, 
     const double quat_time = F.rs_on ? F.start_ts + F.row_readout_time * (double)(A.horizontal ? px : py) : F.start_ts;
     const Quat q = qmul(F.q0, quat_at_timestamp(A.org, A.duration_ms, A.offsets, quat_time));
     double m[9];
-    frame_rotation(q, A.rot_c, A.rot_s, A.new_k, false, A.suppress_rotation, m);
+    frame_rotation(q, F.rot_c, F.rot_s, A.new_k, false, A.suppress_rotation, m);
     for (int t = 0; t < 9; ++t) rot[t] = (float)m[t];
 }
 
@@ -71,76 +69,26 @@ __device__ bool point_shift(const ZoomFrame& F, float py, size_t index, float (&
     return true;
 }
 
-// light refraction — cpu_undistort.rs:767-776, :805-814
-__device__ __forceinline__ void refract(float lrc, float& x, float& y) {
-    if (lrc != 1.0f && lrc > 0.0f) {
-        const float r = sqrtf(x * x + y * y);
-        if (r != 0.0f) {
-            const float sin_theta_d = (r / sqrtf(1.0f + r * r)) / lrc;
-            const float r_d = sin_theta_d / sqrtf(1.0f - sin_theta_d * sin_theta_d);
-            const float s = r_d / r;
-            x = x * s; y = y * s;
-        }
-    }
-}
-
-// map_coord (util.rs:144-147) in f32, IEEE division
-__device__ __forceinline__ float pm_map(float x, float in_min, float in_max, float out_min, float out_max) {
-    return (x - in_min) * (out_max - out_min) / (in_max - in_min) + out_min;
-}
-// The mesh block of undistort_points — cpu_undistort.rs:712-746: focal-plane distortion first (added here, subtracted in the warp), then
-// the distorting mesh through the f64 bivariate spline.  No inverted-framebuffer flips on this path.
-__device__ void point_mesh(const ZoomArgs& A, const ZoomFrame& F, float& x, float& y) {
-    const double* __restrict__ m = F.mesh;
-    const float fw = (float)A.kp.width, fh = (float)A.kp.height;
-    const double m0 = __ldg(m);
-    const double size_x = __ldg(m + 3), size_y = __ldg(m + 4);
-    const float ox = (float)__ldg(m + 5), oy = (float)__ldg(m + 6), cw = (float)__ldg(m + 7), ch = (float)__ldg(m + 8);
-    const uint32_t o = as_usize_small(m0);
-    if (m0 > 0.0 && o < F.mesh_len && __ldg(m + o) > 0.0) {          // FocalPlaneDistortion :714-733 (the reference indexes unchecked)
-        const double stblz_grid = size_y / 8.0;
-        x = pm_map(x, 0.0f, fw, ox, ox + cw);
-        y = pm_map(y, 0.0f, fh, oy, oy + ch);
-        const double q = floor((double)y / stblz_grid);
-        const uint32_t idx = as_usize_small(fmin(fmax(q, 0.0), 7.0));            // f64::max / min ignore NaN: NaN -> 0
-        const double delta = (double)y - stblz_grid * (double)idx;
-        x += (float)(__ldg(m + o + 4 + idx * 2 + 0) * delta);
-        y += (float)(__ldg(m + o + 4 + idx * 2 + 1) * delta);
-        for (uint32_t j = 0; j < idx; ++j) {
-            x += (float)(__ldg(m + o + 4 + j * 2 + 0) * stblz_grid);
-            y += (float)(__ldg(m + o + 4 + j * 2 + 1) * stblz_grid);
-        }
-        x = pm_map(x, ox, ox + cw, 0.0f, fw);
-        y = pm_map(y, oy, oy + ch, 0.0f, fh);
-    }
-    if (m0 > 10.0) {                                                 // :735-745
-        x = pm_map(x, 0.0f, fw, ox, ox + cw);
-        y = pm_map(y, 0.0f, fh, oy, oy + ch);
-        const uint32_t n_x = as_usize_small(__ldg(m + 1)), n_y = as_usize_small(__ldg(m + 2));
-        const MeshView mv{ m };
-        double nx = (double)x, ny = (double)y;
+// The mesh block of undistort_points — cpu_undistort.rs:712-746: focal-plane distortion first, then the distorting mesh.  No
+// inverted-framebuffer flips on this path.
+__device__ void point_mesh(const ZoomFrame& F, float& x, float& y) {
+    const MeshView mesh{ F.mesh };
+    const MeshAux& aux = F.mesh_aux;
+    const double mesh0 = mesh[0];
+    const uint32_t o = as_usize_small(mesh0);
+    if (mesh0 > 0.0 && o < F.mesh_len && mesh[o] > 0.0) focal_plane_shift<true>(mesh, aux, o, x, y);     // :714-733 (the reference indexes unchecked)
+    if (mesh0 > 10.0) {                                                                                     // :735-745
+        x = map_apply(x, aux.to_crop_x);
+        y = map_apply(y, aux.to_crop_y);
+        const uint32_t n_x = as_usize_small(mesh[1]), n_y = as_usize_small(mesh[2]);
         if (n_x >= 2 && n_x <= GF_MAX_GRID && n_y >= 2 && n_y <= GF_MAX_GRID) {
-            nx = mesh_bivariate(mv, n_x, n_y, size_x, size_y, 0, (double)x, (double)y);
-            ny = mesh_bivariate(mv, n_x, n_y, size_x, size_y, 1, (double)x, (double)y);
+            double nx, ny;
+            mesh_spline(mesh, aux, n_x, n_y, mesh[3], mesh[4], (double)x, (double)y, nx, ny);
+            x = (float)nx; y = (float)ny;
         }
-        x = pm_map((float)nx, ox, ox + cw, 0.0f, fw);
-        y = pm_map((float)ny, oy, oy + ch, 0.0f, fh);
+        x = map_apply(x, aux.to_frame_x);
+        y = map_apply(y, aux.to_frame_y);
     }
-}
-
-template <int LENS, int DIGITAL>
-__device__ void lc_r_of(const ZoomArgs& A, float ox, float oy, float& rx, float& ry) {        // cpu_undistort.rs:794-815
-    const gf_kernel_params& P = A.kp;
-    float qx = ox, qy = oy;
-    if (DIGITAL != GF_LENS_NONE) {
-        const float uzx = (qx - A.out_cx) * A.fov + A.out_cx, uzy = (qy - A.out_cy) * A.fov + A.out_cy;
-        float dx, dy;
-        if (Lens<DIGITAL>::undistort(uzx, uzy, P, false, dx, dy)) { qx = (dx - A.out_cx) / A.fov + A.out_cx; qy = (dy - A.out_cy) / A.fov + A.out_cy; }
-    }
-    float nx = (qx - A.out_cx) / A.out_fx, ny = (qy - A.out_cy) / A.out_fy;
-    { float dx, dy; if (Lens<LENS>::undistort(nx, ny, P, A.lens_noop != 0, dx, dy)) { nx = dx; ny = dy; } }
-    refract(P.light_refraction_coefficient, nx, ny);
-    rx = (nx * A.out_fx) + A.out_cx; ry = (ny * A.out_fy) + A.out_cy;
 }
 
 // one point of undistort_points — cpu_undistort.rs:699-857
@@ -153,28 +101,30 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     if (A.hstretch != 0.0f) x *= A.hstretch;
     if (A.vstretch != 0.0f) y *= A.vstretch;
     if (DIGITAL != GF_LENS_NONE) { float tx, ty; if (Lens<DIGITAL>::undistort(x, y, P, false, tx, ty)) { x = tx; y = ty; } }
-    if (F.mesh && F.mesh_len > 9) point_mesh(A, F, x, y);          // cpu_undistort.rs:712-746
+    if (F.mesh && F.mesh_len > 9) point_mesh(F, x, y);             // cpu_undistort.rs:712-746
     float sh[5];
     if (point_shift(F, py, index, sh)) {             // cpu_undistort.rs:748-757 (sic: y is rotated with the already rotated x)
         const float cos_a = gf_cosf(sh[2]), sin_a = gf_sinf(sh[2]);
-        x = x - A.cx - sh[3] + sh[0];
-        y = y - A.cy - sh[4] + sh[1];
-        x = cos_a * x - sin_a * y + A.cx;
-        y = sin_a * x + cos_a * y + A.cy;
+        x = x - P.c[0] - sh[3] + sh[0];
+        y = y - P.c[1] - sh[4] + sh[1];
+        x = cos_a * x - sin_a * y + P.c[0];
+        y = sin_a * x + cos_a * y + P.c[1];
     }
-    const float pwx = (x - A.cx) / A.fx, pwy = (y - A.cy) / A.fy;
+    const float pwx = (x - P.c[0]) / P.f[0], pwy = (y - P.c[1]) / P.f[1];
     float ptx, pty;
     if (!Lens<LENS>::undistort(pwx, pwy, P, A.lens_noop != 0, ptx, pty)) { outx = -1000000.0f; outy = -1000000.0f; return; }
-    refract(P.light_refraction_coefficient, ptx, pty);
+    const bool refract = F.lrc != 1.0f && F.lrc > 0.0f;
+    if (refract) refract_undistort(ptx, pty, F.lrc);
     const float pr0 = rot[0] * ptx + rot[1] * pty + rot[2] * 1.0f;
     const float pr1 = rot[3] * ptx + rot[4] * pty + rot[5] * 1.0f;
     const float pr2 = rot[6] * ptx + rot[7] * pty + rot[8] * 1.0f;
     ptx = pr0 / pr2; pty = pr1 / pr2;
-    if (A.lc) {                                         // :782-852
-        const float nx = (ptx - A.out_cx) / A.out_fx, ny = (pty - A.out_cy) / A.out_fy;
+    if (F.lc) {                                         // :782-852
+        const float amount = F.amount, factor = F.factor, out_fx = F.out_fx, out_fy = F.out_fy;
+        const float nx = (ptx - A.out_cx) / out_fx, ny = (pty - A.out_cy) / out_fy;
         float dx, dy;
         Lens<LENS>::distort(nx, ny, 1.0f, P, A.lens_noop != 0, dx, dy);
-        float p2x = (dx * A.out_fx) + A.out_cx, p2y = (dy * A.out_fy) + A.out_cy;
+        float p2x = (dx * out_fx) + A.out_cx, p2y = (dy * out_fy) + A.out_cy;
         if (DIGITAL != GF_LENS_NONE) {
             const float uzx = (p2x - A.out_cx) * A.fov + A.out_cx, uzy = (p2y - A.out_cy) * A.fov + A.out_cy;
             float ddx, ddy;
@@ -182,17 +132,20 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
             p2x = (ddx - A.out_cx) / A.fov + A.out_cx; p2y = (ddy - A.out_cy) / A.fov + A.out_cy;
         }
         float ox = ptx, oy = pty;
-        if (isfinite(p2x) && isfinite(p2y)) { ox = p2x * A.factor + ptx * A.amount; oy = p2y * A.factor + pty * A.amount; }
+        if (isfinite(p2x) && isfinite(p2y)) { ox = p2x * factor + ptx * amount; oy = p2y * factor + pty * amount; }
+        auto r_of = [&](float qx, float qy, float& rx, float& ry) {          // :794-815
+            lens_correction_undistort<LENS, DIGITAL>(qx, qy, P, A.out_cx, A.out_cy, out_fx, out_fy, A.fov, A.lens_noop != 0, true, refract, F.lrc, rx, ry);
+        };
         for (int it = 0; it < 10; ++it) {
-            float rx, ry; lc_r_of<LENS, DIGITAL>(A, ox, oy, rx, ry);
-            const float g0 = A.amount * ox + A.factor * rx - ptx, g1 = A.amount * oy + A.factor * ry - pty;
+            float rx, ry; r_of(ox, oy, rx, ry);
+            const float g0 = amount * ox + factor * rx - ptx, g1 = amount * oy + factor * ry - pty;
             if (fabsf(g0) < 0.02f && fabsf(g1) < 0.02f) break;
             const float eps = 1.0f;
             float rxx, rxy, ryx, ryy;
-            lc_r_of<LENS, DIGITAL>(A, ox + eps, oy, rxx, rxy);
-            lc_r_of<LENS, DIGITAL>(A, ox, oy + eps, ryx, ryy);
-            const float j11 = A.amount + A.factor * (rxx - rx) / eps, j21 = A.factor * (rxy - ry) / eps;
-            const float j12 = A.factor * (ryx - rx) / eps,            j22 = A.amount + A.factor * (ryy - ry) / eps;
+            r_of(ox + eps, oy, rxx, rxy);
+            r_of(ox, oy + eps, ryx, ryy);
+            const float j11 = amount + factor * (rxx - rx) / eps, j21 = factor * (rxy - ry) / eps;
+            const float j12 = factor * (ryx - rx) / eps,          j22 = amount + factor * (ryy - ry) / eps;
             const float det = j11 * j22 - j12 * j21;
             if (!isfinite(det) || fabsf(det) < 1e-9f) break;
             const float ddx = ( j22 * g0 - j12 * g1) / det, ddy = (-j21 * g0 + j11 * g1) / det;
@@ -207,45 +160,38 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
 constexpr int ZOOM_RECT_LEN = RECT_POINTS;
 constexpr int ZOOM_INTERP_LEN = 63;       // (30 + 1) * 3 - 30
 
+// nearest_edge: order-dependent fold over the polygon (fov_iterative.rs:136-151), shrinking (w, h); the index of the last point that
+// shrank it, or -1
+__device__ int nearest_edge(const float* poly, int plen, float cx, float cy, float inv_aspect, float& w, float& h) {
+    int idx = -1;
+    for (int i = 0; i < plen; ++i) {
+        const float ap0 = fabsf(poly[2 * i] - cx), ap1 = fabsf(poly[2 * i + 1] - cy);
+        if (ap0 < w && ap1 < h) {
+            if (ap1 > ap0 * inv_aspect) { w = ap1 / inv_aspect; h = ap1; } else { w = ap0; h = ap0 * inv_aspect; }
+            idx = i;
+        }
+    }
+    return idx;
+}
+
 template <int LENS, int DIGITAL>
-__global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ ZoomArgs A0, const ZoomFrame* __restrict__ frames, double* __restrict__ out) {
+__global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ ZoomArgs A, const ZoomFrame* __restrict__ frames, double* __restrict__ out) {
     __shared__ float rect[2 * ZOOM_RECT_LEN], poly[2 * ZOOM_RECT_LEN];
     __shared__ float sw, sh; __shared__ int sidx;
-    const ZoomFrame F = frames[blockIdx.x];
+    const ZoomFrame& F = frames[blockIdx.x];
     const int tid = threadIdx.x;
-    // keyframed clips: this frame's rotation / zoom centre / lens-correction strength / refraction replace the per-call values
-    __shared__ ZoomArgs SA;
-    if (F.keyed) {
-        if (tid == 0) {
-            SA = A0;
-            SA.rot_c = F.rot_c; SA.rot_s = F.rot_s; SA.zc_x = F.zc_x; SA.zc_y = F.zc_y; SA.kp.light_refraction_coefficient = F.lrc;
-            SA.lc = F.lc; SA.amount = F.amount; SA.factor = F.factor; SA.out_fx = F.out_fx; SA.out_fy = F.out_fy;
-        }
-        __syncthreads();
-    }
-    const ZoomArgs& A = F.keyed ? SA : A0;
     const float cx = A.in_w / 2.0f, cy = A.in_h / 2.0f;
     if (tid < ZOOM_RECT_LEN) {
         float x, y; rect_point(A.in_w, A.in_h, A.margin, tid, x, y);
         rect[2 * tid] = x; rect[2 * tid + 1] = y;
         float ux, uy; undistort_point_rs<LENS, DIGITAL>(A, F, x, y, (size_t)tid, ux, uy);
-        poly[2 * tid] = ux - A.zc_x; poly[2 * tid + 1] = uy - A.zc_y;
+        poly[2 * tid] = ux - F.zc_x; poly[2 * tid + 1] = uy - F.zc_y;
     }
     if (tid == 0) { sw = 1000000.0f; sh = 1000000.0f * A.inv_aspect; }
     __syncthreads();
     int plen = ZOOM_RECT_LEN;
     for (int it = 1; it < 5; ++it) {
-        if (tid == 0) {                                  // nearest_edge: order-dependent fold (fov_iterative.rs:136-151)
-            float w = sw, h = sh; int idx = -1;
-            for (int i = 0; i < plen; ++i) {
-                const float ap0 = fabsf(poly[2 * i] - cx), ap1 = fabsf(poly[2 * i + 1] - cy);
-                if (ap0 < w && ap1 < h) {
-                    if (ap1 > ap0 * A.inv_aspect) { w = ap1 / A.inv_aspect; h = ap1; } else { w = ap0; h = ap0 * A.inv_aspect; }
-                    idx = i;
-                }
-            }
-            sw = w; sh = h; sidx = idx;
-        }
+        if (tid == 0) sidx = nearest_edge(poly, plen, cx, cy, A.inv_aspect, sw, sh);
         __syncthreads();
         const int idx = sidx;
         if (idx < 0) break;
@@ -262,17 +208,10 @@ __global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ Z
             undistort_point_rs<LENS, DIGITAL>(A, F, dx, dy, (size_t)tid, nx, ny);
         }
         __syncthreads();                                 // everyone has read rect/poly of this round
-        if (tid < ZOOM_INTERP_LEN) { poly[2 * tid] = nx - A.zc_x; poly[2 * tid + 1] = ny - A.zc_y; }
+        if (tid < ZOOM_INTERP_LEN) { poly[2 * tid] = nx - F.zc_x; poly[2 * tid + 1] = ny - F.zc_y; }
         plen = ZOOM_INTERP_LEN;
         __syncthreads();
-        if (tid == 0) {                                  // :127 nearest_edge again (index discarded)
-            float w = sw, h = sh;
-            for (int i = 0; i < plen; ++i) {
-                const float ap0 = fabsf(poly[2 * i] - cx), ap1 = fabsf(poly[2 * i + 1] - cy);
-                if (ap0 < w && ap1 < h) { if (ap1 > ap0 * A.inv_aspect) { w = ap1 / A.inv_aspect; h = ap1; } else { w = ap0; h = ap0 * A.inv_aspect; } }
-            }
-            sw = w; sh = h;
-        }
+        if (tid == 0) (void)nearest_edge(poly, plen, cx, cy, A.inv_aspect, sw, sh);       // :127 nearest_edge again (index discarded)
         __syncthreads();
     }
     if (tid == 0) out[blockIdx.x] = (double)(sw * 2.0f / A.out_w);      // :133
@@ -336,80 +275,62 @@ static double points_fov(const gf_compute_params* cp, size_t frame, bool use_fov
 
 // Everything undistort_points (cpu_undistort.rs:652-698) and at_timestamp_for_points (frame_transform.rs:352-410) derive from
 // ComputeParams for one call: kernel params, K_new.
-static void setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, double fov, double lens_correction_amount, ZoomArgs& A) {
+static void setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, double fov, ZoomArgs& A) {
     memset(&A, 0, sizeof(A));
     const double* K = cp.camera_matrix;
     get_new_k(&cp, K, fov, A.new_k);
     A.horizontal = cp.readout_horizontal; A.suppress_rotation = cp.suppress_rotation;
-    const double a = cp.video_rotation * (M_PI / 180.0);
-    A.rot_c = cos(a); A.rot_s = sin(a);
     A.org = g->org_track();
     A.duration_ms = cp.duration_ms;
     A.offsets = g->sync_offsets(cp.gyro_offset_ms);
     gf_kernel_params& kp = A.kp;                                                            // cpu_undistort.rs:671-683
     kp.width = cp.width; kp.height = cp.height; kp.output_width = cp.output_width; kp.output_height = cp.output_height;
-    A.fx = (float)K[0]; A.fy = (float)K[4]; A.cx = (float)K[2]; A.cy = (float)K[5];
-    kp.f[0] = A.fx; kp.f[1] = A.fy; kp.c[0] = A.cx; kp.c[1] = A.cy;
+    kp.f[0] = (float)K[0]; kp.f[1] = (float)K[4]; kp.c[0] = (float)K[2]; kp.c[1] = (float)K[5];
     for (int i = 0; i < 12; ++i) kp.k[i] = (float)cp.distortion_coeffs[i];
     for (int i = 0; i < 16 && i < cp.n_digital_lens_params; ++i) kp.digital_lens_params[i] = (float)cp.digital_lens_params[i];
-    kp.light_refraction_coefficient = (float)cp.light_refraction_coefficient;
     A.lens_noop = lens_noop(distortion_model, kp.k) ? 1 : 0;
     A.hstretch = cp.input_horizontal_stretch > 0.001 ? (float)cp.input_horizontal_stretch : 0.0f;
     A.vstretch = cp.input_vertical_stretch   > 0.001 ? (float)cp.input_vertical_stretch   : 0.0f;
-    A.lc = lens_correction_amount < 1.0 ? 1 : 0;
-    if (A.lc) {
-        A.out_cx = (float)cp.output_width / 2.0f; A.out_cy = (float)cp.output_height / 2.0f;
-        A.amount = (float)lens_correction_amount; A.factor = fmaxf(1.0f - A.amount, 0.001f);
-        A.out_fx = A.fx / (float)fov / A.factor; A.out_fy = A.fy / (float)fov / A.factor; A.fov = (float)fov;
-    }
+    A.out_cx = (float)cp.output_width / 2.0f; A.out_cy = (float)cp.output_height / 2.0f; A.fov = (float)fov;
 }
-// readout timing, smoothed(ts) * org(ts)^-1, shifts and distorting mesh of one frame — frame_transform.rs:366-388,412-434
-static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& cp, double ts, size_t frame) {
-    ZoomFrame f;
+// One frame's record at timestamp `ts`: readout timing, smoothed(ts) * org(ts)^-1, shifts and distorting mesh (frame_transform.rs:366-388,
+// 412-434), video rotation (:354), refraction (cpu_undistort.rs:661) and the lens-correction blend (:686-694) of strength
+// `lens_correction_amount`.  `zoom_keys` (find_fov, fov_iterative.rs:44-46): the zoom centre and the lens-correction strength follow their
+// tracks, `lens_correction_amount` being the value without one.
+static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& cp, const ZoomArgs& A, double ts, size_t frame,
+                                double lens_correction_amount, bool zoom_keys) {
+    ZoomFrame f{};
     const FrameTiming t = frame_timing(&cp, frame, ts, false);
     f.q0 = t.q0; f.start_ts = t.start_ts; f.row_readout_time = t.row_readout_time;
     f.rs_on = fabs(t.frame_readout_time) > 0.0 ? 1 : 0;
-    f.keyed = 0;
     f.mesh = g->frame_mesh(frame, f.mesh_len);
+    if (f.mesh) make_mesh_aux(g->mesh_index[frame].header, (float)cp.width, (float)cp.height, f.mesh_aux);
     StabSplines sp;
     const bool shifts = !(cp.suppress_rotation && cp.frame_readout_time == 0.0) && g->frame_splines(frame, sp);       // :432-434
     f.stab = camera_stab_at(&cp, frame, false, shifts ? &sp : nullptr);
+    const double a = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation) * (M_PI / 180.0);
+    f.rot_c = cos(a); f.rot_s = sin(a);
+    f.lrc = (float)keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);
+    double lca = lens_correction_amount;
+    if (zoom_keys) {
+        f.zc_x = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * A.in_w;
+        f.zc_y = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * A.in_h;
+        lca = keyframed(&cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, lens_correction_amount);
+    }
+    f.lc = lca < 1.0 ? 1 : 0;
+    f.amount = (float)lca; f.factor = fmaxf(1.0f - f.amount, 0.001f);
+    f.out_fx = A.kp.f[0] / A.fov / f.factor; f.out_fy = A.kp.f[1] / A.fov / f.factor;
     return f;
 }
-// at_timestamp_for_points / undistort_points for ONE timestamp: the tracks they read become the constants of a private copy
-static gf_compute_params resolve_point_keyframes(const gf_compute_params& cp, double ts, size_t frame) {
+// get_lens_data_at_timestamp of this frame (frame_transform.rs:360) for ONE timestamp: the per-frame lens in a private copy of `cp`
+static gf_compute_params resolve_point_lens(const gf_compute_params& cp, size_t frame) {
     gf_compute_params r = cp;
-    if (cp.lens_per_frame && frame < cp.n_lens_per_frame) {                         // get_lens_data_at_timestamp of this frame (:360)
+    if (cp.lens_per_frame && frame < cp.n_lens_per_frame) {
         const gf_lens_data& L = cp.lens_per_frame[frame];
         memcpy(r.camera_matrix, L.camera_matrix, sizeof(r.camera_matrix)); memcpy(r.distortion_coeffs, L.distortion_coeffs, sizeof(r.distortion_coeffs));
         r.radial_distortion_limit = L.radial_distortion_limit;
     }
-    r.video_rotation = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation);                                  // frame_transform.rs:354
-    r.light_refraction_coefficient = keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);   // cpu_undistort.rs:661
     return r;
-}
-static bool zoom_any_keyframes(const gf_compute_params& cp) {
-    const int used[] = { GF_KF_VIDEO_ROTATION, GF_KF_ZOOMING_CENTER_X, GF_KF_ZOOMING_CENTER_Y, GF_KF_LENS_CORRECTION_STRENGTH, GF_KF_LIGHT_REFRACTION_COEFF };
-    for (int t : used) if (cp.keyframes[t].n > 0 && cp.keyframes[t].ts_us && cp.keyframes[t].value) return true;
-    return false;
-}
-// The values of frame `ts` that replace ZoomArgs' per-call ones (`A` supplies fx / fy / fov / sizes): video rotation
-// (frame_transform.rs:354), refraction (cpu_undistort.rs:661), zoom centre and lens-correction strength (fov_iterative.rs:44-46;
-// `lens_correction_default` = what the caller would have used without a track).
-static void fill_keyed(ZoomFrame& f, const gf_compute_params& cp, const ZoomArgs& A, double ts, double fov, double lens_correction_default, bool zoom_center) {
-    f.keyed = 1;
-    const double a = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation) * (M_PI / 180.0);
-    f.rot_c = cos(a); f.rot_s = sin(a);
-    f.lrc = (float)keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);
-    f.zc_x = A.zc_x; f.zc_y = A.zc_y;
-    if (zoom_center) {
-        f.zc_x = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * A.in_w;
-        f.zc_y = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * A.in_h;
-    }
-    const double lca = zoom_center ? keyframed(&cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, lens_correction_default) : lens_correction_default;
-    f.lc = lca < 1.0 ? 1 : 0;
-    f.amount = (float)lca; f.factor = fmaxf(1.0f - f.amount, 0.001f);
-    f.out_fx = A.fx / (float)fov / f.factor; f.out_fy = A.fy / (float)fov / f.factor;
 }
 
 // ---- the temporal filters of zoom_dynamic.rs, on the host like in the reference ----
@@ -478,22 +399,14 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
 
     ZoomArgs A;
     const double fov = points_fov(&cp, 0, false, 0.0);            // use_fovs = false: 1 after the adjustments
-    setup_points_args(g, cp, distortion_model, fov, cp.lens_correction_amount, A);
+    setup_points_args(g, cp, distortion_model, fov, A);
     const float ratio = (float)cp.width / (float)(org_ow > 1 ? org_ow : 1);                // FovIterative::new :78-89
     A.in_w = (float)cp.width; A.in_h = (float)cp.height;
     A.out_w = (float)org_ow * ratio; const float out_h = (float)org_oh * ratio;
     A.inv_aspect = out_h / A.out_w; A.margin = fov_algorithm_margin;
-    A.zc_x = (float)cp.adaptive_zoom_center_offset[0] * A.in_w; A.zc_y = (float)cp.adaptive_zoom_center_offset[1] * A.in_h;
     // per-frame uniforms on the host: two O(log n) lookups per frame
     std::vector<ZoomFrame> hf(n);
-    const bool keyed = zoom_any_keyframes(cp);
-    if (keyed) {          // the lens-correction constants of ZoomArgs are needed even when the default strength is 1
-        A.out_cx = (float)cp.output_width / 2.0f; A.out_cy = (float)cp.output_height / 2.0f; A.fov = (float)fov;
-    }
-    for (size_t i = 0; i < n; ++i) {
-        hf[i] = frame_uniforms(g, cp, timestamps_ms[i], i);
-        if (keyed) fill_keyed(hf[i], cp, A, timestamps_ms[i], fov, cp.lens_correction_amount, true);
-    }
+    for (size_t i = 0; i < n; ++i) hf[i] = frame_uniforms(g, cp, A, timestamps_ms[i], i, cp.lens_correction_amount, true);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     ZoomFrame* d_frames = nullptr; double* d_out = nullptr;
     cudaError_t e;
@@ -519,11 +432,11 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
     if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     ZoomArgs A;
-    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // lens, video rotation and refraction at this timestamp
+    const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
     const gf_compute_params* cp = &rcp;
     const double fov = points_fov(cp, frame, use_fovs != 0, timestamp_ms);
-    setup_points_args(g, *cp, distortion_model, fov, lens_correction_amount, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frame);
+    setup_points_args(g, *cp, distortion_model, fov, A);
+    const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, lens_correction_amount, false);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     float2* d_in = nullptr; float* d_out = nullptr;
     cudaError_t e;
@@ -546,14 +459,14 @@ GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* c
     if (!g || !cp_user || !out_rgb_dev) return GF_ERR_BAD_PARAMS;
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
     if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
-    const gf_compute_params rcp = resolve_point_keyframes(*cp_user, timestamp_ms, frame);     // lens, video rotation and refraction at this timestamp
+    const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
     const gf_compute_params* cp = &rcp;
     if (cp->width < 1 || cp->height < 1) return GF_ERR_BAD_PARAMS;
     if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     ZoomArgs A;
     const double fov = points_fov(cp, frame, true, timestamp_ms);
-    setup_points_args(g, *cp, distortion_model, fov, 1.0, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, timestamp_ms, frame);
+    setup_points_args(g, *cp, distortion_model, fov, A);
+    const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, 1.0, false);
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
     const size_t n = (size_t)cp->width * (size_t)cp->height;
     k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);

@@ -199,9 +199,9 @@ def test_device_point_path_with_ibis_shifts_matches_oracle(kw):
     assert np.abs(want / base - 1).max() > 1e-3          # the shifts do move the polygon
 
 
-def _distorting_mesh(w, h, fpd):
+def _distorting_mesh(w, h, fpd, rows=9):
     from gyroflow_b200 import synth
-    return np.asarray(synth.synthetic_mesh(w, h, amp=6.0, n=9, with_fpd=fpd), dtype=np.float64)     # same layout as mesh_correction[frame].0 (sony.rs:483-511)
+    return np.asarray(synth.synthetic_mesh(w, h, amp=6.0, n=rows, with_fpd=fpd), dtype=np.float64)     # same layout as mesh_correction[frame].0 (sony.rs:483-511)
 
 
 @pytest.mark.parametrize("fpd", [False, True])
@@ -229,10 +229,11 @@ def test_point_path_distorting_mesh_oracle_matches_second_restatement(fpd):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("fpd", [False, True])
-def test_device_point_path_with_distorting_mesh_matches_oracle(fpd):
+@pytest.mark.parametrize("fpd,rows", [(False, 9), (True, 9), (False, 7), (True, 7)], ids=["False", "True", "False-7rows", "True-7rows"])
+def test_device_point_path_with_distorting_mesh_matches_oracle(fpd, rows):
+    """9-row meshes take the unrolled spline (mesh_interpolate9), other grids the general one (mesh_bivariate)."""
     n = 12
-    meshes = [_distorting_mesh(1920, 1080, fpd) if i % 3 != 2 else None for i in range(n)]
+    meshes = [_distorting_mesh(1920, 1080, fpd, rows) if i % 3 != 2 else None for i in range(n)]
     cp = make_cp(lens="sony", camera_stab=_zoom_stab(n, 1080), distorting_meshes=meshes)
     lib = oracle_lib.load()
     dg = g.DeviceGyro(cp)
