@@ -24,27 +24,11 @@ using namespace gf;
 
 namespace {
 
-thread_local std::string g_last_error;
-
-// A device buffer (PINNED: page-locked host memory) that grows on demand.  Growing waits for the stream, whose queued work may still
-// use the old buffer, frees it and allocates the new size.  `len` counts elements.
-template <class T, bool PINNED = false> struct GrowBuf {
-    T* ptr = nullptr; size_t len = 0;
-    cudaError_t reserve(size_t n, cudaStream_t st) {
-        if (n <= len) return cudaSuccess;
-        if (ptr) { const cudaError_t e = cudaStreamSynchronize(st); if (e != cudaSuccess) return e; release(); }
-        const cudaError_t e = PINNED ? cudaMallocHost((void**)&ptr, n * sizeof(T)) : cudaMalloc((void**)&ptr, n * sizeof(T));
-        if (e == cudaSuccess) len = n; else ptr = nullptr;
-        return e;
-    }
-    void release() { if (ptr) { if (PINNED) cudaFreeHost(ptr); else cudaFree(ptr); } ptr = nullptr; len = 0; }
-};
-
 struct Slot {                                   // one in-flight set of per-frame tables
     GrowBuf<float, true> h_mat, h_mesh;
     GrowBuf<float> d_mat, d_mesh;
     GrowBuf<double> d_mesh64;                   // the mesh widened to f64 once per frame (cpu_undistort.rs:539), then one MeshAux
-    cudaEvent_t done = nullptr;
+    Event done;
 };
 constexpr int kSlots = 4;
 
@@ -89,7 +73,7 @@ struct gf_cuda_ctx {
     // HOST multi-plane frames (gf_cuda_undistort_planes): one device staging pair per plane
     std::vector<GrowBuf<uint8_t>> plane_src, plane_dst;
     GrowBuf<uint2> coords;               // two-pass path: the frame's coordinate map(s)
-    cudaStream_t stream = nullptr;
+    Stream stream;
     size_t max_rows = 0;
     Slot slots[kSlots];
     int next_slot = 0;
@@ -99,16 +83,6 @@ struct gf_cuda_ctx {
 };
 
 namespace {
-
-int fail(gf_cuda_ctx* ctx, int code, const std::string& msg) {
-    g_last_error = msg;
-    if (ctx) ctx->last_error = msg;
-    return code;
-}
-int cuda_fail(gf_cuda_ctx* ctx, cudaError_t e, const char* what) {
-    return fail(ctx, GF_ERR_CUDA, std::string(what) + ": " + cudaGetErrorName(e) + " (" + cudaGetErrorString(e) + ")");
-}
-#define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return cuda_fail(ctx, e_, #call); } while (0)
 
 // LAY_* of a pixel type (GF_PIX_*), or -1 if unknown
 int pix_layout(int pixel_type) {
@@ -147,29 +121,30 @@ const char* const kLensNames[GF_LENS_COUNT] = {
     "gopro", "gopro_superview", "gopro_hyperview", "gopro_warp", "digital_stretch", "gopro6_superview" };
 
 // process_pixels / OclWrapper::new validation (stabilization/mod.rs:613,636-640; opencl.rs:179; wgpu.rs:150)
-int validate(gf_cuda_ctx* ctx, const gf_kernel_params* p, const gf_buffer_desc* in, const gf_buffer_desc* out, int bpp) {
-    if (!p || !in || !out) return fail(ctx, GF_ERR_BAD_PARAMS, "null argument");
+// `err`: the context's message, or nullptr before there is a context.
+int validate(std::string* err, const gf_kernel_params* p, const gf_buffer_desc* in, const gf_buffer_desc* out, int bpp) {
+    if (!p || !in || !out) return fail(err, GF_ERR_BAD_PARAMS, "null argument");
     if (in->height < 4 || out->height < 4 || p->height < 4 || p->output_height < 4)
-        return fail(ctx, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall: height < 4");
-    if (p->stride < 1 || p->output_stride < 1) return fail(ctx, GF_ERR_BAD_STRIDE, "InvalidStride: stride < 1");
+        return fail(err, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall: height < 4");
+    if (p->stride < 1 || p->output_stride < 1) return fail(err, GF_ERR_BAD_STRIDE, "InvalidStride: stride < 1");
     if (p->width > 16384 || p->output_width > 16384 || p->width < 1 || p->output_width < 1)
-        return fail(ctx, GF_ERR_BAD_PARAMS, "width out of range (1..16384)");
-    if (in->width > p->stride)         return fail(ctx, GF_ERR_BAD_STRIDE, "InvalidStride: input width > stride");
-    if (out->width > p->output_stride) return fail(ctx, GF_ERR_BAD_STRIDE, "InvalidStride: output width > output_stride");
+        return fail(err, GF_ERR_BAD_PARAMS, "width out of range (1..16384)");
+    if (in->width > p->stride)         return fail(err, GF_ERR_BAD_STRIDE, "InvalidStride: input width > stride");
+    if (out->width > p->output_stride) return fail(err, GF_ERR_BAD_STRIDE, "InvalidStride: output width > output_stride");
     if (p->stride != in->stride || p->output_stride != out->stride)
-        return fail(ctx, GF_ERR_BAD_STRIDE, "InvalidStride: KernelParams stride differs from the buffer description");
-    if (p->bytes_per_pixel != bpp) return fail(ctx, GF_ERR_BAD_PARAMS, "bytes_per_pixel does not match the pixel type");
-    if (p->matrix_count < 1) return fail(ctx, GF_ERR_BAD_PARAMS, "matrix_count < 1");
+        return fail(err, GF_ERR_BAD_STRIDE, "InvalidStride: KernelParams stride differs from the buffer description");
+    if (p->bytes_per_pixel != bpp) return fail(err, GF_ERR_BAD_PARAMS, "bytes_per_pixel does not match the pixel type");
+    if (p->matrix_count < 1) return fail(err, GF_ERR_BAD_PARAMS, "matrix_count < 1");
     if ((in->kind != GF_BUF_HOST && in->kind != GF_BUF_DEVICE) || (out->kind != GF_BUF_HOST && out->kind != GF_BUF_DEVICE) || !in->ptr || !out->ptr)
-        return fail(ctx, GF_ERR_BAD_PARAMS, "unsupported buffer source");
+        return fail(err, GF_ERR_BAD_PARAMS, "unsupported buffer source");
     // every tap the kernel may read must be inside the input buffer (Rust would panic on the slice index)
     const long long x0 = p->source_rect[0], y0 = p->source_rect[1], x1 = x0 + p->source_rect[2], y1 = y0 + p->source_rect[3];
     if (p->source_rect[2] > 0 && p->source_rect[3] > 0) {
-        if (x0 < 0 || y0 < 0) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "source_rect has a negative origin");
+        if (x0 < 0 || y0 < 0) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "source_rect has a negative origin");
         const unsigned long long last = (unsigned long long)(y1 - 1) * (unsigned long long)p->stride + (unsigned long long)x1 * (unsigned long long)bpp;
-        if (last > in->len) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input: source_rect exceeds the input buffer");
+        if (last > in->len) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input: source_rect exceeds the input buffer");
     }
-    if (out->len == 0) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "empty output buffer");
+    if (out->len == 0) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "empty output buffer");
     return GF_OK;
 }
 
@@ -396,8 +371,9 @@ const dim3 kBlock(GF_BLOCK_X, GF_BLOCK_Y);
 // One frame through the warp: the steps of run_warp and what they hand on to each other.
 struct FrameRun {
     gf_cuda_ctx* const ctx; const FrameJob& job;
+    std::string* const err = &ctx->last_error;
     const gf_buffer_desc* const in = job.in; const gf_buffer_desc* const out = job.out; const gf_kernel_params* const p = job.p;
-    const cudaStream_t st = job.stream ? (cudaStream_t)job.stream : ctx->stream;
+    const cudaStream_t st = job.stream ? (cudaStream_t)job.stream : ctx->stream.get();
     WarpArgs A;
     Slot* slot = nullptr;                   // the table slot of this frame, if it uses one (host tables, or a mesh to widen)
     uint32_t table_flags = TBL_WILD;        // host-known verdict: device tables are not trusted until validated
@@ -413,7 +389,7 @@ struct FrameRun {
         if (!job.tables_on_device || job.mesh_len > 0) {      // device tables still need a slot for the widened mesh
             slot = &ctx->slots[ctx->next_slot];
             ctx->next_slot = (ctx->next_slot + 1) % kSlots;
-            CK(cudaEventSynchronize(slot->done));            // the slot's previous frame has consumed its tables
+            CK(err, cudaEventSynchronize(slot->done.get()));            // the slot's previous frame has consumed its tables
         }
         if (job.tables_on_device) {
             // the verdict travels with the data: a device word written on this stream (or ordered before it) by whoever produced the table
@@ -424,11 +400,11 @@ struct FrameRun {
             memcpy(slot->h_mat.ptr, job.matrices, mat_bytes);
             table_flags = gf_table_flags_host(slot->h_mat.ptr, (size_t)p->matrix_count);
             A.table_flags = ctx->const_flags.ptr + (table_flags ? 1 : 0);
-            CK(cudaMemcpyAsync(slot->d_mat.ptr, slot->h_mat.ptr, mat_bytes, cudaMemcpyHostToDevice, st));
+            CK(err, cudaMemcpyAsync(slot->d_mat.ptr, slot->h_mat.ptr, mat_bytes, cudaMemcpyHostToDevice, st));
             A.matrices = slot->d_mat.ptr;
             if (job.mesh_len) {
                 memcpy(slot->h_mesh.ptr, job.mesh, job.mesh_len * sizeof(float));
-                CK(cudaMemcpyAsync(slot->d_mesh.ptr, slot->h_mesh.ptr, job.mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
+                CK(err, cudaMemcpyAsync(slot->d_mesh.ptr, slot->h_mesh.ptr, job.mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
                 A.mesh = slot->d_mesh.ptr;
             }
         }
@@ -436,7 +412,7 @@ struct FrameRun {
         if (job.mesh_len) {                                    // cpu_undistort.rs:539 — `mesh_data.iter().map(|x| *x as f64)`, once per frame
             double* const m64 = slot->d_mesh64.ptr;
             widen_mesh_kernel<<<(unsigned)((job.mesh_len + 255) / 256), 256, 0, st>>>(A.mesh, m64, (int)job.mesh_len, (float)p->width, (float)p->height);
-            CK(cudaGetLastError());
+            CK(err, cudaGetLastError());
             A.mesh64 = m64; A.mesh_aux = reinterpret_cast<const MeshAux*>(m64 + GF_MESH_MAX_LEN);
         }
         A.src = (const uint8_t*)in->ptr; A.dst = (uint8_t*)out->ptr; A.src_len = in->len; A.dst_len = out->len;
@@ -444,7 +420,7 @@ struct FrameRun {
             nvtxRangePushA("gf_h2d_frame");
             cudaError_t e_h2d = cudaMemcpyAsync(ctx->src_stage.ptr, in->ptr, in->len, cudaMemcpyHostToDevice, st);
             nvtxRangePop();
-            CK(e_h2d);
+            CK(err, e_h2d);
             A.src = ctx->src_stage.ptr;
         }
         // Does the kernel write every pixel of [0,w) x [0,h)?  (output_rect == whole buffer == output size: the bounds test of
@@ -454,7 +430,7 @@ struct FrameRun {
                      out->width == p->output_width && out->height == p->output_height && (p->flags & 4) == 0 &&
                      (size_t)out->height * (size_t)p->output_stride <= out->len + (size_t)(p->output_stride - out->width * ctx->combo.bpp());
         if (out->kind == GF_BUF_HOST) {
-            if (!full_cover) CK(cudaMemcpyAsync(ctx->dst_stage.ptr, out->ptr, out->len, cudaMemcpyHostToDevice, st));
+            if (!full_cover) CK(err, cudaMemcpyAsync(ctx->dst_stage.ptr, out->ptr, out->len, cudaMemcpyHostToDevice, st));
             A.dst = ctx->dst_stage.ptr;
         }
         return GF_OK;
@@ -465,22 +441,22 @@ struct FrameRun {
         if (!job.overlays(ctx)) return GF_OK;
         bool any_input_stage = false;
         if ((p->flags & GF_FLAG_DRAWING_ENABLED) && job.drawing && job.drawing_len) {
-            CK(ctx->h_drawing.reserve(job.drawing_len, st));   // (a growing reserve waits for the stream itself)
-            CK(ctx->d_drawing.reserve(job.drawing_len, st));
-            CK(cudaStreamSynchronize(st));                     // the previous frame's upload has left the pinned copy
+            CK(err, ctx->h_drawing.reserve(job.drawing_len, st));   // (a growing reserve waits for the stream itself)
+            CK(err, ctx->d_drawing.reserve(job.drawing_len, st));
+            CK(err, cudaStreamSynchronize(st));                     // the previous frame's upload has left the pinned copy
             for (size_t i = 0; i < job.drawing_len; ++i) { const uint8_t d = job.drawing[i]; ctx->h_drawing.ptr[i] = d; any_input_stage |= (d != 0 && (d & 1u) == 0u); }
-            CK(cudaMemcpyAsync(ctx->d_drawing.ptr, ctx->h_drawing.ptr, job.drawing_len, cudaMemcpyHostToDevice, st));   // opencl.rs: buf_drawing.write(drawing_buffer)
+            CK(err, cudaMemcpyAsync(ctx->d_drawing.ptr, ctx->h_drawing.ptr, job.drawing_len, cudaMemcpyHostToDevice, st));   // opencl.rs: buf_drawing.write(drawing_buffer)
             drawing_dev = ctx->d_drawing.ptr;
         }
         if (!any_input_stage) return GF_OK;
         if (in->kind == GF_BUF_DEVICE) {                       // never draw into the caller's buffer: private copy
-            CK(ctx->src_ovl.reserve(in->len, st));
-            CK(cudaMemcpyAsync(ctx->src_ovl.ptr, in->ptr, in->len, cudaMemcpyDeviceToDevice, st));
+            CK(err, ctx->src_ovl.reserve(in->len, st));
+            CK(err, cudaMemcpyAsync(ctx->src_ovl.ptr, in->ptr, in->len, cudaMemcpyDeviceToDevice, st));
             A.src = ctx->src_ovl.ptr;
         }
         const LayoutInfo& L = kLayouts[ctx->combo.layout];
         if (gf_internal_draw_overlays((void*)st, const_cast<uint8_t*>(A.src), in->len, in->width, in->height, p->stride, p, L.channels, L.scalar, 1,
-                                      drawing_dev, job.drawing_len) != GF_OK) return fail(ctx, GF_ERR_CUDA, "overlay kernel (input stage) failed");
+                                      drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (input stage) failed");
         return GF_OK;
     }
 
@@ -488,11 +464,11 @@ struct FrameRun {
     int plan_launch() {
         fill_uniforms(A, ctx->combo);
         grid = dim3((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);
-        if (grid.x == 0 || grid.y == 0 || grid.y > 65535) return fail(ctx, GF_ERR_BAD_PARAMS, "output buffer geometry out of range");
+        if (grid.x == 0 || grid.y == 0 || grid.y > 65535) return fail(err, GF_ERR_BAD_PARAMS, "output buffer geometry out of range");
         plan = plan_frame(ctx->combo, A, table_flags, job);
         if (plan.two_pass) {
-            if (!ctx->fn_shade && !job.coord_only) return fail(ctx, GF_ERR_UNSUPPORTED_COMBO, "no sampling kernel for this pixel layout");
-            CK(ctx->coords.reserve((size_t)A.out_cols * (size_t)A.out_rows * (size_t)plan.n_maps, st));
+            if (!ctx->fn_shade && !job.coord_only) return fail(err, GF_ERR_UNSUPPORTED_COMBO, "no sampling kernel for this pixel layout");
+            CK(err, ctx->coords.reserve((size_t)A.out_cols * (size_t)A.out_rows * (size_t)plan.n_maps, st));
             A.coord_out = ctx->coords.ptr;
         }
         return GF_OK;
@@ -507,8 +483,8 @@ struct FrameRun {
             const dim3 block2(GF_BLOCK_X, kPackedBlockY), grid2(grid.x, (A.out_rows + 2 * kPackedBlockY - 1) / (2 * kPackedBlockY));
             if (plan.a_cap > 0.0f) {
                 if (!ctx->defer_q.ptr) {                       // 4 MB: 1 M pairs = a quarter of a 4K frame's pairs; a full queue falls back inline
-                    CK(ctx->defer_q.reserve(1u << 20, st)); CK(ctx->defer_count.reserve(2, st));
-                    CK(cudaMemsetAsync(ctx->defer_count.ptr, 0, 2 * sizeof(unsigned), st));
+                    CK(err, ctx->defer_q.reserve(1u << 20, st)); CK(err, ctx->defer_count.reserve(2, st));
+                    CK(err, cudaMemsetAsync(ctx->defer_count.ptr, 0, 2 * sizeof(unsigned), st));
                 }
                 const unsigned cur = (unsigned)(ctx->filter_frames & 1ull);
                 ctx->filter_frames++;
@@ -516,23 +492,23 @@ struct FrameRun {
                 A.flt.q = ctx->defer_q.ptr; A.flt.cap = (uint32_t)ctx->defer_q.len;
                 A.flt.count = ctx->defer_count.ptr + cur; A.flt.count_next = ctx->defer_count.ptr + (cur ^ 1u);
                 A.flt.rho = 0x1p-17f; A.flt.a_cap = plan.a_cap; A.flt.tail = 0;
-                CK(launch_pdl(fn, grid2, block2, A, st));
+                CK(err, launch_pdl(fn, grid2, block2, A, st));
                 A.flt.tail = 1;                                // the deferred pairs, exact pre-pass; also re-arms the other counter
                 // one thread per deferred pair for up to 2 % of a 4K frame's pairs in a single wave of tiny blocks (idle blocks exit at once);
                 // more entries than threads are covered by the grid-stride loop
-                CK(launch_pdl(fn, dim3(ctx->sm_count * 16, 1), block2, A, st));
+                CK(err, launch_pdl(fn, dim3(ctx->sm_count * 16, 1), block2, A, st));
                 ctx->launches++;
-            } else CK(launch_pdl(fn, grid2, block2, A, st));
+            } else CK(err, launch_pdl(fn, grid2, block2, A, st));
         } else {
             const size_t map_len = (size_t)A.out_cols * (size_t)A.out_rows;
             for (int mi = 0; mi < plan.n_maps; ++mi) {        // one launch, or three for EWA (pixel, x-probe, y-probe)
                 if (plan.two_pass) { A.coord_out = ctx->coords.ptr + (size_t)mi * map_len; A.coord_shift = mi; }
                 fn<<<grid, kBlock, 0, st>>>(A);
-                CK(cudaGetLastError());
+                CK(err, cudaGetLastError());
                 if (mi > 0) ctx->launches++;
             }
         }
-        CK(cudaGetLastError());
+        CK(err, cudaGetLastError());
         ctx->launches++;
         return GF_OK;
     }
@@ -547,19 +523,19 @@ struct FrameRun {
                 if (job.more_planes > 0) { B.src = (const uint8_t*)in[i].ptr; B.dst = (uint8_t*)out[i].ptr; B.src_len = in[i].len; B.dst_len = out[i].len; }
                 fill_uniforms(B, ctx->combo);
                 ctx->fn_shade<<<grid, kBlock, 0, st>>>(B);
-                CK(cudaGetLastError());
+                CK(err, cudaGetLastError());
                 ctx->launches++;
             }
         }
-        if (slot) CK(cudaEventRecord(slot->done, st));
+        if (slot) CK(err, cudaEventRecord(slot->done.get(), st));
         if (job.overlays(ctx)) {                               // output stage: stage-1 drawing entries + safe area, on the final pixels
             const LayoutInfo& L = kLayouts[ctx->combo.layout];
             if (gf_internal_draw_overlays((void*)st, A.dst, out->len, out->width, out->height, p->output_stride, p, L.channels, L.scalar, 0,
-                                          drawing_dev, job.drawing_len) != GF_OK) return fail(ctx, GF_ERR_CUDA, "overlay kernel (output stage) failed");
+                                          drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (output stage) failed");
         }
         // render queue: per-frame output checksum, before the result leaves the device
         if (job.checksum_dev && gf_cuda_checksum_dev(A.dst, std::min<size_t>(out->len, (size_t)out->height * (size_t)p->output_stride), job.checksum_dev, (void*)st) != GF_OK)
-            return fail(ctx, GF_ERR_CUDA, "checksum kernel failed");
+            return fail(err, GF_ERR_CUDA, "checksum kernel failed");
         if (out->kind == GF_BUF_HOST) {                                                                              // opencl.rs:413
             nvtxRangePushA("gf_d2h_frame");
             cudaError_t e_d2h;
@@ -567,32 +543,33 @@ struct FrameRun {
                                                       (size_t)out->width * (size_t)ctx->combo.bpp(), (size_t)out->height, cudaMemcpyDeviceToHost, st);
             else            e_d2h = cudaMemcpyAsync(out->ptr, ctx->dst_stage.ptr, out->len, cudaMemcpyDeviceToHost, st);
             nvtxRangePop();
-            CK(e_d2h);
+            CK(err, e_d2h);
         }
-        if (job.sync_host && (in->kind == GF_BUF_HOST || out->kind == GF_BUF_HOST)) CK(cudaStreamSynchronize(st));
+        if (job.sync_host && (in->kind == GF_BUF_HOST || out->kind == GF_BUF_HOST)) CK(err, cudaStreamSynchronize(st));
         return GF_OK;
     }
 };
 
 int run_warp(gf_cuda_ctx* ctx, const FrameJob& job) {
     if (!ctx) return fail(nullptr, GF_ERR_BAD_PARAMS, "ctx is null");
+    std::string* const err = &ctx->last_error;
     const gf_kernel_params* p = job.p;
-    int rc = validate(ctx, p, job.in, job.out, ctx->combo.bpp());
+    int rc = validate(err, p, job.in, job.out, ctx->combo.bpp());
     if (rc != GF_OK) return rc;
-    if (!job.matrices) return fail(ctx, GF_ERR_NO_DATA, "NoStabilizationData: matrices is null");
+    if (!job.matrices) return fail(err, GF_ERR_NO_DATA, "NoStabilizationData: matrices is null");
     if (p->width != ctx->width || p->height != ctx->height || p->output_width != ctx->output_width || p->output_height != ctx->output_height)
-        return fail(ctx, GF_ERR_SIZE_MISMATCH, "SizeMismatch: KernelParams size differs from the size this context was created for");
+        return fail(err, GF_ERR_SIZE_MISMATCH, "SizeMismatch: KernelParams size differs from the size this context was created for");
     if (p->interpolation != ctx->interpolation)
-        return fail(ctx, GF_ERR_UNSUPPORTED_COMBO, "interpolation differs from the one this context was created for");
-    if ((size_t)p->matrix_count > job.matrix_rows) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices: matrix_count > rows supplied");
-    if (!job.tables_on_device && job.matrix_rows > ctx->max_rows) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices");
-    if (job.mesh_len > GF_MESH_MAX_LEN) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
-    if (job.mesh_len > 0 && !job.mesh) return fail(ctx, GF_ERR_BAD_PARAMS, "mesh is null");
-    if (job.mesh_len > 0 && job.mesh_len < 9) return fail(ctx, GF_ERR_BAD_PARAMS, "mesh shorter than its 9-value header (the reference would index out of bounds)");
-    if (job.in->kind == GF_BUF_HOST && job.in->len > ctx->src_stage.len)   return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input");
-    if (job.out->kind == GF_BUF_HOST && job.out->len > ctx->dst_stage.len) return fail(ctx, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch output");
-    if (job.tables_on_device && (reinterpret_cast<uintptr_t>(job.matrices) & 7u)) return fail(ctx, GF_ERR_BAD_PARAMS, "device matrices must be 8-byte aligned");
-    CK(cudaSetDevice(ctx->device));
+        return fail(err, GF_ERR_UNSUPPORTED_COMBO, "interpolation differs from the one this context was created for");
+    if ((size_t)p->matrix_count > job.matrix_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices: matrix_count > rows supplied");
+    if (!job.tables_on_device && job.matrix_rows > ctx->max_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices");
+    if (job.mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
+    if (job.mesh_len > 0 && !job.mesh) return fail(err, GF_ERR_BAD_PARAMS, "mesh is null");
+    if (job.mesh_len > 0 && job.mesh_len < 9) return fail(err, GF_ERR_BAD_PARAMS, "mesh shorter than its 9-value header (the reference would index out of bounds)");
+    if (job.in->kind == GF_BUF_HOST && job.in->len > ctx->src_stage.len)   return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input");
+    if (job.out->kind == GF_BUF_HOST && job.out->len > ctx->dst_stage.len) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch output");
+    if (job.tables_on_device && (reinterpret_cast<uintptr_t>(job.matrices) & 7u)) return fail(err, GF_ERR_BAD_PARAMS, "device matrices must be 8-byte aligned");
+    CK(err, cudaSetDevice(ctx->device));
     FrameRun F{ctx, job};
     ctx->last_stream = F.st;
     memset(&F.A, 0, sizeof(F.A));
@@ -640,15 +617,14 @@ extern "C" {
 GF_API int gf_cuda_device_count(void) {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess) { g_last_error = std::string("cudaGetDeviceCount: ") + cudaGetErrorString(e); (void)cudaGetLastError(); return 0; }
+    if (e != cudaSuccess) { cuda_error(e, "cudaGetDeviceCount", nullptr); return 0; }
     return n;
 }
 
 GF_API int gf_cuda_device_name(int device, char* buf, size_t buf_len) {
     if (!buf || buf_len == 0) return GF_ERR_BAD_PARAMS;
     cudaDeviceProp prop;
-    cudaError_t e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return fail(nullptr, GF_ERR_CUDA, std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e)); }
+    CK(nullptr, cudaGetDeviceProperties(&prop, device));
     snprintf(buf, buf_len, "[CUDA] %s", prop.name);      // listed like "[OpenCL] ..." / "[wgpu] ..." (stabilization/mod.rs:399-410)
     return GF_OK;
 }
@@ -693,57 +669,43 @@ GF_API int gf_cuda_create(gf_cuda_ctx** out_ctx, int device, const gf_kernel_par
     if (!combo.kernels[KV_GENERAL])
         return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "no kernel compiled for this (lens, digital lens, pixel type, interpolation)");
 
-    gf_cuda_ctx* ctx = new gf_cuda_ctx();
+    std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx(new gf_cuda_ctx());
     ctx->device = device; ctx->combo = combo; ctx->interpolation = params->interpolation;
     ctx->fn_shade = gf_shade_kernel(combo.layout);
     ctx->width = params->width; ctx->height = params->height; ctx->output_width = params->output_width; ctx->output_height = params->output_height;
-    auto bail = [&](int rc) { std::string m = ctx->last_error; gf_cuda_destroy(ctx); g_last_error = m; return rc; };
 
-    cudaError_t e = cudaSetDevice(device);
-    if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaSetDevice"); return bail(GF_ERR_CUDA); }
-    e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
-    if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaDeviceGetAttribute(multiprocessor count)"); return bail(GF_ERR_CUDA); }
-    e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) { cuda_fail(ctx, e, "cudaStreamCreate"); return bail(GF_ERR_CUDA); }
+    CK(nullptr, cudaSetDevice(device));
+    CK(nullptr, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
+    CK(nullptr, create_stream(ctx->stream));
+    const cudaStream_t st = ctx->stream.get();
     // matrices: 14 * max(W, H) f32 (rows = height, or width for horizontal rolling shutter) — opencl.rs:268, wgpu.rs:260
     size_t rows = (size_t)std::max(std::max(params->width, params->height), std::max(params->output_width, params->output_height));
     rows = std::max(rows, (size_t)params->matrix_count);
     ctx->max_rows = rows;
-    {
-        const uint32_t words[2] = { 0u, 1u };
-        if ((e = ctx->const_flags.reserve(2, ctx->stream)) != cudaSuccess ||
-            (e = cudaMemcpy(ctx->const_flags.ptr, words, sizeof(words), cudaMemcpyHostToDevice)) != cudaSuccess ||
-            (e = ctx->vflags.reserve(1, ctx->stream)) != cudaSuccess) { cuda_fail(ctx, e, "table-verdict words"); return bail(GF_ERR_CUDA); }
+    const uint32_t words[2] = { 0u, 1u };
+    CK(nullptr, ctx->const_flags.reserve(2, st));
+    CK(nullptr, cudaMemcpy(ctx->const_flags.ptr, words, sizeof(words), cudaMemcpyHostToDevice));
+    CK(nullptr, ctx->vflags.reserve(1, st));
+    for (Slot& sl : ctx->slots) {
+        CK(nullptr, sl.h_mat.reserve(rows * GF_MATRIX_STRIDE, st));
+        CK(nullptr, sl.d_mat.reserve(rows * GF_MATRIX_STRIDE, st));
+        CK(nullptr, sl.h_mesh.reserve(GF_MESH_MAX_LEN, st));
+        CK(nullptr, sl.d_mesh.reserve(GF_MESH_MAX_LEN, st));
+        CK(nullptr, sl.d_mesh64.reserve(GF_MESH_MAX_LEN + (sizeof(MeshAux) + 7) / 8, st));
+        CK(nullptr, create_event(sl.done));
     }
-    for (int s = 0; s < kSlots; ++s) {
-        Slot& sl = ctx->slots[s];
-        if ((e = sl.h_mat.reserve(rows * GF_MATRIX_STRIDE, ctx->stream)) != cudaSuccess || (e = sl.d_mat.reserve(rows * GF_MATRIX_STRIDE, ctx->stream)) != cudaSuccess ||
-            (e = sl.h_mesh.reserve(GF_MESH_MAX_LEN, ctx->stream)) != cudaSuccess || (e = sl.d_mesh.reserve(GF_MESH_MAX_LEN, ctx->stream)) != cudaSuccess ||
-            (e = sl.d_mesh64.reserve(GF_MESH_MAX_LEN + (sizeof(MeshAux) + 7) / 8, ctx->stream)) != cudaSuccess ||
-            (e = cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming)) != cudaSuccess) {
-            cuda_fail(ctx, e, "table staging allocation"); return bail(GF_ERR_CUDA);
-        }
-    }
-    if (in->kind == GF_BUF_HOST && (e = ctx->src_stage.reserve(in->len, ctx->stream)) != cudaSuccess)  { cuda_fail(ctx, e, "cudaMalloc(src staging)"); return bail(GF_ERR_CUDA); }
-    if (out->kind == GF_BUF_HOST && (e = ctx->dst_stage.reserve(out->len, ctx->stream)) != cudaSuccess) { cuda_fail(ctx, e, "cudaMalloc(dst staging)"); return bail(GF_ERR_CUDA); }
-    *out_ctx = ctx;
+    if (in->kind == GF_BUF_HOST) CK(nullptr, ctx->src_stage.reserve(in->len, st));
+    if (out->kind == GF_BUF_HOST) CK(nullptr, ctx->dst_stage.reserve(out->len, st));
+    *out_ctx = ctx.release();
     return GF_OK;
 }
 
 GF_API void gf_cuda_destroy(gf_cuda_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    for (Slot& sl : ctx->slots) {
-        sl.h_mat.release(); sl.d_mat.release(); sl.h_mesh.release(); sl.d_mesh.release(); sl.d_mesh64.release();
-        if (sl.done) cudaEventDestroy(sl.done);
-    }
-    ctx->src_stage.release(); ctx->dst_stage.release(); ctx->defer_q.release(); ctx->defer_count.release(); ctx->const_flags.release(); ctx->vflags.release();
-    for (size_t i = 0; i < ctx->plane_src.size(); ++i) { ctx->plane_src[i].release(); ctx->plane_dst[i].release(); }
-    ctx->h_drawing.release(); ctx->d_drawing.release(); ctx->src_ovl.release(); ctx->coords.release();
-    if (ctx->stream) cudaStreamDestroy(ctx->stream);
-    (void)cudaGetLastError();
+    if (ctx->stream) cudaStreamSynchronize(ctx->stream.get());
     delete ctx;
+    (void)cudaGetLastError();       // a failed teardown call must not fail the thread's next call
 }
 
 GF_API int gf_cuda_undistort_image(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out,
@@ -773,8 +735,7 @@ GF_API int gf_cuda_undistort_image_dev_flagged(gf_cuda_ctx* ctx, const gf_buffer
 GF_API int gf_cuda_scan_tables_dev(const float* matrices_dev, size_t matrix_rows, uint32_t* table_flags_dev, void* cu_stream) {
     if (!matrices_dev || !table_flags_dev || matrix_rows == 0) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
     scan_tables_kernel<<<1, 1024, 0, (cudaStream_t)cu_stream>>>(matrices_dev, matrix_rows, table_flags_dev);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(nullptr, e, "scan_tables_kernel");
+    CK(nullptr, cudaGetLastError());
     return GF_OK;
 }
 
@@ -862,22 +823,21 @@ GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_u
     gf_buffer_desc d; memset(&d, 0, sizeof(d));
     d.width = (int)new_w; d.height = (int)new_h; d.stride = (int)new_w; d.kind = GF_BUF_DEVICE;
     d.ptr = undist_rgb_dev; d.len = (size_t)new_w * (size_t)new_h;                          // never dereferenced in coordinate mode
-    gf_cuda_ctx* ctx = nullptr;
-    int device = 0; cudaGetDevice(&device);
-    rc = gf_cuda_create(&ctx, device, &kq, GF_PIX_LUMA8, distortion_model, digital_lens, &d, &d, 0);
-    if (rc != GF_OK) return rc;
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream;
-    FrameJob job{&d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};
-    job.coord_only = true;
-    rc = run_warp(ctx, job);
-    if (rc == GF_OK) {
+    {
+        gf_cuda_ctx* raw = nullptr;
+        int device = 0; cudaGetDevice(&device);
+        rc = gf_cuda_create(&raw, device, &kq, GF_PIX_LUMA8, distortion_model, digital_lens, &d, &d, 0);
+        if (rc != GF_OK) return rc;
+        const std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx(raw);
+        cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
+        FrameJob job{&d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};
+        job.coord_only = true;
+        if ((rc = run_warp(ctx.get(), job)) != GF_OK) return rc;
         const dim3 block(32, 8), grid(((unsigned)new_w + 31) / 32, ((unsigned)new_h + 7) / 8);
         stmap_rgb_kernel<<<grid, block, 0, st>>>(ctx->coords.ptr, (int)new_w, (int)new_h, (int)new_w, undist_rgb_dev);
-        if (cudaGetLastError() != cudaSuccess) rc = GF_ERR_CUDA;
+        CK(nullptr, cudaGetLastError());
+        CK(nullptr, cudaStreamSynchronize(st));
     }
-    if (rc == GF_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = GF_ERR_CUDA;
-    gf_cuda_destroy(ctx);
-    if (rc != GF_OK) return rc;
 
     cp.width = width; cp.height = height; cp.output_width = width; cp.output_height = height;   // :111-112 (fov_scale stays)
     rc = gf_cuda_stmap_distort_dev(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, dist_rgb_dev, cu_stream);
@@ -893,10 +853,10 @@ GF_API int gf_cuda_undistort_planes_dev(gf_cuda_ctx* ctx, size_t n_planes, const
 GF_API int gf_cuda_undistort_planes_dev_flagged(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                                 const gf_kernel_params* params, const float* matrices_dev, size_t matrix_rows,
                                                 const float* mesh_dev, size_t mesh_len, const uint32_t* table_flags_dev, void* cu_stream) {
-    if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx, GF_ERR_BAD_PARAMS, "null argument");
+    if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
     for (size_t i = 0; i < n_planes; ++i) {
-        if (in[i].kind != GF_BUF_DEVICE || out[i].kind != GF_BUF_DEVICE) return fail(ctx, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes_dev takes DEVICE buffers");
-        int rc = validate(ctx, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
+        if (in[i].kind != GF_BUF_DEVICE || out[i].kind != GF_BUF_DEVICE) return fail(&ctx->last_error, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes_dev takes DEVICE buffers");
+        int rc = validate(&ctx->last_error, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
     }
     FrameJob job{in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
     job.tables_on_device = true; job.table_flags_dev = table_flags_dev;
@@ -909,29 +869,30 @@ GF_API int gf_cuda_undistort_planes_dev_flagged(gf_cuda_ctx* ctx, size_t n_plane
 GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                     const gf_kernel_params* params, const float* matrices, size_t matrix_rows,
                                     const float* mesh, size_t mesh_len, void* cu_stream) {
-    if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx, GF_ERR_BAD_PARAMS, "null argument");
+    if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    std::string* const err = &ctx->last_error;
     for (size_t i = 0; i < n_planes; ++i) {
-        if (in[i].kind != GF_BUF_HOST || out[i].kind != GF_BUF_HOST) return fail(ctx, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes takes HOST buffers (DEVICE: gf_cuda_undistort_planes_dev)");
-        int rc = validate(ctx, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
+        if (in[i].kind != GF_BUF_HOST || out[i].kind != GF_BUF_HOST) return fail(err, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes takes HOST buffers (DEVICE: gf_cuda_undistort_planes_dev)");
+        int rc = validate(err, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
     }
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream;
+    CK(err, cudaSetDevice(ctx->device));
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
     ctx->last_stream = st;
     if (ctx->plane_src.size() < n_planes) { ctx->plane_src.resize(n_planes); ctx->plane_dst.resize(n_planes); }
     std::vector<gf_buffer_desc> din(in, in + n_planes), dout(out, out + n_planes);
     for (size_t i = 0; i < n_planes; ++i) {
-        CK(ctx->plane_src[i].reserve(in[i].len, st));
-        CK(ctx->plane_dst[i].reserve(out[i].len, st));
-        CK(cudaMemcpyAsync(ctx->plane_src[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ctx->plane_dst[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));   // untouched pixels keep their content, like on the CPU path
+        CK(err, ctx->plane_src[i].reserve(in[i].len, st));
+        CK(err, ctx->plane_dst[i].reserve(out[i].len, st));
+        CK(err, cudaMemcpyAsync(ctx->plane_src[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
+        CK(err, cudaMemcpyAsync(ctx->plane_dst[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));   // untouched pixels keep their content, like on the CPU path
         din[i].kind = GF_BUF_DEVICE; din[i].ptr = ctx->plane_src[i].ptr;
         dout[i].kind = GF_BUF_DEVICE; dout[i].ptr = ctx->plane_dst[i].ptr;
     }
     FrameJob job{din.data(), dout.data(), params, matrices, matrix_rows, mesh, mesh_len, (void*)st};
     job.sync_host = false;
     { int rc = run_planes(ctx, n_planes, din.data(), dout.data(), params, job); if (rc != GF_OK) return rc; }
-    for (size_t i = 0; i < n_planes; ++i) CK(cudaMemcpyAsync(out[i].ptr, ctx->plane_dst[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    for (size_t i = 0; i < n_planes; ++i) CK(err, cudaMemcpyAsync(out[i].ptr, ctx->plane_dst[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
+    CK(err, cudaStreamSynchronize(st));
     return GF_OK;
 }
 
@@ -959,25 +920,27 @@ GF_API int gf_cuda_plan(const gf_kernel_params* params, int pixel_type, int dist
 }
 
 GF_API int gf_cuda_validate_tables_dev(gf_cuda_ctx* ctx, const float* matrices_dev, size_t matrix_rows) {
-    if (!ctx || !matrices_dev) return fail(ctx, GF_ERR_BAD_PARAMS, "null argument");
-    CK(cudaSetDevice(ctx->device));
+    if (!ctx || !matrices_dev) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    std::string* const err = &ctx->last_error;
+    CK(err, cudaSetDevice(ctx->device));
     // A synchronous QUERY: nothing is cached.  (Round 1 kept a pointer-keyed cache of verdicts; a table rewritten in place or an
     // allocation reused at the same address was then silently trusted.)  To render device tables on the trusted path pass a verdict
     // word to gf_cuda_undistort_image_dev_flagged — written by gf_cuda_scan_tables_dev or by gf_cuda_frame_transform_dev.
-    CK(cudaDeviceSynchronize());                               // the table may have been written on any stream
-    scan_tables_kernel<<<1, 1024, 0, ctx->stream>>>(matrices_dev, matrix_rows, ctx->vflags.ptr);
-    CK(cudaGetLastError());
+    CK(err, cudaDeviceSynchronize());                               // the table may have been written on any stream
+    scan_tables_kernel<<<1, 1024, 0, ctx->stream.get()>>>(matrices_dev, matrix_rows, ctx->vflags.ptr);
+    CK(err, cudaGetLastError());
     uint32_t f = 0;
-    CK(cudaMemcpyAsync(&f, ctx->vflags.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    CK(err, cudaMemcpyAsync(&f, ctx->vflags.ptr, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream.get()));
+    CK(err, cudaStreamSynchronize(ctx->stream.get()));
     return (int)f;      // 0 = tame and IBIS-free; bit 0 = wild entry, bit 1 = IBIS rows present (both still render correctly, on the guarded path)
 }
 
 GF_API int gf_cuda_synchronize(gf_cuda_ctx* ctx) {
     if (!ctx) return fail(nullptr, GF_ERR_BAD_PARAMS, "ctx is null");
-    CK(cudaSetDevice(ctx->device));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (ctx->last_stream && ctx->last_stream != ctx->stream) CK(cudaStreamSynchronize(ctx->last_stream));   // calls made with a caller-supplied stream
+    std::string* const err = &ctx->last_error;
+    CK(err, cudaSetDevice(ctx->device));
+    CK(err, cudaStreamSynchronize(ctx->stream.get()));
+    if (ctx->last_stream && ctx->last_stream != ctx->stream.get()) CK(err, cudaStreamSynchronize(ctx->last_stream));   // calls made with a caller-supplied stream
     return GF_OK;
 }
 

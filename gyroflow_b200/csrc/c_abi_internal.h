@@ -1,12 +1,73 @@
 // c_abi_internal.h — entry points shared between the translation units of libgyroflow_cuda.so, NOT exported
 // (the library is built with -fvisibility=hidden; only GF_API symbols leave it).
 #pragma once
+#include <cuda_runtime.h>
 #include <cstddef>
 #include <cstdint>
+#include <memory>
+#include <string>
 #include "../../include/gyroflow_cuda.h"
 #include "frame_geometry.cuh"
 
 namespace gf {
+
+// ---- Errors: every entry point reports a failure through these ----
+
+// The calling thread's last error message (gf_cuda_last_error(NULL)).
+inline thread_local std::string g_last_error;
+
+// `msg` becomes the thread's last error and, when `sink` is given, the message of the context or queue the failure belongs to.
+inline int fail(std::string* sink, int code, const std::string& msg) {
+    g_last_error = msg;
+    if (sink) *sink = msg;
+    return code;
+}
+// A failed CUDA call: clears the runtime's pending error, so that the thread's next call does not fail on it, and reports
+// "what: name (description)".
+inline int cuda_error(cudaError_t e, const char* what, std::string* sink) {
+    (void)cudaGetLastError();
+    return fail(sink, GF_ERR_CUDA, std::string(what) + ": " + cudaGetErrorName(e) + " (" + cudaGetErrorString(e) + ")");
+}
+#define CK(sink, call) do { const cudaError_t e_ = (call); if (e_ != cudaSuccess) return gf::cuda_error(e_, #call, sink); } while (0)
+
+// ---- Owners: each CUDA resource is released by the object that holds it ----
+// The objects the entry points hand out (contexts, queues, gyro uploads) are torn down by setting their device, synchronising their
+// streams and deleting them: the members' destructors must not free what queued work may still use.
+
+// A device buffer (PINNED: page-locked host memory) of `len` elements that grows on demand.  Growing waits for the stream, whose queued
+// work may still use the old buffer, frees it and allocates the new size; on an empty buffer reserve is a plain allocation.
+template <class T, bool PINNED = false> struct GrowBuf {
+    T* ptr = nullptr; size_t len = 0;
+    GrowBuf() = default;
+    GrowBuf(GrowBuf&& o) noexcept : ptr(o.ptr), len(o.len) { o.ptr = nullptr; o.len = 0; }
+    ~GrowBuf() { release(); }
+    cudaError_t reserve(size_t n, cudaStream_t st) {
+        if (n <= len) return cudaSuccess;
+        if (ptr) { const cudaError_t e = cudaStreamSynchronize(st); if (e != cudaSuccess) return e; release(); }
+        const cudaError_t e = PINNED ? cudaMallocHost((void**)&ptr, n * sizeof(T)) : cudaMalloc((void**)&ptr, n * sizeof(T));
+        if (e == cudaSuccess) len = n; else ptr = nullptr;
+        return e;
+    }
+private:
+    void release() { if (ptr) { if (PINNED) cudaFreeHost(ptr); else cudaFree(ptr); } ptr = nullptr; len = 0; }
+};
+
+// unique_ptr deleter calling `Destroy` (cudaStreamDestroy, gf_cuda_destroy, ...)
+template <auto Destroy> struct Deleter { template <class T> void operator()(T* h) const { Destroy(h); } };
+using Stream = std::unique_ptr<CUstream_st, Deleter<cudaStreamDestroy>>;
+using Event = std::unique_ptr<CUevent_st, Deleter<cudaEventDestroy>>;
+inline cudaError_t create_stream(Stream& s) {
+    cudaStream_t h = nullptr;
+    const cudaError_t e = cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking);
+    if (e == cudaSuccess) s.reset(h);
+    return e;
+}
+inline cudaError_t create_event(Event& ev) {
+    cudaEvent_t h = nullptr;
+    const cudaError_t e = cudaEventCreateWithFlags(&h, cudaEventDisableTiming);
+    if (e == cudaSuccess) ev.reset(h);
+    return e;
+}
 
 // Trust verdict of a matrix table (rows of GF_MATRIX_STRIDE floats), as the packed warp kernel wants it: 0 = trusted, TBL_WILD = an
 // entry of columns 0-8 is not tame (below), TBL_IBIS = an entry of columns 9-13 (IBIS / OIS shifts) is non-zero.

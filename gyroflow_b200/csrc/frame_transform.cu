@@ -283,6 +283,12 @@ Spline3 stab_spline(const double* pos, const double* xyz, size_t n) {
     return Spline3{ pos, xyz, (pos && xyz) ? n : 0 };
 }
 
+// a device copy of n host values, into an empty buffer
+template <class T> cudaError_t upload(GrowBuf<T>& d, const T* h, size_t n) {
+    const cudaError_t e = d.reserve(n, nullptr);
+    return e == cudaSuccess ? cudaMemcpy(d.ptr, h, n * sizeof(T), cudaMemcpyHostToDevice) : e;
+}
+
 } // namespace
 
 #include "gyro_dev.h"
@@ -323,26 +329,23 @@ GF_API uint32_t gf_table_flags_host(const float* matrices, size_t rows) {
 GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_params* cp) {
     if (!out || !cp || !cp->org.ts_us || !cp->org.quats) return GF_ERR_BAD_PARAMS;
     *out = nullptr;
-    if (cudaSetDevice(device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
-    gf_cuda_gyro* g = new gf_cuda_gyro();
+    CK(nullptr, cudaSetDevice(device));
+    std::unique_ptr<gf_cuda_gyro, Deleter<gf_cuda_gyro_free>> g(new gf_cuda_gyro());
     g->device = device; g->n_org = cp->org.n;
-    bool ok = cudaMalloc(&g->d_org_ts, cp->org.n * sizeof(int64_t)) == cudaSuccess &&
-              cudaMalloc(&g->d_org_q, cp->org.n * 4 * sizeof(double)) == cudaSuccess &&
-              cudaMemcpy(g->d_org_ts, cp->org.ts_us, cp->org.n * sizeof(int64_t), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaMemcpy(g->d_org_q, cp->org.quats, cp->org.n * 4 * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess &&
-              cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaMalloc(&g->d_scratch, 2 * gf_cuda_gyro::kScratchPairs * sizeof(unsigned)) == cudaSuccess &&
-              cudaMemset(g->d_scratch, 0, 2 * gf_cuda_gyro::kScratchPairs * sizeof(unsigned)) == cudaSuccess;
+    CK(nullptr, upload(g->d_org_ts, cp->org.ts_us, cp->org.n));
+    CK(nullptr, upload(g->d_org_q, cp->org.quats, cp->org.n * 4));
+    CK(nullptr, create_stream(g->stream));
+    CK(nullptr, g->d_scratch.reserve(2 * gf_cuda_gyro::kScratchPairs, nullptr));
+    CK(nullptr, cudaMemset(g->d_scratch.ptr, 0, 2 * gf_cuda_gyro::kScratchPairs * sizeof(unsigned)));
     // multi-point sync offsets (offsets_adjusted) ride along with the tracks
     const SyncOffsets ho = host_offsets_of(cp);
-    if (ok && ho.n > 0) {
+    if (ho.n > 0) {
         g->n_offsets = ho.n;
-        ok = cudaMalloc(&g->d_off_ts, ho.n * sizeof(int64_t)) == cudaSuccess && cudaMalloc(&g->d_off_ms, ho.n * sizeof(double)) == cudaSuccess &&
-             cudaMemcpy(g->d_off_ts, ho.ts, ho.n * sizeof(int64_t), cudaMemcpyHostToDevice) == cudaSuccess &&
-             cudaMemcpy(g->d_off_ms, ho.ms, ho.n * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
+        CK(nullptr, upload(g->d_off_ts, ho.ts, ho.n));
+        CK(nullptr, upload(g->d_off_ms, ho.ms, ho.n));
     }
     // per-frame IBIS / OIS spline points (camera_stab_data): one flat device array + per-frame offsets kept on the host
-    if (ok && cp->camera_stab && cp->n_camera_stab > 0) {
+    if (cp->camera_stab && cp->n_camera_stab > 0) {
         std::vector<double> flat;
         g->stab_index.resize(cp->n_camera_stab);
         for (size_t f = 0; f < cp->n_camera_stab; ++f) {
@@ -354,12 +357,10 @@ GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_
             ix.ois_pos = flat.size();  flat.insert(flat.end(), is.ois_pos, is.ois_pos + ix.n_ois);
             ix.ois_val = flat.size();  flat.insert(flat.end(), is.ois_xyz, is.ois_xyz + 3 * ix.n_ois);
         }
-        if (!flat.empty())
-            ok = cudaMalloc(&g->d_stab, flat.size() * sizeof(double)) == cudaSuccess &&
-                 cudaMemcpy(g->d_stab, flat.data(), flat.size() * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
+        if (!flat.empty()) CK(nullptr, upload(g->d_stab, flat.data(), flat.size()));
     }
     // per-frame distorting meshes of the point path (mesh_correction[frame].0)
-    if (ok && cp->distorting_mesh && cp->n_distorting_mesh > 0) {
+    if (cp->distorting_mesh && cp->n_distorting_mesh > 0) {
         std::vector<double> flat;
         g->mesh_index.resize(cp->n_distorting_mesh);
         for (size_t f = 0; f < cp->n_distorting_mesh; ++f) {
@@ -369,29 +370,18 @@ GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_
             if (m.data) flat.insert(flat.end(), m.data, m.data + m.len);
             if (ix.len >= 9) memcpy(ix.header, m.data, sizeof(ix.header));
         }
-        if (!flat.empty())
-            ok = cudaMalloc(&g->d_mesh, flat.size() * sizeof(double)) == cudaSuccess &&
-                 cudaMemcpy(g->d_mesh, flat.data(), flat.size() * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
+        if (!flat.empty()) CK(nullptr, upload(g->d_mesh, flat.data(), flat.size()));
     }
-    if (!ok) { (void)cudaGetLastError(); gf_cuda_gyro_free(g); return GF_ERR_CUDA; }
-    *out = g;
+    *out = g.release();
     return GF_OK;
 }
 
 GF_API void gf_cuda_gyro_free(gf_cuda_gyro* g) {
     if (!g) return;
     cudaSetDevice(g->device);
-    if (g->stream) cudaStreamSynchronize(g->stream);
-    if (g->d_org_ts) cudaFree(g->d_org_ts);
-    if (g->d_org_q) cudaFree(g->d_org_q);
-    if (g->d_off_ts) cudaFree(g->d_off_ts);
-    if (g->d_off_ms) cudaFree(g->d_off_ms);
-    if (g->d_stab) cudaFree(g->d_stab);
-    if (g->d_mesh) cudaFree(g->d_mesh);
-    if (g->d_scratch) cudaFree(g->d_scratch);
-    if (g->stream) cudaStreamDestroy(g->stream);
-    (void)cudaGetLastError();
+    if (g->stream) cudaStreamSynchronize(g->stream.get());
     delete g;
+    (void)cudaGetLastError();       // a failed teardown call must not fail the thread's next call
 }
 
 // `table_flags_dev` (nullable): receives the table's trust verdict on the same stream (see gf_cuda_undistort_image_dev_flagged).
@@ -402,7 +392,7 @@ GF_API int gf_cuda_frame_transform_dev_flagged(gf_cuda_gyro* g, const gf_compute
                                                gf_kernel_params* out_params, float* matrices_dev, size_t max_rows, uint32_t* table_flags_dev,
                                                size_t* out_rows, double* out_fov, double* out_minimal_fov, void* cu_stream) {
     if (!g || !cp || !matrices_dev) return GF_ERR_BAD_PARAMS;
-    if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(g->device));
     RowCtx C;
     // the two per-frame lookups (org(ts), smoothed(ts)) stay on the host: O(log n) each; the per-row ones run on the device
     StabSplines sp;
@@ -412,11 +402,11 @@ GF_API int gf_cuda_frame_transform_dev_flagged(gf_cuda_gyro* g, const gf_compute
     if (rows > max_rows) return GF_ERR_BUFFER_TOO_SMALL;
     C.org = g->org_track();
     C.offsets = g->sync_offsets(cp->gyro_offset_ms);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
-    unsigned* scratch = g->d_scratch + 2u * (g->next_scratch++ % gf_cuda_gyro::kScratchPairs);     // self-cleaning: the last block re-arms it
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    unsigned* scratch = g->d_scratch.ptr + 2u * (g->next_scratch++ % gf_cuda_gyro::kScratchPairs);     // self-cleaning: the last block re-arms it
     frame_rows_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(C, rows, matrices_dev, table_flags_dev, scratch);
-    if (cudaGetLastError() != cudaSuccess) return GF_ERR_CUDA;
-    if (!cu_stream && cudaStreamSynchronize(st) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaGetLastError());
+    if (!cu_stream) CK(nullptr, cudaStreamSynchronize(st));
     return GF_OK;
 }
 

@@ -5,39 +5,40 @@
 #include <cstddef>
 #include <vector>
 #include "frame_geometry.cuh"
+#include "c_abi_internal.h"
 
 struct gf_cuda_gyro {
     int device = 0;
-    int64_t* d_org_ts = nullptr; double* d_org_q = nullptr; size_t n_org = 0;       // quaternions (org track)
-    int64_t* d_off_ts = nullptr; double* d_off_ms = nullptr; size_t n_offsets = 0;  // offsets_adjusted (multi-point sync), may be empty
-    double* d_stab = nullptr;                                                       // IBIS / OIS spline points of every frame, flat
+    gf::GrowBuf<int64_t> d_org_ts; gf::GrowBuf<double> d_org_q; size_t n_org = 0;       // quaternions (org track)
+    gf::GrowBuf<int64_t> d_off_ts; gf::GrowBuf<double> d_off_ms; size_t n_offsets = 0;  // offsets_adjusted (multi-point sync), may be empty
+    gf::GrowBuf<double> d_stab;                                                         // IBIS / OIS spline points of every frame, flat
     struct StabIndex { size_t ibis_pos, ibis_val, n_ibis, ois_pos, ois_val, n_ois; };
-    std::vector<StabIndex> stab_index;                                              // offsets into d_stab per frame
-    double* d_mesh = nullptr;                                                       // distorting meshes of every frame (point path), flat
+    std::vector<StabIndex> stab_index;                                                  // offsets into d_stab per frame
+    gf::GrowBuf<double> d_mesh;                                                         // distorting meshes of every frame (point path), flat
     struct MeshIndex { size_t off, len; double header[9]; };                       // header: host copy of the mesh's first 9 values
     std::vector<MeshIndex> mesh_index;
     // verdict accumulator + ticket of frame_rows_kernel: a pool of pairs handed out round-robin, so that producer launches that overlap
     // on different streams (the render queue's slots) never share one
     static constexpr unsigned kScratchPairs = 64;
-    unsigned* d_scratch = nullptr; unsigned next_scratch = 0;
-    cudaStream_t stream = nullptr;
+    gf::GrowBuf<unsigned> d_scratch; unsigned next_scratch = 0;
+    gf::Stream stream;
 
-    gf::Track org_track() const { return gf::Track{ d_org_ts, d_org_q, n_org }; }
+    gf::Track org_track() const { return gf::Track{ d_org_ts.ptr, d_org_q.ptr, n_org }; }
     // the uploaded multi-point sync offsets; `scalar_ms` (gyro_offset_ms) applies when there are none
-    gf::SyncOffsets sync_offsets(double scalar_ms) const { return gf::SyncOffsets{ d_off_ts, d_off_ms, n_offsets, scalar_ms }; }
+    gf::SyncOffsets sync_offsets(double scalar_ms) const { return gf::SyncOffsets{ d_off_ts.ptr, d_off_ms.ptr, n_offsets, scalar_ms }; }
     // this frame's IBIS / OIS spline points; false when the upload had no camera_stab entry for it
     bool frame_splines(size_t frame, gf::StabSplines& s) const {
         if (frame >= stab_index.size()) return false;
         const StabIndex& ix = stab_index[frame];
-        s.ibis = gf::Spline3{ d_stab + ix.ibis_pos, d_stab + ix.ibis_val, ix.n_ibis };
-        s.ois  = gf::Spline3{ d_stab + ix.ois_pos,  d_stab + ix.ois_val,  ix.n_ois };
+        s.ibis = gf::Spline3{ d_stab.ptr + ix.ibis_pos, d_stab.ptr + ix.ibis_val, ix.n_ibis };
+        s.ois  = gf::Spline3{ d_stab.ptr + ix.ois_pos,  d_stab.ptr + ix.ois_val,  ix.n_ois };
         return true;
     }
     // this frame's distorting mesh (mesh_correction[frame].0) and its length, or nullptr when it has none of more than 9 values
     const double* frame_mesh(size_t frame, uint32_t& len) const {
         len = 0;
-        if (!d_mesh || frame >= mesh_index.size() || mesh_index[frame].len <= 9) return nullptr;
+        if (!d_mesh.ptr || frame >= mesh_index.size() || mesh_index[frame].len <= 9) return nullptr;
         len = (uint32_t)mesh_index[frame].len;
-        return d_mesh + mesh_index[frame].off;
+        return d_mesh.ptr + mesh_index[frame].off;
     }
 };

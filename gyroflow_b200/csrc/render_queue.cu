@@ -24,16 +24,18 @@
 #include "../../include/gyroflow_cuda.h"
 #include "c_abi_internal.h"
 
+using namespace gf;
+
 namespace {
 
 struct QSlot {
-    gf_cuda_ctx* ctx = nullptr;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t done = nullptr;
-    float* d_mat = nullptr;
-    uint32_t* d_flags = nullptr;
-    float* h_mesh = nullptr; float* d_mesh = nullptr;      // per-frame mesh staging (pinned / device)
-    uint64_t* d_sum = nullptr; uint64_t* h_sum = nullptr;  // checksum (device word, pinned host copy)
+    std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx;
+    Stream stream;
+    Event done;
+    GrowBuf<float> d_mat;
+    GrowBuf<uint32_t> d_flags;
+    GrowBuf<float, true> h_mesh; GrowBuf<float> d_mesh;      // per-frame mesh staging (pinned / device)
+    GrowBuf<uint64_t> d_sum; GrowBuf<uint64_t, true> h_sum;  // checksum (device word, pinned host copy)
     bool busy = false;
     size_t frame = 0;
 };
@@ -53,7 +55,7 @@ __global__ void checksum_kernel(const uint32_t* __restrict__ w, size_t n, unsign
 struct gf_cuda_queue {
     gf_queue_config cfg;
     gf_compute_params cp;                 // shallow copy: the arrays it points to stay owned by the caller for the queue's lifetime
-    gf_cuda_gyro* gyro = nullptr;
+    std::unique_ptr<gf_cuda_gyro, Deleter<gf_cuda_gyro_free>> gyro;
     std::vector<QSlot> slots;
     std::deque<int> fifo;                 // slots in submission order
     int next = 0;
@@ -63,15 +65,9 @@ struct gf_cuda_queue {
 };
 
 namespace {
-int qfail(gf_cuda_queue* q, int code, const std::string& msg) { if (q) q->last_error = msg; return code; }
-int qcuda(gf_cuda_queue* q, cudaError_t e, const char* what) {
-    return qfail(q, GF_ERR_CUDA, std::string(what) + ": " + cudaGetErrorName(e) + " (" + cudaGetErrorString(e) + ")");
-}
-#define QCK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return qcuda(q, e_, #call); } while (0)
-
 int finish_slot(gf_cuda_queue* q, QSlot& s) {
     if (!s.busy) return GF_OK;
-    QCK(cudaEventSynchronize(s.done));
+    CK(&q->last_error, cudaEventSynchronize(s.done.get()));
     s.busy = false;
     return GF_OK;
 }
@@ -81,7 +77,7 @@ extern "C" {
 
 GF_API int gf_cuda_bind_thread_to_device(int device) {
     char bdf[32] = {0};
-    if (cudaDeviceGetPCIBusId(bdf, sizeof(bdf), device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaDeviceGetPCIBusId(bdf, sizeof(bdf), device));
     for (char* c = bdf; *c; ++c) if (*c >= 'A' && *c <= 'F') *c = (char)(*c - 'A' + 'a');      // sysfs uses lower-case hex
     char path[128];
     snprintf(path, sizeof(path), "/sys/bus/pci/devices/%s/local_cpulist", bdf);
@@ -120,23 +116,21 @@ GF_API int gf_cuda_host_register(void* ptr, size_t len) {
     if (!ptr || !len) return GF_ERR_BAD_PARAMS;
     const cudaError_t e = cudaHostRegister(ptr, len, cudaHostRegisterPortable);
     if (e == cudaErrorHostMemoryAlreadyRegistered) { (void)cudaGetLastError(); return GF_OK; }
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
-    return GF_OK;
+    return e == cudaSuccess ? GF_OK : cuda_error(e, "cudaHostRegister", nullptr);
 }
 GF_API int gf_cuda_host_unregister(void* ptr) {
     if (!ptr) return GF_ERR_BAD_PARAMS;
-    const cudaError_t e = cudaHostUnregister(ptr);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaHostUnregister(ptr));
     return GF_OK;
 }
 
 GF_API int gf_cuda_checksum_dev(const void* ptr_dev, size_t len, uint64_t* out_dev, void* cu_stream) {
     if (!ptr_dev || !out_dev) return GF_ERR_BAD_PARAMS;
     cudaStream_t st = (cudaStream_t)cu_stream;
-    if (cudaMemsetAsync(out_dev, 0, sizeof(uint64_t), st) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaMemsetAsync(out_dev, 0, sizeof(uint64_t), st));
     const size_t n = len / 4;
     if (n) checksum_kernel<<<132 * 4, 256, 0, st>>>(reinterpret_cast<const uint32_t*>(ptr_dev), n, reinterpret_cast<unsigned long long*>(out_dev));
-    if (cudaGetLastError() != cudaSuccess) return GF_ERR_CUDA;
+    CK(nullptr, cudaGetLastError());
     return GF_OK;
 }
 
@@ -145,73 +139,78 @@ GF_API int gf_cuda_queue_create(gf_cuda_queue** out, const gf_queue_config* cfg,
     if (!out || !cfg || !cp || !in_proto || !out_proto) return GF_ERR_BAD_PARAMS;
     *out = nullptr;
     if (cfg->depth < 1 || cfg->depth > 16) return GF_ERR_BAD_PARAMS;
-    gf_cuda_queue* q = new gf_cuda_queue();
+    std::unique_ptr<gf_cuda_queue, Deleter<gf_cuda_queue_destroy>> q(new gf_cuda_queue());
     q->cfg = *cfg; q->cp = *cp;
-    auto bail = [&](int rc) { gf_cuda_queue_destroy(q); return rc; };
-    if (cudaSetDevice(cfg->device) != cudaSuccess) { (void)cudaGetLastError(); return bail(GF_ERR_CUDA); }
+    CK(nullptr, cudaSetDevice(cfg->device));
     if (cfg->pin_numa) (void)gf_cuda_bind_thread_to_device(cfg->device);      // before any page-locked staging is allocated
-    int rc = gf_cuda_gyro_upload(&q->gyro, cfg->device, cp);
-    if (rc != GF_OK) return bail(rc);
+    gf_cuda_gyro* gyro = nullptr;
+    int rc = gf_cuda_gyro_upload(&gyro, cfg->device, cp);
+    if (rc != GF_OK) return rc;
+    q->gyro.reset(gyro);
     // a template KernelParams good enough for gf_cuda_create's validation (sizes, strides, interpolation, pixel size)
     gf_kernel_params kp; memset(&kp, 0, sizeof(kp));
     kp.matrix_count = 1;
     rc = gf_get_frame_transform_at(&cfg->stab, cp, in_proto, out_proto, nullptr, 0, 0.0, 0, 1.0, &kp);
-    if (rc != GF_OK) return bail(rc);
+    if (rc != GF_OK) return rc;
     q->max_rows = (size_t)(cp->width > cp->height ? cp->width : cp->height);
     q->slots.resize((size_t)cfg->depth);
     for (QSlot& s : q->slots) {
-        rc = gf_cuda_create(&s.ctx, cfg->device, &kp, cfg->stab.pixel_type, cfg->distortion_model, cfg->digital_lens, in_proto, out_proto, 0);
-        if (rc != GF_OK) { q->last_error = gf_cuda_last_error(nullptr); return bail(rc); }
-        cudaError_t e;
-        if ((e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking)) != cudaSuccess ||
-            (e = cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming)) != cudaSuccess ||
-            (e = cudaMalloc(&s.d_mat, q->max_rows * GF_MATRIX_STRIDE * sizeof(float))) != cudaSuccess ||
-            (e = cudaMalloc(&s.d_flags, sizeof(uint32_t))) != cudaSuccess ||
-            (e = cudaMallocHost(&s.h_mesh, GF_MESH_MAX_LEN * sizeof(float))) != cudaSuccess ||
-            (e = cudaMalloc(&s.d_mesh, GF_MESH_MAX_LEN * sizeof(float))) != cudaSuccess ||
-            (e = cudaMalloc(&s.d_sum, sizeof(uint64_t))) != cudaSuccess ||
-            (e = cudaMallocHost(&s.h_sum, sizeof(uint64_t))) != cudaSuccess) { qcuda(q, e, "queue slot allocation"); return bail(GF_ERR_CUDA); }
-        *s.h_sum = 0;
+        gf_cuda_ctx* ctx = nullptr;
+        rc = gf_cuda_create(&ctx, cfg->device, &kp, cfg->stab.pixel_type, cfg->distortion_model, cfg->digital_lens, in_proto, out_proto, 0);
+        if (rc != GF_OK) return rc;
+        s.ctx.reset(ctx);
+        CK(nullptr, create_stream(s.stream));
+        CK(nullptr, create_event(s.done));
+        const cudaStream_t st = s.stream.get();
+        CK(nullptr, s.d_mat.reserve(q->max_rows * GF_MATRIX_STRIDE, st));
+        CK(nullptr, s.d_flags.reserve(1, st));
+        CK(nullptr, s.h_mesh.reserve(GF_MESH_MAX_LEN, st));
+        CK(nullptr, s.d_mesh.reserve(GF_MESH_MAX_LEN, st));
+        CK(nullptr, s.d_sum.reserve(1, st));
+        CK(nullptr, s.h_sum.reserve(1, st));
+        *s.h_sum.ptr = 0;
     }
-    *out = q;
+    *out = q.release();
     return GF_OK;
 }
 
 GF_API int gf_cuda_queue_submit(gf_cuda_queue* q, size_t frame, double timestamp_ms, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                 const float* mesh, size_t mesh_len) {
-    if (!q || !in || !out) return qfail(q, GF_ERR_BAD_PARAMS, "null argument");
-    if (mesh_len > GF_MESH_MAX_LEN) return qfail(q, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
-    QCK(cudaSetDevice(q->cfg.device));
+    if (!q || !in || !out) return fail(q ? &q->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    std::string* const err = &q->last_error;
+    if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
+    CK(err, cudaSetDevice(q->cfg.device));
     QSlot& s = q->slots[(size_t)q->next];
-    if (s.busy) return qfail(q, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
+    if (s.busy) return fail(err, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
+    const cudaStream_t st = s.stream.get();
     nvtxRangePushA("gf_queue_submit");
     // FrameTransform::at_timestamp on the device: rows x 14 table + its trust verdict, then the per-buffer half of KernelParams
     gf_kernel_params kp; size_t rows = 0; double fov = 1.0, minimal_fov = 1.0;
-    int rc = gf_cuda_frame_transform_dev_flagged(q->gyro, &q->cp, timestamp_ms, frame, &kp, s.d_mat, q->max_rows, s.d_flags,
-                                                 &rows, &fov, &minimal_fov, (void*)s.stream);
-    if (rc != GF_OK) { nvtxRangePop(); return qfail(q, rc, "gf_cuda_frame_transform_dev_flagged failed"); }
+    int rc = gf_cuda_frame_transform_dev_flagged(q->gyro.get(), &q->cp, timestamp_ms, frame, &kp, s.d_mat.ptr, q->max_rows, s.d_flags.ptr,
+                                                 &rows, &fov, &minimal_fov, (void*)st);
+    if (rc != GF_OK) { nvtxRangePop(); return fail(err, rc, "gf_cuda_frame_transform_dev_flagged failed"); }
     q->launches++;
     rc = gf_get_frame_transform_at(&q->cfg.stab, &q->cp, in, out, mesh, mesh_len, timestamp_ms, frame, minimal_fov, &kp);
-    if (rc != GF_OK) { nvtxRangePop(); return qfail(q, rc, "gf_get_frame_transform_at failed"); }
+    if (rc != GF_OK) { nvtxRangePop(); return fail(err, rc, "gf_get_frame_transform_at failed"); }
     const float* mesh_dev = nullptr;
     if (mesh && mesh_len) {
-        memcpy(s.h_mesh, mesh, mesh_len * sizeof(float));
-        cudaError_t e = cudaMemcpyAsync(s.d_mesh, s.h_mesh, mesh_len * sizeof(float), cudaMemcpyHostToDevice, s.stream);
-        if (e != cudaSuccess) { nvtxRangePop(); return qcuda(q, e, "mesh upload"); }
-        mesh_dev = s.d_mesh;
+        memcpy(s.h_mesh.ptr, mesh, mesh_len * sizeof(float));
+        cudaError_t e = cudaMemcpyAsync(s.d_mesh.ptr, s.h_mesh.ptr, mesh_len * sizeof(float), cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) { nvtxRangePop(); return cuda_error(e, "mesh upload", err); }
+        mesh_dev = s.d_mesh.ptr;
     }
-    const unsigned long long l0 = gf_cuda_launch_count(s.ctx);
-    rc = gf_internal_run_frame(s.ctx, in, out, &kp, s.d_mat, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags, (void*)s.stream,
-                               q->cfg.checksum ? s.d_sum : nullptr);
-    if (rc != GF_OK) { q->last_error = gf_cuda_last_error(s.ctx); nvtxRangePop(); return rc; }
-    q->launches += gf_cuda_launch_count(s.ctx) - l0 + (q->cfg.checksum ? 1 : 0);
+    const unsigned long long l0 = gf_cuda_launch_count(s.ctx.get());
+    rc = gf_internal_run_frame(s.ctx.get(), in, out, &kp, s.d_mat.ptr, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags.ptr, (void*)st,
+                               q->cfg.checksum ? s.d_sum.ptr : nullptr);
+    if (rc != GF_OK) { q->last_error = gf_cuda_last_error(s.ctx.get()); nvtxRangePop(); return rc; }
+    q->launches += gf_cuda_launch_count(s.ctx.get()) - l0 + (q->cfg.checksum ? 1 : 0);
     if (q->cfg.checksum) {
-        cudaError_t e = cudaMemcpyAsync(s.h_sum, s.d_sum, sizeof(uint64_t), cudaMemcpyDeviceToHost, s.stream);
-        if (e != cudaSuccess) { nvtxRangePop(); return qcuda(q, e, "checksum download"); }
+        cudaError_t e = cudaMemcpyAsync(s.h_sum.ptr, s.d_sum.ptr, sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
+        if (e != cudaSuccess) { nvtxRangePop(); return cuda_error(e, "checksum download", err); }
     }
-    cudaError_t e = cudaEventRecord(s.done, s.stream);
+    cudaError_t e = cudaEventRecord(s.done.get(), st);
     nvtxRangePop();
-    if (e != cudaSuccess) return qcuda(q, e, "cudaEventRecord");
+    if (e != cudaSuccess) return cuda_error(e, "cudaEventRecord", err);
     s.busy = true; s.frame = frame;
     q->fifo.push_back(q->next);
     q->next = (q->next + 1) % (int)q->slots.size();
@@ -220,13 +219,13 @@ GF_API int gf_cuda_queue_submit(gf_cuda_queue* q, size_t frame, double timestamp
 
 GF_API int gf_cuda_queue_wait(gf_cuda_queue* q, size_t* out_frame, uint64_t* out_checksum) {
     if (!q) return GF_ERR_BAD_PARAMS;
-    if (q->fifo.empty()) return qfail(q, GF_ERR_NO_DATA, "nothing in flight");
+    if (q->fifo.empty()) return fail(&q->last_error, GF_ERR_NO_DATA, "nothing in flight");
     QSlot& s = q->slots[(size_t)q->fifo.front()];
     q->fifo.pop_front();
     int rc = finish_slot(q, s);
     if (rc != GF_OK) return rc;
     if (out_frame) *out_frame = s.frame;
-    if (out_checksum) *out_checksum = *s.h_sum;
+    if (out_checksum) *out_checksum = *s.h_sum.ptr;
     return GF_OK;
 }
 
@@ -242,21 +241,9 @@ GF_API const char* gf_cuda_queue_last_error(gf_cuda_queue* q) { return q ? q->la
 GF_API void gf_cuda_queue_destroy(gf_cuda_queue* q) {
     if (!q) return;
     cudaSetDevice(q->cfg.device);
-    for (QSlot& s : q->slots) {
-        if (s.stream) cudaStreamSynchronize(s.stream);
-        if (s.ctx) gf_cuda_destroy(s.ctx);
-        if (s.d_mat) cudaFree(s.d_mat);
-        if (s.d_flags) cudaFree(s.d_flags);
-        if (s.h_mesh) cudaFreeHost(s.h_mesh);
-        if (s.d_mesh) cudaFree(s.d_mesh);
-        if (s.d_sum) cudaFree(s.d_sum);
-        if (s.h_sum) cudaFreeHost(s.h_sum);
-        if (s.done) cudaEventDestroy(s.done);
-        if (s.stream) cudaStreamDestroy(s.stream);
-    }
-    if (q->gyro) gf_cuda_gyro_free(q->gyro);
-    (void)cudaGetLastError();
+    for (QSlot& s : q->slots) if (s.stream) cudaStreamSynchronize(s.stream.get());
     delete q;
+    (void)cudaGetLastError();       // a failed teardown call must not fail the thread's next call
 }
 
 } // extern "C"

@@ -9,6 +9,7 @@
 #include <vector>
 #include "../../include/gyroflow_cuda.h"
 #include "warp_kernel_x2.cuh"
+#include "c_abi_internal.h"
 
 using namespace gf;
 
@@ -167,7 +168,7 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, int n_cf
 
 extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long seed, int n_cfg, int step, unsigned long long* out4) {
     if (!out4 || n_cfg < 1 || step < 1) return GF_ERR_BAD_PARAMS;
-    if (cudaSetDevice(device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(device));
     std::vector<FilterCfg> cfgs((size_t)n_cfg);
     uint64_t st = seed * 0x9E3779B97F4A7C15ULL + 12345u;
     auto rnd = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return (double)(st >> 11) * (1.0 / 9007199254740992.0); };   // [0, 1)
@@ -197,57 +198,52 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
         for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) C.m[r * 3 + q] = (float)(R[0 * 3 + r] * Ki[0 * 3 + q] + R[1 * 3 + r] * Ki[1 * 3 + q] + R[2 * 3 + r] * Ki[2 * 3 + q]);
         C.f1 = (float)((0.3 + 0.9 * rnd()) * C.w); C.c1 = (float)(cy + (rnd() - 0.5) * 40.0);
     }
-    FilterCfg* d_cfg = nullptr; unsigned long long* d_out = nullptr;
-    cudaError_t e;
-    if ((e = cudaMalloc(&d_cfg, cfgs.size() * sizeof(FilterCfg))) != cudaSuccess || (e = cudaMalloc(&d_out, 4 * sizeof(unsigned long long))) != cudaSuccess) {
-        if (d_cfg) cudaFree(d_cfg); (void)cudaGetLastError(); return GF_ERR_CUDA;
-    }
-    cudaMemcpy(d_cfg, cfgs.data(), cfgs.size() * sizeof(FilterCfg), cudaMemcpyHostToDevice);
-    cudaMemset(d_out, 0, 4 * sizeof(unsigned long long));
-    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg, n_cfg, step, 0x1p-17f, d_out);
-    e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(out4, d_out, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    cudaFree(d_cfg); cudaFree(d_out);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    GrowBuf<FilterCfg> d_cfg; GrowBuf<unsigned long long> d_out;
+    CK(nullptr, d_cfg.reserve(cfgs.size(), nullptr));
+    CK(nullptr, d_out.reserve(4, nullptr));
+    CK(nullptr, cudaMemcpy(d_cfg.ptr, cfgs.data(), cfgs.size() * sizeof(FilterCfg), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemset(d_out.ptr, 0, 4 * sizeof(unsigned long long)));
+    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg.ptr, n_cfg, step, 0x1p-17f, d_out.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaDeviceSynchronize());
+    CK(nullptr, cudaMemcpy(out4, d_out.ptr, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 
 // out2[0]: mismatches of atanf2_core over all floats in [2^-28, 2^24); out2[1]: of sqrt_seq over all floats in [2^-56, 2^48).
 extern "C" GF_API int gf_cuda_selftest_exhaustive(int device, unsigned long long* out2) {
     if (!out2) return GF_ERR_BAD_PARAMS;
-    if (cudaSetDevice(device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
-    unsigned long long* d = nullptr;
-    if (cudaMalloc(&d, 2 * sizeof(unsigned long long)) != cudaSuccess) return GF_ERR_CUDA;
-    cudaMemset(d, 0, 2 * sizeof(unsigned long long));
-    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-28f), __float_as_uint_host(0x1p24f), 0, d);
-    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-56f), __float_as_uint_host(0x1p48f), 1, d + 1);
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(out2, d, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(device));
+    GrowBuf<unsigned long long> d;
+    CK(nullptr, d.reserve(2, nullptr));
+    CK(nullptr, cudaMemset(d.ptr, 0, 2 * sizeof(unsigned long long)));
+    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-28f), __float_as_uint_host(0x1p24f), 0, d.ptr);
+    CK(nullptr, cudaGetLastError());
+    sweep_kernel<<<132 * 16, 256>>>(__float_as_uint_host(0x1p-56f), __float_as_uint_host(0x1p48f), 1, d.ptr + 1);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaDeviceSynchronize());
+    CK(nullptr, cudaMemcpy(out2, d.ptr, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 
 extern "C" GF_API int gf_cuda_selftest(int device, unsigned long long n, unsigned long long seed, unsigned long long* out4) {
     if (!out4) return GF_ERR_BAD_PARAMS;
-    if (cudaSetDevice(device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
-    unsigned long long* d = nullptr;
-    if (cudaMalloc(&d, 4 * sizeof(unsigned long long)) != cudaSuccess) return GF_ERR_CUDA;
-    cudaMemset(d, 0, 4 * sizeof(unsigned long long));
-    uint32_t* dbg = nullptr;
-    if (getenv("GF_SELFTEST_DEBUG")) { cudaMalloc(&dbg, 65 * 4); cudaMemset(dbg, 0, 65 * 4); }
-    selftest_kernel<<<132 * 8, 256>>>(n, seed, d, dbg);
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e == cudaSuccess) e = cudaMemcpy(out4, d, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    if (dbg) {
-        uint32_t h[65]; cudaMemcpy(h, dbg, sizeof(h), cudaMemcpyDeviceToHost);
+    CK(nullptr, cudaSetDevice(device));
+    GrowBuf<unsigned long long> d;
+    CK(nullptr, d.reserve(4, nullptr));
+    CK(nullptr, cudaMemset(d.ptr, 0, 4 * sizeof(unsigned long long)));
+    GrowBuf<uint32_t> dbg;
+    if (getenv("GF_SELFTEST_DEBUG")) { dbg.reserve(65, nullptr); cudaMemset(dbg.ptr, 0, 65 * 4); }
+    selftest_kernel<<<132 * 8, 256>>>(n, seed, d.ptr, dbg.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaDeviceSynchronize());
+    CK(nullptr, cudaMemcpy(out4, d.ptr, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (dbg.ptr) {
+        uint32_t h[65]; cudaMemcpy(h, dbg.ptr, sizeof(h), cudaMemcpyDeviceToHost);
         for (unsigned i = 0; i < (h[0] < 16 ? h[0] : 16); ++i) {
             float x, g, w, o; memcpy(&x, &h[1 + i * 4], 4); memcpy(&g, &h[2 + i * 4], 4); memcpy(&w, &h[3 + i * 4], 4); memcpy(&o, &h[4 + i * 4], 4);
             printf("atanf2 mismatch: x=%a (%08x) got=%a want=%a other-lane=%a (%08x)\n", x, h[1 + i * 4], g, w, o, h[4 + i * 4]);
         }
-        cudaFree(dbg);
     }
-    cudaFree(d);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
     return GF_OK;
 }

@@ -392,7 +392,7 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
     if (n == 0) return GF_OK;
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
     if (!k.find_fov) return GF_ERR_UNSUPPORTED_COMBO;
-    if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(g->device));
     gf_compute_params cp = *cp_user;
     const int org_ow = cp.output_width, org_oh = cp.output_height;
     cp.fov_scale = 1.0; cp.n_fovs = 0; cp.n_minimal_fovs = 0; cp.output_width = cp.width; cp.output_height = cp.height;
@@ -407,18 +407,15 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
     // per-frame uniforms on the host: two O(log n) lookups per frame
     std::vector<ZoomFrame> hf(n);
     for (size_t i = 0; i < n; ++i) hf[i] = frame_uniforms(g, cp, A, timestamps_ms[i], i, cp.lens_correction_amount, true);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
-    ZoomFrame* d_frames = nullptr; double* d_out = nullptr;
-    cudaError_t e;
-    if ((e = cudaMalloc(&d_frames, n * sizeof(ZoomFrame))) != cudaSuccess || (e = cudaMalloc(&d_out, n * sizeof(double))) != cudaSuccess) {
-        if (d_frames) cudaFree(d_frames); (void)cudaGetLastError(); return GF_ERR_CUDA;
-    }
-    e = cudaMemcpyAsync(d_frames, hf.data(), n * sizeof(ZoomFrame), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) { k.find_fov<<<(unsigned)n, 128, 0, st>>>(A, d_frames, d_out); e = cudaGetLastError(); }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_fov_minimal, d_out, n * sizeof(double), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d_frames); cudaFree(d_out);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    GrowBuf<ZoomFrame> d_frames; GrowBuf<double> d_out;
+    CK(nullptr, d_frames.reserve(n, st));
+    CK(nullptr, d_out.reserve(n, st));
+    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(ZoomFrame), cudaMemcpyHostToDevice, st));
+    k.find_fov<<<(unsigned)n, 128, 0, st>>>(A, d_frames.ptr, d_out.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaMemcpyAsync(out_fov_minimal, d_out.ptr, n * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CK(nullptr, cudaStreamSynchronize(st));
     return GF_OK;
 }
 
@@ -430,25 +427,22 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
     if (n == 0) return GF_OK;
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
     if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
-    if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(g->device));
     ZoomArgs A;
     const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
     const gf_compute_params* cp = &rcp;
     const double fov = points_fov(cp, frame, use_fovs != 0, timestamp_ms);
     setup_points_args(g, *cp, distortion_model, fov, A);
     const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, lens_correction_amount, false);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
-    float2* d_in = nullptr; float* d_out = nullptr;
-    cudaError_t e;
-    if ((e = cudaMalloc(&d_in, n * sizeof(float2))) != cudaSuccess || (e = cudaMalloc(&d_out, n * 2 * sizeof(float))) != cudaSuccess) {
-        if (d_in) cudaFree(d_in); (void)cudaGetLastError(); return GF_ERR_CUDA;
-    }
-    e = cudaMemcpyAsync(d_in, points_xy, n * sizeof(float2), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) { k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, d_in, n, 0, 0, d_out); e = cudaGetLastError(); }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_xy, d_out, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d_in); cudaFree(d_out);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    GrowBuf<float2> d_in; GrowBuf<float> d_out;
+    CK(nullptr, d_in.reserve(n, st));
+    CK(nullptr, d_out.reserve(n * 2, st));
+    CK(nullptr, cudaMemcpyAsync(d_in.ptr, points_xy, n * sizeof(float2), cudaMemcpyHostToDevice, st));
+    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, d_in.ptr, n, 0, 0, d_out.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaMemcpyAsync(out_xy, d_out.ptr, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(nullptr, cudaStreamSynchronize(st));
     return GF_OK;
 }
 
@@ -462,15 +456,15 @@ GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* c
     const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
     const gf_compute_params* cp = &rcp;
     if (cp->width < 1 || cp->height < 1) return GF_ERR_BAD_PARAMS;
-    if (cudaSetDevice(g->device) != cudaSuccess) { (void)cudaGetLastError(); return GF_ERR_CUDA; }
+    CK(nullptr, cudaSetDevice(g->device));
     ZoomArgs A;
     const double fov = points_fov(cp, frame, true, timestamp_ms);
     setup_points_args(g, *cp, distortion_model, fov, A);
     const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, 1.0, false);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream;
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
     const size_t n = (size_t)cp->width * (size_t)cp->height;
     k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);
-    if (cudaGetLastError() != cudaSuccess) return GF_ERR_CUDA;
+    CK(nullptr, cudaGetLastError());
     return GF_OK;
 }
 
