@@ -9,7 +9,8 @@
 // One CTA per frame: 120 edge points (then <= 4 rounds of 63 interpolated points) are pushed through the inverse lens
 // model with their own rolling-shutter rotation in parallel; the order-dependent nearest_edge fold runs on one thread.
 // The reference runs this with rayon over frames (fov_iterative.rs:42-56) before rendering starts.
-// The rotations are f64 (device libm vs host libm differ in the last f64 bit), so parity with the oracle is to 1e-6.
+// The rotations are f64, and the slerp's acos / sin differ from glibc's in the last f64 bit, so with the rotation on parity with the
+// oracle is to 1e-6.  With suppress_rotation set no libm result reaches the output and the point path is bit-exact.
 #include <cuda_runtime.h>
 #include <cmath>
 #include <cstring>

@@ -7,8 +7,8 @@
                                                                            src/core/zooming/fov_iterative.rs:76-200
 
 Written from the Rust text in numpy scalars; the C oracle (oracle/gf_oracle.c, gf_oracle_find_fov) and the CUDA kernels
-(gyroflow_b200/csrc/zoom_kernel.cu) are checked against it in tests/test_zoom.py.  The rotations come from numpy's f64 slerp /
-matrix products (tests/np_producer.py), not nalgebra's, so the bar is a relative 1e-6 on the resulting FOV, like the device-vs-oracle bar.
+(gyroflow_b200/csrc/zoom_kernel.cu) are checked against it in tests/test_zoom.py and tests/test_point_matrix.py.  The rotations come
+from numpy's f64 slerp / matrix products (tests/np_producer.py), which round like the oracle's on the host: the two agree bit for bit.
 """
 import math
 
