@@ -240,6 +240,7 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     A.smap_x = make_map(0.0f, A.frame_w, (float)p->source_rect[0], (float)(p->source_rect[0] + p->source_rect[2]), -1.0f);
     A.smap_y = make_map(0.0f, A.frame_h, (float)p->source_rect[1], (float)(p->source_rect[1] + p->source_rect[3]), -1.0f);
     A.rs_lim = (p->flags & 16) == 16 ? p->width : p->height;
+    A.row_lim = std::min(A.rs_lim, p->matrix_count - 1);
     const float lim = p->pixel_value_limit;
     A.u8_limit = (lim != lim) ? 255 : (lim < 0.0f ? 0 : (lim >= 255.0f ? 255 : (int)lim));
     A.src_rect[0] = p->source_rect[0]; A.src_rect[1] = p->source_rect[1];
@@ -267,6 +268,13 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
         A.hot.full_rows = (int)std::min<size_t>(A.dst_len / (size_t)p->output_stride, (size_t)A.out_rows);
         const size_t tail = A.dst_len - (size_t)A.hot.full_rows * (size_t)p->output_stride;
         A.hot.last_cols = (A.hot.full_rows < A.out_rows) ? (int)std::min<size_t>(tail / (size_t)bpp, (size_t)A.out_cols) : 0;
+        // a last row that holds all of [x0, x1) or none of it is a plain row bound: fold it into y1 and keep the per-pixel test to
+        // four compares; only a row cut inside [x0, x1) needs the full_rows / last_cols test (F_SHORTROW)
+        if (A.hot.full_rows < A.out_rows) {
+            if (A.hot.last_cols >= A.hot.x1) A.hot.y1 = std::min(A.hot.y1, A.hot.full_rows + 1);
+            else if (A.hot.last_cols <= A.hot.x0) A.hot.y1 = std::min(A.hot.y1, A.hot.full_rows);
+            else A.feat |= F_SHORTROW;
+        }
         A.feat |= F_INTPRO;
     }
 }

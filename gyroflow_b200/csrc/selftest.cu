@@ -153,8 +153,8 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, int n_cf
             const float diff = fabsf(tv - tv_exact);
             ++in_regime;
             if (!(diff <= bound)) ++violations;
-            const float z = tv - 0.5f;
-            if (!(fabsf(z - ((z + 12582912.0f) - 12582912.0f)) > bound)) ++uncertain;
+            int row;
+            if (!certify_row(tv, bound, C.h, row)) ++uncertain;
             const float ratio = bound > 0.0f ? diff / bound : (diff > 0.0f ? 1e9f : 0.0f);
             worst = max(worst, (unsigned)fminf(ratio * 1e6f, 4.0e9f));
         }
@@ -207,6 +207,31 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
     CK(nullptr, cudaGetLastError());
     CK(nullptr, cudaDeviceSynchronize());
     CK(nullptr, cudaMemcpy(out4, d_out.ptr, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    return GF_OK;
+}
+
+namespace {
+__global__ void certify_kernel(const float* __restrict__ t, size_t n, float eps, int lim, uint8_t* __restrict__ cert, int32_t* __restrict__ row) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        int r;
+        cert[i] = certify_row(t[i], eps, lim, r) ? 1 : 0;
+        row[i] = r;
+    }
+}
+} // namespace
+
+extern "C" GF_API int gf_cuda_selftest_certify(int device, const float* t, size_t n, float eps, int lim, uint8_t* cert_out, int32_t* row_out) {
+    if (!t || !cert_out || !row_out) return GF_ERR_BAD_PARAMS;
+    if (n == 0) return GF_OK;
+    CK(nullptr, cudaSetDevice(device));
+    GrowBuf<float> d_t; GrowBuf<uint8_t> d_c; GrowBuf<int32_t> d_r;
+    CK(nullptr, d_t.reserve(n, nullptr)); CK(nullptr, d_c.reserve(n, nullptr)); CK(nullptr, d_r.reserve(n, nullptr));
+    CK(nullptr, cudaMemcpy(d_t.ptr, t, n * sizeof(float), cudaMemcpyHostToDevice));
+    certify_kernel<<<132 * 8, 256>>>(d_t.ptr, n, eps, lim, d_c.ptr, d_r.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaDeviceSynchronize());
+    CK(nullptr, cudaMemcpy(cert_out, d_c.ptr, n, cudaMemcpyDeviceToHost));
+    CK(nullptr, cudaMemcpy(row_out, d_r.ptr, n * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 

@@ -70,6 +70,7 @@ enum : uint32_t {
     F_INTPRO     = 1u << 23,  // packed kernel: both output maps are the identity -> integer prologue (X2Hot below)
     F_FILTER     = 1u << 24,  // packed kernel: filtered rolling-shutter pre-pass (approximate mid-row evaluation + deferred exact pairs)
     F_SRC_VEC8   = 1u << 25,  // source pointer, stride and length are multiples of 8: every aligned 8-byte word that holds a valid byte is readable
+    F_SHORTROW   = 1u << 26,  // packed kernel, F_INTPRO: the last output row is written only in part (X2Hot full_rows / last_cols)
 };
 
 // Features the specialised ("lean") instantiation compiles out entirely.  The reference's OpenCL backend does the same
@@ -126,6 +127,7 @@ struct WarpArgs {
     float frame_w, frame_h;         // frame size after input_rotation (:485-489)
     float rot_cos, rot_sin;         // cos/sin(input_rotation * PI/180) via gf_cosf/gf_sinf
     int   rs_lim;                   // HRS ? width : height
+    int   row_lim;                  // min(rs_lim, matrix_count - 1): the packed kernel's one clamp of a matrix row index
     int   u8_limit;                 // trunc(min(pixel_value_limit, 255)) for the integer u8 sampler
     int   src_rect[4];              // rx0, ry0, rx1, ry1
     int   interior_span[2];         // rx1 - 2 - rx0, ry1 - 2 - ry0: a bilinear footprint at (sx, sy) is interior iff (unsigned)(sx - rx0) <= span (both axes)
@@ -133,8 +135,8 @@ struct WarpArgs {
     // identity (F_INTPRO), and the sampler's rect constants side by side (one 128-bit constant load)
     struct X2Hot {
         int x_off, y_off;           // opx == (float)(x + x_off), opy likewise (exact: integers below 2^24)
-        int x0, x1, y0, y1;         // pixel (x, y) is written iff x0 <= x < x1 and y0 <= y < y1 ...
-        int full_rows, last_cols;   // ... and it fits the buffer: y < full_rows, or y == full_rows and x < last_cols (short last row)
+        int x0, x1, y0, y1;         // pixel (x, y) is written iff x0 <= x < x1 and y0 <= y < y1 (rows that do not fit the buffer folded in) ...
+        int full_rows, last_cols;   // ... and, with F_SHORTROW only, it fits the buffer: y < full_rows, or y == full_rows and x < last_cols
         int rect[4];                // rx0, ry0, span_x, span_y
     } hot;
 };

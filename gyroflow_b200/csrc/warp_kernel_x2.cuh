@@ -63,7 +63,7 @@ template <> struct Lens2<GF_LENS_OPENCV_FISHEYE> {
         const float x = _x * iw, y = _y * iw;
         const float a = __fmaf_rn(x, x, y * y);
         const uint32_t ab = __float_as_uint(a);
-        const int idx = min(max((int)(ab >> 19) - (int)GF_APX_BASE, 0), GF_APX_ROWS - 1);
+        const int idx = __vimin_s32_relu((int)(ab >> 19) - (int)GF_APX_BASE, GF_APX_ROWS - 1);     // max(min(., ROWS - 1), 0): any a, NaN included
         const float a0 = __uint_as_float((ab & 0xfff80000u) | 0x00040000u);      // midpoint of a's 1/16-octave interval
         const float4 c = __ldg(&GF_APX_TAB[idx]);
         const float d = a - a0;
@@ -527,11 +527,25 @@ GF_DEV void round_half_away_w(f2 a2, int& wa, int& wb) {
     const float sb = __fadd_rz(BOUNDED ? a2.y : fmaxf(a2.y, -4.0f), 8388608.0f);
     wa = __float_as_int(sa) - 0x4affffff; wb = __float_as_int(sb) - 0x4affffff;
 }
-// max(min(round(t) as i32, lim), 0) for both lanes, 0 <= lim < 2^22
+// max(min(round(t) as i32, lim), 0) for both lanes, lim < 2^22
 GF_DEV void round_away_clamped_x2(f2 t, int lim, int& ra, int& rb) {
     int wa, wb;
     round_half_away_w(p2::mul(t, p2::bc(2.0f)), wa, wb);
-    ra = max(min(wa >> 1, lim), 0); rb = max(min(wb >> 1, lim), 0);
+    ra = __vimin_s32_relu(wa >> 1, lim); rb = __vimin_s32_relu(wb >> 1, lim);
+}
+
+// Certificate of the filtered pre-pass, and the row it certifies, in one rounding (FILTER_ANALYSIS.md "test form").
+// For |t| < 2^20, s = RN(t + 1.5 * 2^23) lies in [2^23, 2^24) where the float spacing is 1, so n = s - 1.5 * 2^23 = RNE(t) exactly,
+// r = t - n is exact and |r| <= 1/2, and the distance from t to the nearest boundary n +- 1/2 is 1/2 - |r|, computed rounded DOWN
+// (exact whenever |t| >= 1/4; below, the rounding can only shrink it).  Returns true when that distance exceeds eps: then t is no
+// tie, RNE(t) is f32::round (half away from zero), and every t' within eps of t rounds to the same row.  row = max(min(n, lim), 0)
+// from the bits of s, for any input (NaN and large t give some row; the caller only uses it when certified).
+GF_DEV bool certify_row(float t, float eps, int lim, int& row) {
+    const float s = __fadd_rn(t, 12582912.0f);
+    const float r = __fsub_rn(t, __fsub_rn(s, 12582912.0f));
+    const float d = __fsub_rd(0.5f, fabsf(r));
+    row = __vimin_s32_relu(__float_as_int(s) - 0x4b400000, lim);
+    return (d > eps) & (fabsf(t) < 0x1p20f);
 }
 
 // everything that is not "valid pixel with an interior 8-bit bilinear footprint": background fill or the generic sampler,
@@ -582,6 +596,30 @@ GF_DEV void shade_lean(bool ok, bool far, float u, float v, int wu, int wv, cons
 
 #define GF_X2_ROWS_PER_BLOCK (2 * GF_BLOCK_Y)
 
+// cold: the final evaluation set `bad`.  The scalar kernel's exact code evaluates both pixels of the pair, and this call also shades
+// them (or writes their coordinates), so the hot path after it only ever sees pixels that are Some(..) with coordinates inside the
+// domain of the rounding shortcut.
+template <int LENS, int DIGITAL, class PIX, bool COORD>
+static __device__ __noinline__ void finish_pair_cold(const WarpArgs& A, int x, int y0, float pxs, f2 py, uint32_t idx_a, uint32_t idx_b,
+                                                     bool wr_a, bool wr_b) {
+    const PairUV c = rotate_and_distort_cold<LENS, DIGITAL>(pxs, py.x, py.y, idx_a, idx_b, A, 1);
+    const bool ok_a = (c.ok & 1) != 0, ok_b = (c.ok & 2) != 0;
+    if (COORD) {      // the exact coordinates; None / not-written pixels as markers
+        uint2* const cm_a = A.coord_out + ((size_t)y0 * (size_t)A.out_cols + (size_t)x);
+        *cm_a = !wr_a ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : (ok_a ? make_uint2(__float_as_uint(c.ua), __float_as_uint(c.va)) : make_uint2(GF_COORD_MARK, GF_COORD_NONE));
+        if ((y0 + 1) < A.out_rows) cm_a[A.out_cols] = !wr_b ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : (ok_b ? make_uint2(__float_as_uint(c.ub), __float_as_uint(c.vb)) : make_uint2(GF_COORD_MARK, GF_COORD_NONE));
+        return;
+    }
+    const unsigned long long off_a = (unsigned long long)y0 * (unsigned long long)A.p.output_stride + (unsigned long long)x * (unsigned long long)PIX::BYTES;
+    int wu_a = 0, wu_b = 0, wv_a = 0, wv_b = 0;
+    if (PIX::SCALAR == SC_U8) {      // as on the hot path; the value of a far lane is not used (`interior` is false for it)
+        round_half_away_w<true>(p2::mul(p2::mk(c.ua, c.ub), p2::bc(64.0f)), wu_a, wu_b);
+        round_half_away_w<true>(p2::mul(p2::mk(c.va, c.vb), p2::bc(64.0f)), wv_a, wv_b);
+    }
+    if (wr_a) shade_lean<PIX>(ok_a, (c.ok & 4) != 0, c.ua, c.va, wu_a, wv_a, A, A.dst + off_a);
+    if (wr_b) shade_lean<PIX>(ok_b, (c.ok & 8) != 0, c.ub, c.vb, wu_b, wv_b, A, A.dst + off_a + (unsigned long long)A.p.output_stride);
+}
+
 // COORD: pass 1 of the two-pass mode — write the coordinates to A.coord_out instead of sampling (pixel-format independent: the
 // pixel size then comes from KernelParams, PIX is a placeholder).
 // exact_prepass: evaluate the mid-row transform with the reference's own arithmetic (always true unless the frame runs the filtered
@@ -599,10 +637,14 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
     float opx, opy_a, opy_b;
     bool wr_a, wr_b;
     if (A.feat & F_INTPRO) {                                 // identity rect maps: the same tests on integers (host: fill_uniforms)
-        const bool in_x = (x >= A.hot.x0) & (x < A.hot.x1);
         const int y1 = y0 + 1;
-        wr_a = in_x & (y0 >= A.hot.y0) & (y0 < A.hot.y1) & ((y0 < A.hot.full_rows) | ((y0 == A.hot.full_rows) & (x < A.hot.last_cols)));
-        wr_b = in_x & (y1 >= A.hot.y0) & (y1 < A.hot.y1) & ((y1 < A.hot.full_rows) | ((y1 == A.hot.full_rows) & (x < A.hot.last_cols)));
+        const bool in_x = (x >= A.hot.x0) & (x < A.hot.x1);
+        wr_a = in_x & (y0 >= A.hot.y0) & (y0 < A.hot.y1);
+        wr_b = in_x & (y1 >= A.hot.y0) & (y1 < A.hot.y1);
+        if (A.feat & F_SHORTROW) {                           // a last row that holds some but not all of [x0, x1): y1 cannot express it
+            wr_a &= (y0 < A.hot.full_rows) | ((y0 == A.hot.full_rows) & (x < A.hot.last_cols));
+            wr_b &= (y1 < A.hot.full_rows) | ((y1 == A.hot.full_rows) & (x < A.hot.last_cols));
+        }
         opx = (float)(x + A.hot.x_off); opy_a = (float)(y0 + A.hot.y_off); opy_b = (float)(y1 + A.hot.y_off);
     } else {
         opx = map_apply_int_lean((float)x, A.omap_x);
@@ -623,79 +665,69 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
     const float pxs = opx + P.translation2d[0];
     const f2 px = bc(pxs);
     const f2 py = mk(opy_a + P.translation2d[1], opy_b + P.translation2d[1]);
-    const int lim = A.rs_lim;
-    int sy_a, sy_b;
-    round_away_clamped_x2(py, lim, sy_a, sy_b);                                                         // :465-469
-    bool have_row = false;
-    if constexpr (TRUSTED && LensApprox<LENS>::value && DIGITAL == GF_LENS_NONE) if (!exact_prepass) {  // F_FILTER & F_RS (host)
-        // :470-479, filtered: certify round(v_mid) from the approximate evaluation, defer the pair when it cannot be
-        const MatRow9 rm = load_row9(A.matrices, (uint32_t)P.matrix_count / 2u);
-        const float bx = pxs * rm.m01.x, by = pxs * rm.m23.y, bw = pxs * rm.m67.x;                      // the reference's products and sums, unfused
-        const float xa = (bx + py.x * rm.m01.y) + rm.m23.x, xb = (bx + py.y * rm.m01.y) + rm.m23.x;
-        const float ya = (by + py.x * rm.m45.x) + rm.m45.y, yb = (by + py.y * rm.m45.x) + rm.m45.y;
-        const float wa = (bw + py.x * rm.m67.y) + rm.m8,    wb = (bw + py.y * rm.m67.y) + rm.m8;
-        float ca, cb;
-        const bool ra = Lens2<LENS>::approx_v(xa, ya, wa, P, A.flt.a_cap, ca);
-        const bool rb = Lens2<LENS>::approx_v(xb, yb, wb, P, A.flt.a_cap, cb);
-        const float ta = ca + P.c[1], tb = cb + P.c[1];
-        // distance of t to the nearest rounding boundary n + 1/2 (|t| < 2^20: the magic-number rounding is exact)
-        const float za = ta - 0.5f, zb = tb - 0.5f;
-        const float da = fabsf(za - ((za + 12582912.0f) - 12582912.0f)), db = fabsf(zb - ((zb + 12582912.0f) - 12582912.0f));
-        const float ea = __fmaf_rn(fabsf(ca), A.flt.rho, fabsf(ta) * 0x1p-22f), eb = __fmaf_rn(fabsf(cb), A.flt.rho, fabsf(tb) * 0x1p-22f);
-        const bool sure = ra & rb & (da > ea) & (db > eb) & (fabsf(ta) < 0x1p20f) & (fabsf(tb) < 0x1p20f);
-        if (sure) {
-            round_away_clamped_x2(mk(ta, tb), lim, sy_a, sy_b);
-            have_row = true;
-        } else {                                         // append the pair to the frame's queue (warp-aggregated), rendered by the tail launch
-            const unsigned m = __activemask();
-            const unsigned lane = threadIdx.x & 31u;
-            const int leader = __ffs((int)m) - 1;
-            unsigned base = 0;
-            if ((int)lane == leader) base = atomicAdd(A.flt.count, (unsigned)__popc(m));
-            base = __shfl_sync(m, base, leader);
-            const unsigned slot = base + (unsigned)__popc(m & ((1u << lane) - 1u));
-            if (slot < A.flt.cap) { A.flt.q[slot] = (uint32_t)x | ((uint32_t)(y0 >> 1) << 16); return; }
-            // queue full: this thread evaluates the exact pre-pass itself
+    // matrix row of each pixel (:465-482).  Without rolling shutter the table has one row (F_RS <=> matrix_count > 1), so the row is 0.
+    // lim = min(rs_lim, matrix_count - 1): clamp(., 0, rs_lim) of :469 and the min(., matrix_count - 1) of :482 in one clamp.
+    const int lim = A.row_lim;
+    int sy_a = 0, sy_b = 0;
+    do {      // `break`: the rows are known
+        if constexpr (TRUSTED && LensApprox<LENS>::value && DIGITAL == GF_LENS_NONE) {
+            if (!exact_prepass) {                        // F_FILTER, which implies F_RS (host)
+                // :470-479, filtered: certify round(v_mid) from the approximate evaluation, defer the pair when it cannot be
+                const MatRow9 rm = load_row9(A.matrices, (uint32_t)P.matrix_count / 2u);
+                const float bx = pxs * rm.m01.x, by = pxs * rm.m23.y, bw = pxs * rm.m67.x;              // the reference's products and sums, unfused
+                const float xa = (bx + py.x * rm.m01.y) + rm.m23.x, xb = (bx + py.y * rm.m01.y) + rm.m23.x;
+                const float ya = (by + py.x * rm.m45.x) + rm.m45.y, yb = (by + py.y * rm.m45.x) + rm.m45.y;
+                const float wa = (bw + py.x * rm.m67.y) + rm.m8,    wb = (bw + py.y * rm.m67.y) + rm.m8;
+                float ca, cb;
+                const bool ra = Lens2<LENS>::approx_v(xa, ya, wa, P, A.flt.a_cap, ca);
+                const bool rb = Lens2<LENS>::approx_v(xb, yb, wb, P, A.flt.a_cap, cb);
+                const float ta = ca + P.c[1], tb = cb + P.c[1];
+                const float ea = __fmaf_rn(fabsf(ca), A.flt.rho, fabsf(ta) * 0x1p-22f), eb = __fmaf_rn(fabsf(cb), A.flt.rho, fabsf(tb) * 0x1p-22f);
+                const bool ca_ok = certify_row(ta, ea, lim, sy_a), cb_ok = certify_row(tb, eb, lim, sy_b);
+                if (ra & rb & ca_ok & cb_ok) break;
+                // append the pair to the frame's queue (warp-aggregated), rendered by the tail launch
+                const unsigned m = __activemask();
+                const unsigned lane = threadIdx.x & 31u;
+                const int leader = __ffs((int)m) - 1;
+                unsigned base = 0;
+                if ((int)lane == leader) base = atomicAdd(A.flt.count, (unsigned)__popc(m));
+                base = __shfl_sync(m, base, leader);
+                const unsigned slot = base + (unsigned)__popc(m & ((1u << lane) - 1u));
+                if (slot < A.flt.cap) { A.flt.q[slot] = (uint32_t)x | ((uint32_t)(y0 >> 1) << 16); return; }
+                // queue full: this thread evaluates the exact pre-pass itself
+            } else if (!(A.feat & F_RS)) break;
+        } else {
+            if (!(A.feat & F_RS)) break;
         }
-    }
-    if ((A.feat & F_RS) && !have_row) {                                                                 // :470-479
+        // :470-479, exact
         const uint32_t mid = (uint32_t)P.matrix_count / 2u;
-        f2 tu, tv; bool oa = true, ob = true, bad = false;
+        f2 tu, tv; bool bad = false;
         rotate_and_distort_x2<LENS, DIGITAL, TRUSTED>(px, py, mid, mid, A, tu, tv, bad);
-        if (bad) {                                       // cold: exact scalar code for both pixels
+        if (bad) {                                       // cold: exact scalar code for both pixels; None keeps the pixel's own row
             const PairUV c = rotate_and_distort_cold<LENS, DIGITAL>(pxs, py.x, py.y, mid, mid, A, 0);
-            oa = (c.ok & 1) != 0; ob = (c.ok & 2) != 0; tv = mk(c.va, c.vb);
+            tv = mk((c.ok & 1) ? c.va : py.x, (c.ok & 2) ? c.vb : py.y);
         }
-        int ra, rb;
-        round_away_clamped_x2(tv, lim, ra, rb);
-        sy_a = oa ? ra : sy_a; sy_b = ob ? rb : sy_b;
-    }
-    const uint32_t last = (uint32_t)(P.matrix_count - 1);
-    const uint32_t idx_a = min((uint32_t)sy_a, last), idx_b = min((uint32_t)sy_b, last);               // :482
-    f2 u, v; bool ok_a = true, ok_b = true, far_a = false, far_b = false, bad = false;
-    rotate_and_distort_x2<LENS, DIGITAL, TRUSTED>(px, py, idx_a, idx_b, A, u, v, bad);                           // :483
+        round_away_clamped_x2(tv, lim, sy_a, sy_b);
+    } while (false);
+    f2 u, v; bool bad = false;
+    rotate_and_distort_x2<LENS, DIGITAL, TRUSTED>(px, py, (uint32_t)sy_a, (uint32_t)sy_b, A, u, v, bad);    // :483
     u = map_apply_x2(u, A.smap_x, bad);                                                                 // :510-515
     v = map_apply_x2(v, A.smap_y, bad);
-    if (bad) {
-        const PairUV c = rotate_and_distort_cold<LENS, DIGITAL>(pxs, py.x, py.y, idx_a, idx_b, A, 1);
-        ok_a = (c.ok & 1) != 0; ok_b = (c.ok & 2) != 0; far_a = (c.ok & 4) != 0; far_b = (c.ok & 8) != 0;
-        u = mk(c.ua, c.ub); v = mk(c.va, c.vb);
-    }
+    if (bad) { finish_pair_cold<LENS, DIGITAL, PIX, COORD>(A, x, y0, pxs, py, (uint32_t)sy_a, (uint32_t)sy_b, wr_a, wr_b); return; }
 
-    if (COORD) {      // the exact coordinates (hot or cold path alike); None / not-written pixels as markers
-        *cm_a = !wr_a ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : (ok_a ? make_uint2(__float_as_uint(u.x), __float_as_uint(v.x)) : make_uint2(GF_COORD_MARK, GF_COORD_NONE));
-        if (row_b) cm_a[A.out_cols] = !wr_b ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : (ok_b ? make_uint2(__float_as_uint(u.y), __float_as_uint(v.y)) : make_uint2(GF_COORD_MARK, GF_COORD_NONE));
+    // from here on both pixels are Some(..) with |u|, |v| < 2^16 (map_apply_x2)
+    if (COORD) {      // the exact coordinates; not-written pixels as markers
+        *cm_a = !wr_a ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : make_uint2(__float_as_uint(u.x), __float_as_uint(v.x));
+        if (row_b) cm_a[A.out_cols] = !wr_b ? make_uint2(GF_COORD_MARK, GF_COORD_SKIP) : make_uint2(__float_as_uint(u.y), __float_as_uint(v.y));
         return;
     }
     int wu_a = 0, wu_b = 0, wv_a = 0, wv_b = 0;
-    if (PIX::SCALAR == SC_U8) {                          // (u * 32).round() for both pixels: 64 * u == 2 * (32 * u) exactly.
-        // |u|, |v| < 2^16 here unless far_* is set (then the result is not used), so the unguarded form of the shortcut applies;
-        // a garbage value for a far lane is harmless because `interior` below is false for it
-        round_half_away_w<true>(mul(u, bc(64.0f)), wu_a, wu_b);
+    if (PIX::SCALAR == SC_U8) {                          // (u * 32).round() for both pixels: 64 * u == 2 * (32 * u) exactly, inside the
+        round_half_away_w<true>(mul(u, bc(64.0f)), wu_a, wu_b);                    // unguarded shortcut's domain
         round_half_away_w<true>(mul(v, bc(64.0f)), wv_a, wv_b);
     }
-    if (wr_a) shade_lean<PIX>(ok_a, far_a, u.x, v.x, wu_a, wv_a, A, A.dst + off_a);                     // :615-622
-    if (wr_b) shade_lean<PIX>(ok_b, far_b, u.y, v.y, wu_b, wv_b, A, A.dst + off_b);
+    if (wr_a) shade_lean<PIX>(true, false, u.x, v.x, wu_a, wv_a, A, A.dst + off_a);                     // :615-622
+    if (wr_b) shade_lean<PIX>(true, false, u.y, v.y, wu_b, wv_b, A, A.dst + off_b);
 }
 
 // The kernel: both table-trust variants in one launch, selected by a DEVICE word.  `A.table_flags` points to the verdict on the

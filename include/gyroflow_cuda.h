@@ -328,6 +328,9 @@ GF_API int         gf_cuda_selftest_exhaustive(int device, unsigned long long* o
  * `step`-th pixel evaluated by the approximate and by the exact chain on the device.  out4 = { pixels inside the regime, pixels whose
  * difference exceeds the proven bound (must be 0), pixels the certificate leaves uncertain, max difference / bound in 1e-6 units }. */
 GF_API int         gf_cuda_selftest_filter(int device, unsigned long long seed, int n_cfg, int step, unsigned long long* out4);
+/* The pre-pass's certify-and-round step (certify_row in warp_kernel_x2.cuh, the device function the packed kernel runs) on n host
+ * values t with one eps and row limit: cert_out[i] = 1 when t[i] is certified, row_out[i] = the clamped row it yields.  Test hook. */
+GF_API int         gf_cuda_selftest_certify(int device, const float* t, size_t n, float eps, int lim, uint8_t* cert_out, int32_t* row_out);
 
 
 /* ------------------------------------------------------------------------------------------
