@@ -169,6 +169,18 @@ PIXEL_TYPES = {
 
 BUF_NONE, BUF_HOST, BUF_DEVICE = 0, 1, 2
 
+# the per-frame feature word (F_* of csrc/warp_kernel.cuh) that gf_cuda_plan_features reports; F_GENERAL_ONLY: the bits only the general
+# kernel implements (the lean and packed kernels compile them out)
+F = {"F_RS": 1 << 0, "F_HRS": 1 << 1, "F_RLIMIT": 1 << 2, "F_REFRACT": 1 << 3, "F_MESH": 1 << 4, "F_DIGITAL": 1 << 5,
+     "F_HSTRETCH": 1 << 6, "F_VSTRETCH": 1 << 7, "F_LCA": 1 << 8, "F_INROT": 1 << 9, "F_BG1": 1 << 10, "F_BG2": 1 << 11,
+     "F_BG3": 1 << 12, "F_FIXRANGE": 1 << 13, "F_FILLBG": 1 << 14, "F_LENS_NOOP": 1 << 15, "F_SRC_VEC": 1 << 16, "F_DST_VEC": 1 << 17,
+     "F_FB_INV": 1 << 18, "F_IS_Y": 1 << 19, "F_T3D": 1 << 20, "F_PIXLIMIT": 1 << 21, "F_WILD": 1 << 22, "F_INTPRO": 1 << 23,
+     "F_FILTER": 1 << 24, "F_SRC_VEC8": 1 << 25, "F_SHORTROW": 1 << 26}
+F_GENERAL_ONLY = 0
+for _n in ("F_HRS", "F_RLIMIT", "F_REFRACT", "F_MESH", "F_HSTRETCH", "F_VSTRETCH", "F_LCA", "F_INROT", "F_BG1", "F_BG2", "F_BG3",
+           "F_FIXRANGE", "F_FILLBG", "F_LENS_NOOP", "F_FB_INV", "F_T3D", "F_PIXLIMIT"):
+    F_GENERAL_ONLY |= F[_n]
+
 ERRORS = {0: "Ok", -1: "BadParams", -2: "SizeTooSmall", -3: "SizeMismatch", -4: "InvalidStride",
           -5: "UnsupportedCombo", -6: "CudaError", -7: "BufferTooSmall", -8: "NoStabilizationData"}
 
@@ -204,6 +216,8 @@ EXPORTS = [
     ("gf_cuda_selftest_filter", C.c_int, [C.c_int, C.c_ulonglong, C.c_int, C.c_int, C.POINTER(C.c_ulonglong)]),
     ("gf_cuda_selftest_certify", C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     ("gf_cuda_plan", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t]),
+    ("gf_cuda_plan_features", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t,
+                                        _P(C.c_uint32)]),
     ("gf_cuda_synchronize", C.c_int, [C.c_void_p]),
     ("gf_cuda_set_overlays", C.c_int, [C.c_void_p, C.c_int]),
     ("gf_cuda_last_error", C.c_char_p, [C.c_void_p]),

@@ -907,9 +907,12 @@ GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_
 // Host-only: which kernel variant would render this frame (no CUDA call, no context).  table_flags: 0 = validated tame tables without
 // IBIS rows, non-zero = anything else.  Returns 0 general, 1 lean, 2 packed, 3 packed + trusted tables, | 0x10 two-pass (plan_frame,
 // the planner run_warp uses), or a negative GF_ERR_*.  A planning aid for integrators and the hook the CPU-only tests use to check
-// the host logic.
-GF_API int gf_cuda_plan(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
-                        const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags, size_t n_planes) {
+// the host logic.  gf_cuda_plan_features also writes the frame's feature word (F_* of warp_kernel.cuh) to *feat_out: the bits
+// fill_uniforms computes, plus F_FILTER when the plan runs the filtered pre-pass (launch() sets that bit at launch time).
+GF_API int gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
+                                 const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags, size_t n_planes,
+                                 uint32_t* feat_out) {
+    if (feat_out) *feat_out = 0;
     if (!params || !in || !out) return GF_ERR_BAD_PARAMS;
     Combo c;
     if (!make_combo(pixel_type, distortion_model, digital_lens, params->interpolation, &c)) return GF_ERR_BAD_PARAMS;
@@ -924,7 +927,13 @@ GF_API int gf_cuda_plan(const gf_kernel_params* params, int pixel_type, int dist
     const Plan pl = plan_frame(c, A, table_flags, job);
     // packed: the trusted path runs when the table's verdict word is 0, which the host knows only for tables it scanned
     const int v = pl.kernel == KV_GENERAL ? 0 : (pl.kernel == KV_LEAN ? 1 : (table_flags == 0 ? 3 : 2));
+    if (feat_out) *feat_out = A.feat | (pl.a_cap > 0.0f ? (uint32_t)F_FILTER : 0u);
     return v | (pl.two_pass ? 0x10 : 0);
+}
+
+GF_API int gf_cuda_plan(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
+                        const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags, size_t n_planes) {
+    return gf_cuda_plan_features(params, pixel_type, distortion_model, digital_lens, in, out, mesh_len, table_flags, n_planes, nullptr);
 }
 
 GF_API int gf_cuda_validate_tables_dev(gf_cuda_ctx* ctx, const float* matrices_dev, size_t matrix_rows) {

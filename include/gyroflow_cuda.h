@@ -301,6 +301,12 @@ GF_API int         gf_cuda_validate_tables_dev(gf_cuda_ctx* ctx, const float* ma
  * Returns 0 general, 1 lean, 2 packed, 3 packed with trusted tables, OR-ed with 0x10 when the two-pass path is used; < 0 on error. */
 GF_API int         gf_cuda_plan(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
                                 const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags, size_t n_planes);
+/* gf_cuda_plan, and the frame's feature word written to *feat_out (0 on error): the per-frame feature bits the kernels branch on
+ * (F_* in csrc/warp_kernel.cuh, mirrored as abi.F), including F_FILTER when the plan runs the packed kernel's filtered pre-pass.
+ * Host-only like gf_cuda_plan; a test hook for the dispatch logic, not a stable interface. */
+GF_API int         gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
+                                         const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags,
+                                         size_t n_planes, uint32_t* feat_out);
 
 /* Preview overlays of the reference's GPU kernels — draw_pixel + draw_safe_area, src/core/gpu/opencl_undistort.cl:109-154, buffer
  * produced by gpu/drawing.rs:8-50 (SURVEY §8 f4).  OFF by default: the CPU path, the parity target, draws none

@@ -17,7 +17,7 @@ def gyro(duration=4.0):
 
 
 def build(case):
-    """case keys: w,h [,ow,oh] pix lens [digital] [interp] [rs] [ts] [stride_pad] [edge_values] plus any KernelParams field override
+    """case keys: w,h [,ow,oh] pix lens [digital] [interp] [rs] [ts] [stride_pad] [edge_values] [flags] [clear_flags] plus any KernelParams field override
     under 'params' and rects under 'in_rect'/'out_rect' (x,y,w,h) with 'in_size'/'out_size' = buffer (w,h)."""
     w, h = case["w"], case["h"]
     ow, oh = case.get("ow", w), case.get("oh", h)
@@ -57,6 +57,8 @@ def build(case):
         p.flags |= abi.FLAG_HORIZONTAL_RS
     if case.get("flags"):
         p.flags |= case["flags"]
+    if case.get("clear_flags"):
+        p.flags &= ~case["clear_flags"]
     rs = case.get("rs", True)
     if case.get("identity"):
         m = np_producer.identity_matrices(p, rows=(h if rs else 1))

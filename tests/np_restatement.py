@@ -76,6 +76,8 @@ def map_coord(x, in_min, in_max, out_min, out_max):      # util.rs:144-147
 
 def fisheye_distort(x, y, z, k):             # opencv_fisheye.rs:72-93
     x = x / z; y = y / z
+    if k[0] == 0 and k[1] == 0 and k[2] == 0 and k[3] == 0:         # :75
+        return x, y
     r = sqrtf(x * x + y * y)
     theta = atanf(r)
     theta2 = theta * theta; theta4 = theta2 * theta2; theta6 = theta4 * theta2; theta8 = theta4 * theta4

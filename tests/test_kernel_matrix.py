@@ -103,11 +103,13 @@ def _aligned(n, fill=0):
 
 
 def build(case, pix, lens, digital, interp, out_len):
-    """cases.build with 64-byte aligned buffers and an output of exactly out_len bytes (+ GUARD sentinel bytes after it)."""
+    """cases.build with 64-byte aligned buffers and an output of exactly out_len bytes (+ GUARD sentinel bytes after it).  The case
+    keys src_offset / dst_offset start the input / output that many bytes past the 64-byte boundary instead."""
     p, src, m, mesh, dst0, _, _, _ = cases.build(dict(case, pix=pix, lens=lens, digital=digital, interp=interp))
-    a = _aligned(src.size)
+    so, do = case.get("src_offset", 0), case.get("dst_offset", 0)
+    a = _aligned(src.size + so)[so:]
     a[:] = src.reshape(-1)
-    dst = _aligned(out_len + GUARD, 0xA5)
+    dst = _aligned(out_len + GUARD + do, 0xA5)[do:]
     return p, a, m, dst
 
 
@@ -120,10 +122,10 @@ def descs(case, p, src, dst, out_len):
                      g.BufferDescription((obw, obh, p.output_stride), dst.data_ptr(), length=out_len))
 
 
-def plan(p, pix, lens, digital, bufs, table_flags):
+def plan(p, pix, lens, digital, bufs, table_flags, mesh_len=0):
     i, o = bufs.input.to_c(), bufs.output.to_c()
     return g.load_library().gf_cuda_plan(C.byref(p), abi.PIXEL_TYPES[pix][0], abi.LENS[lens], abi.LENS[digital] if digital else 0,
-                                         C.byref(i), C.byref(o), 0, table_flags, 1)
+                                         C.byref(i), C.byref(o), mesh_len, table_flags, 1)
 
 
 def set_switch(monkeypatch, switch):
@@ -206,30 +208,39 @@ def test_switches_leave_the_default_plan_alone(monkeypatch):
 # ---- the GPU matrix --------------------------------------------------------------------------------------------------------------
 def render(case, pix, lens, digital, interp, tables, out_len, kinds):
     """Render one cell for each buffer kind in `kinds` ("host" / "device") on one context.  Returns (want, [(kind, got incl. guard,
-    launches)], plan code)."""
+    launches)], plan code).  A case with a mesh (cases.build's mesh / fpd keys) renders with it; DEVICE buffers keep the case's
+    src_offset / dst_offset."""
     import torch
     p, src, m, dst = build(case, pix, lens, digital, interp, out_len)
+    mesh = cases.build(dict(case, pix=pix, lens=lens, digital=digital, interp=interp))[3] if case.get("mesh") else None
+    mesh_len = 0 if mesh is None else mesh.size
     want = dst[:out_len].copy()
-    assert oracle_lib.undistort_image(src, want, p, pix, lens, digital, m) == 0
-    itm = g.FrameTransform(matrices=m, kernel_params=p)
+    assert oracle_lib.undistort_image(src, want, p, pix, lens, digital, m, mesh) == 0
+    itm = g.FrameTransform(matrices=m, kernel_params=p, **({} if mesh is None else dict(mesh_data=mesh)))
     host = descs(case, p, src, dst, out_len)
-    code = plan(p, pix, lens, digital, host, g.load_library().gf_table_flags_host(m.ctypes.data, m.shape[0]) if tables == "host" else 1)
+    code = plan(p, pix, lens, digital, host, g.load_library().gf_table_flags_host(m.ctypes.data, m.shape[0]) if tables == "host" else 1, mesh_len)
     ctx = g.CudaWrapper.new(p, pix, lens, digital, host)
     tm = torch.from_numpy(m).cuda() if tables == "device" else None
+    tmesh = torch.from_numpy(mesh).cuda() if tables == "device" and mesh is not None else None
+
+    def dev(a, off):                    # a device copy of `a` that starts `off` bytes past an allocation's (256-byte aligned) start
+        t = torch.empty(a.size + off, dtype=torch.uint8, device="cuda")
+        t[off:].copy_(torch.from_numpy(a.copy()))
+        return t[off:]
     outs = []
     try:
         for kind in kinds:
             if kind == "host":
                 d = dst.copy(); bufs = descs(case, p, src, d, out_len)
             else:
-                tsrc, d = torch.from_numpy(src.copy()).cuda(), torch.from_numpy(dst.copy()).cuda()
+                tsrc, d = dev(src, case.get("src_offset", 0)), dev(dst, case.get("dst_offset", 0))
                 bufs = descs(case, p, tsrc, d, out_len)
             torch.cuda.synchronize()
             l0 = ctx.launch_count
             if tables == "host":
                 ctx.undistort_image(bufs, itm)
             else:
-                ctx.undistort_image_dev(bufs, p, tm.data_ptr(), m.shape[0])
+                ctx.undistort_image_dev(bufs, p, tm.data_ptr(), m.shape[0], tmesh.data_ptr() if tmesh is not None else 0, mesh_len)
             ctx.synchronize()
             outs.append((kind, d if kind == "host" else d.cpu().numpy(), ctx.launch_count - l0))
     finally:
