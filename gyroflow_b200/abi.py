@@ -210,6 +210,10 @@ EXPORTS = [
     ("gf_cuda_stmap_distort_dev", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("gf_cuda_generate_stmap", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("gf_cuda_stmap_sizes", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+                                      C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("gf_cuda_generate_stmaps_dev", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p]),
     ("gf_cuda_undistort_planes_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("gf_cuda_undistort_planes", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("gf_cuda_selftest_exhaustive", C.c_int, [C.c_int, C.POINTER(C.c_ulonglong)]),

@@ -450,6 +450,52 @@ class DeviceGyro:
         torch.cuda.synchronize()
         return dist.cpu().numpy(), und.cpu().numpy()
 
+    def _clip(self, timestamps_ms, frames):
+        ts = np.ascontiguousarray(timestamps_ms, dtype=np.float64).reshape(-1)
+        fr = np.arange(ts.size, dtype=np.uintp) if frames is None else np.ascontiguousarray(frames, dtype=np.uintp).reshape(-1)
+        assert fr.size == ts.size
+        return ts, fr
+
+    def stmap_sizes(self, distortion_model: str, digital_lens, timestamps_ms, frames=None, per_frame=True, stream=0):
+        """The undistorted size of every frame of a clip's ST maps (gf_cuda_stmap_sizes, stmap.rs:58-77): (new_widths, new_heights) as
+        int32 arrays.  frames: the frame index of each timestamp (default 0, 1, 2, ...)."""
+        ts, fr = self._clip(timestamps_ms, frames)
+        nw, nh = np.zeros(ts.size, np.int32), np.zeros(ts.size, np.int32)
+        rc = self._lib.gf_cuda_stmap_sizes(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
+                                           int(per_frame), fr.ctypes.data, ts.ctypes.data, ts.size, nw.ctypes.data, nh.ctypes.data, stream or None)
+        if rc != 0:
+            raise GyroflowCoreError(rc, (self._lib.gf_cuda_last_error(None) or b"").decode())
+        return nw, nh
+
+    def generate_stmaps(self, distortion_model: str, digital_lens, timestamps_ms, frames=None, per_frame=True, stream=None):
+        """generate_stmaps for a clip (stmap.rs:6-146): stmap_sizes, then gf_cuda_generate_stmaps_dev, which enqueues both maps of every
+        frame on `stream` (default: torch's current stream) and returns without waiting for them.  Returns (dists, undists): per frame a
+        [h, w, 3] and a [new_h, new_w, 3] float32 CUDA tensor, each map byte-identical to generate_stmap of that frame."""
+        import torch
+        ts, fr = self._clip(timestamps_ms, frames)
+        if ts.size == 0:
+            return [], []
+        m, d = abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0
+        # NULL means the gyro object's own stream to the C ABI: torch's legacy default stream (handle 0) goes as cudaStreamLegacy (1)
+        st = (torch.cuda.current_stream().cuda_stream or 1) if stream is None else stream
+        nw, nh = self.stmap_sizes(distortion_model, digital_lens, ts, fr, per_frame, st)
+        w, h, n = self.cp.c.width, self.cp.c.height, ts.size
+        cap = 3 * int((nw.astype(np.int64) * nh).max())
+        dists = [torch.empty((h, w, 3), dtype=torch.float32, device="cuda") for _ in range(n)]
+        bufs = [torch.empty(cap, dtype=torch.float32, device="cuda") for _ in range(n)]
+        if stream and stream != torch.cuda.current_stream().cuda_stream:
+            ext = torch.cuda.ExternalStream(stream)
+            for t in dists + bufs:
+                t.record_stream(ext)             # the allocator must not reuse them before that stream has written them
+        dp = (C.c_void_p * n)(*[t.data_ptr() for t in dists])
+        up = (C.c_void_p * n)(*[t.data_ptr() for t in bufs])
+        rc = self._lib.gf_cuda_generate_stmaps_dev(self._h, C.byref(self.cp.c), m, d, int(per_frame), fr.ctypes.data, ts.ctypes.data, n,
+                                                   nw.ctypes.data, nh.ctypes.data, dp, up, w * h * 3, cap, st or None)
+        if rc != 0:
+            raise GyroflowCoreError(rc, (self._lib.gf_cuda_last_error(None) or b"").decode())
+        undists = [b[: 3 * int(nw[i]) * int(nh[i])].view(int(nh[i]), int(nw[i]), 3) for i, b in enumerate(bufs)]
+        return dists, undists
+
     def close(self):
         if self._h:
             self._lib.gf_cuda_gyro_free(self._h); self._h = None

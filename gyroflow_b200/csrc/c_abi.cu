@@ -18,6 +18,7 @@
 
 #include "kernel_registry.h"
 #include "c_abi_internal.h"
+#include "gyro_dev.h"
 #include <nvtx3/nvToolsExt.h>
 
 using namespace gf;
@@ -769,53 +770,36 @@ __global__ void stmap_rgb_kernel(const uint2* __restrict__ coords, int w, int h,
     o[0] = cx / (float)w; o[1] = 1.0f - (cy / (float)h); o[2] = 0.0f;
 }
 
-extern "C" int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens,
-                                        double timestamp_ms, size_t frame, int use_fovs, double lens_correction_amount,
-                                        const float* points_xy, size_t n, float* out_xy, void* cu_stream);
-extern "C" int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens,
-                                         double timestamp_ms, size_t frame, float* out_rgb_dev, void* cu_stream);
+} // extern "C"
 
-GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
-                                  int per_frame, size_t frame, double timestamp_ms, int32_t* out_new_width, int32_t* out_new_height,
-                                  float* dist_rgb_dev, size_t dist_capacity_floats, float* undist_rgb_dev, size_t undist_capacity_floats,
-                                  void* cu_stream) {
-    if (!g || !cp_user || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    gf_compute_params cp = *cp_user;                                                         // stmap.rs:24-35
+namespace {
+
+// The coordinate-mode warp context of the undistort map (LUMA8, bilinear, pass 1 only) for maps of up to max_w x max_h, with a
+// table slot of max(max_w, max_h) rows.  `any_dev`: a device pointer for the buffer description validation wants (coordinate mode
+// never dereferences it).
+int create_stmap_ctx(int device, int lens, int digital, int max_w, int max_h, void* any_dev, gf_cuda_ctx** out) {
+    gf_kernel_params kq; memset(&kq, 0, sizeof(kq));
+    kq.width = kq.output_width = kq.stride = kq.output_stride = max_w; kq.height = kq.output_height = max_h;
+    kq.matrix_count = 1; kq.interpolation = GF_INTERP_BILINEAR; kq.bytes_per_pixel = 1; kq.pix_element_count = 1;
+    gf_buffer_desc d; memset(&d, 0, sizeof(d));
+    d.width = max_w; d.height = max_h; d.stride = max_w; d.kind = GF_BUF_DEVICE; d.ptr = any_dev; d.len = (size_t)max_w * (size_t)max_h;
+    return gf_cuda_create(out, device, &kq, GF_PIX_LUMA8, lens, digital, &d, &d, 0);
+}
+
+// Both maps of one frame, enqueued on `st` without waiting — stmap.rs:73-116.  `cp`: stmap_params of the user's ComputeParams.  `ctx`:
+// a context of create_stmap_ctx at least new_w x new_h; it is set to this frame's size.
+int enqueue_stmap_frame(gf_cuda_ctx* ctx, gf_cuda_gyro* g, gf_compute_params cp, int distortion_model, int digital_lens, size_t frame,
+                        double timestamp_ms, int new_w, int new_h, float* dist_rgb_dev, float* undist_rgb_dev, cudaStream_t st) {
     const int width = cp.width, height = cp.height;
-    if (width < 4 || height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall");
-    if (!per_frame) cp.frame_readout_time = 0.0;
-    cp.suppress_rotation = 1; cp.fovs = nullptr; cp.n_fovs = 0; cp.minimal_fovs = nullptr; cp.n_minimal_fovs = 0;
-    cp.fov_scale = 1.0; cp.output_width = width; cp.output_height = height;                  // :44-46
-
-    // bbox of the undistorted frame edge: points_around_rect(width, height, 31, 31) with fov_algorithm_margin = 0 (:58-60, fov_iterative.rs:154-175)
-    std::vector<float> rect(2 * RECT_POINTS), und(2 * RECT_POINTS);
-    for (int k = 0; k < RECT_POINTS; ++k) rect_point((float)width, (float)height, 0.0f, k, rect[2 * k], rect[2 * k + 1]);
-    int rc = gf_cuda_undistort_points(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, 0, 1.0, rect.data(), rect.size() / 2, und.data(), cu_stream);
-    if (rc != GF_OK) return fail(nullptr, rc, "gf_cuda_undistort_points failed");
-    float min_x = 0.0f, min_y = 0.0f, max_x = 0.0f, max_y = 0.0f;                             // :62-71 (f32::min / max ignore NaN)
-    for (size_t i = 0; i < und.size(); i += 2) {
-        min_x = fminf(und[i], min_x); min_y = fminf(und[i + 1], min_y);
-        max_x = fmaxf(und[i], max_x); max_y = fmaxf(und[i + 1], max_y);
-    }
-    const float fw = ceilf(max_x - min_x), fh = ceilf(max_y - min_y);
-    // `as usize`: truncating, saturating, NaN -> 0
-    const long long new_w = fw != fw ? 0 : (fw <= 0.0f ? 0 : (fw >= 2147483647.0f ? 2147483647LL : (long long)fw));
-    const long long new_h = fh != fh ? 0 : (fh <= 0.0f ? 0 : (fh >= 2147483647.0f ? 2147483647LL : (long long)fh));
-    *out_new_width = (int32_t)new_w; *out_new_height = (int32_t)new_h;
-    if (new_w < 4 || new_h < 4 || new_w > 32768 || new_h > 32768) return fail(nullptr, GF_ERR_SIZE_MISMATCH, "ST map: undistorted frame size out of range");
-    if (!dist_rgb_dev || !undist_rgb_dev) return GF_OK;                                      // size query
-    if (dist_capacity_floats < (size_t)width * height * 3 || undist_capacity_floats < (size_t)new_w * new_h * 3)
-        return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "ST map output buffers too small");
-
     cp.fov_scale = (double)fmaxf((float)new_w / (float)width, (float)new_h / (float)height);  // :75
-    cp.width = (int)new_w; cp.height = (int)new_h; cp.output_width = (int)new_w; cp.output_height = (int)new_h;
+    cp.width = new_w; cp.height = new_h; cp.output_width = new_w; cp.output_height = new_h;
     gf_kernel_params kp;
     const size_t max_rows = (size_t)std::max(new_w, new_h);
     std::vector<float> mats(max_rows * GF_MATRIX_STRIDE);
     size_t rows = 0;
-    rc = gf_frame_transform_at_timestamp(&cp, timestamp_ms, frame, &kp, mats.data(), max_rows, &rows, nullptr, nullptr);   // :79
+    int rc = gf_frame_transform_at_timestamp(&cp, timestamp_ms, frame, &kp, mats.data(), max_rows, &rows, nullptr, nullptr);   // :79
     if (rc != GF_OK) return fail(nullptr, rc, "gf_frame_transform_at_timestamp failed");
-    kp.width = (int)new_w; kp.height = (int)new_h; kp.output_width = (int)new_w; kp.output_height = (int)new_h;   // :80-84
+    kp.width = new_w; kp.height = new_h; kp.output_width = new_w; kp.output_height = new_h;   // :80-84
     kp.flags = (digital_lens != GF_LENS_NONE ? GF_FLAG_HAS_DIGITAL_LENS : 0) | (cp.readout_horizontal ? GF_FLAG_HORIZONTAL_RS : 0);
     // The closure of :88-109 is undistort_coord's row selection + rotate_and_distort and nothing else: run the warp kernel in
     // coordinate mode with the optional stages switched off (no lens-correction blend, no source-rect map: background mode 3
@@ -824,31 +808,98 @@ GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_u
     kq.lens_correction_amount = 1.0f; kq.background_mode = 3; kq.input_rotation = 0.0f;
     kq.translation2d[0] = kq.translation2d[1] = 0.0f;
     kq.interpolation = GF_INTERP_BILINEAR; kq.bytes_per_pixel = 1; kq.pix_element_count = 1;
-    kq.stride = (int)new_w; kq.output_stride = (int)new_w;
-    kq.source_rect[0] = kq.source_rect[1] = 0; kq.source_rect[2] = (int)new_w; kq.source_rect[3] = (int)new_h;
-    kq.output_rect[0] = kq.output_rect[1] = 0; kq.output_rect[2] = (int)new_w; kq.output_rect[3] = (int)new_h;
+    kq.stride = new_w; kq.output_stride = new_w;
+    kq.source_rect[0] = kq.source_rect[1] = 0; kq.source_rect[2] = new_w; kq.source_rect[3] = new_h;
+    kq.output_rect[0] = kq.output_rect[1] = 0; kq.output_rect[2] = new_w; kq.output_rect[3] = new_h;
     kq.max_pixel_value = 255.0f; kq.pixel_value_limit = 255.0f;
     gf_buffer_desc d; memset(&d, 0, sizeof(d));
-    d.width = (int)new_w; d.height = (int)new_h; d.stride = (int)new_w; d.kind = GF_BUF_DEVICE;
+    d.width = new_w; d.height = new_h; d.stride = new_w; d.kind = GF_BUF_DEVICE;
     d.ptr = undist_rgb_dev; d.len = (size_t)new_w * (size_t)new_h;                          // never dereferenced in coordinate mode
-    {
-        gf_cuda_ctx* raw = nullptr;
-        int device = 0; cudaGetDevice(&device);
-        rc = gf_cuda_create(&raw, device, &kq, GF_PIX_LUMA8, distortion_model, digital_lens, &d, &d, 0);
-        if (rc != GF_OK) return rc;
-        const std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx(raw);
-        cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
-        FrameJob job{&d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};
-        job.coord_only = true;
-        if ((rc = run_warp(ctx.get(), job)) != GF_OK) return rc;
-        const dim3 block(32, 8), grid(((unsigned)new_w + 31) / 32, ((unsigned)new_h + 7) / 8);
-        stmap_rgb_kernel<<<grid, block, 0, st>>>(ctx->coords.ptr, (int)new_w, (int)new_h, (int)new_w, undist_rgb_dev);
-        CK(nullptr, cudaGetLastError());
-        CK(nullptr, cudaStreamSynchronize(st));
-    }
-
+    ctx->width = ctx->output_width = new_w; ctx->height = ctx->output_height = new_h;
+    FrameJob job{&d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};                    // the table is staged through a slot
+    job.coord_only = true;
+    if ((rc = run_warp(ctx, job)) != GF_OK) return rc;
+    const dim3 block(32, 8), grid(((unsigned)new_w + 31) / 32, ((unsigned)new_h + 7) / 8);
+    stmap_rgb_kernel<<<grid, block, 0, st>>>(ctx->coords.ptr, new_w, new_h, new_w, undist_rgb_dev);
+    CK(nullptr, cudaGetLastError());
     cp.width = width; cp.height = height; cp.output_width = width; cp.output_height = height;   // :111-112 (fov_scale stays)
-    rc = gf_cuda_stmap_distort_dev(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, dist_rgb_dev, cu_stream);
+    return gf_cuda_stmap_distort_dev(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, dist_rgb_dev, st);
+}
+
+} // namespace
+
+extern "C" {
+
+GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
+                                  int per_frame, size_t frame, double timestamp_ms, int32_t* out_new_width, int32_t* out_new_height,
+                                  float* dist_rgb_dev, size_t dist_capacity_floats, float* undist_rgb_dev, size_t undist_capacity_floats,
+                                  void* cu_stream) {
+    if (!g || !cp_user || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    int rc = gf_cuda_stmap_sizes(g, cp_user, distortion_model, digital_lens, per_frame, &frame, &timestamp_ms, 1, out_new_width, out_new_height, cu_stream);
+    if (rc != GF_OK) return rc;
+    if (!dist_rgb_dev || !undist_rgb_dev) return GF_OK;                                      // size query
+    const int new_w = *out_new_width, new_h = *out_new_height;
+    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
+    if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < (size_t)new_w * new_h * 3)
+        return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "ST map output buffers too small");
+    gf_cuda_ctx* raw = nullptr;
+    if ((rc = create_stmap_ctx(g->device, distortion_model, digital_lens, new_w, new_h, undist_rgb_dev, &raw)) != GF_OK) return rc;
+    const std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx(raw);
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
+    if ((rc = enqueue_stmap_frame(ctx.get(), g, cp, distortion_model, digital_lens, frame, timestamp_ms, new_w, new_h, dist_rgb_dev, undist_rgb_dev, st)) != GF_OK)
+        return rc;
+    CK(nullptr, cudaStreamSynchronize(st));
+    return GF_OK;
+}
+
+GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens, int per_frame,
+                                       const size_t* frames, const double* timestamps_ms, size_t n,
+                                       const int32_t* new_w, const int32_t* new_h, float* const* dist_rgb_dev, float* const* undist_rgb_dev,
+                                       size_t dist_capacity_floats, size_t undist_capacity_floats, void* cu_stream) {
+    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    if (n == 0) return GF_OK;
+    if (!frames || !timestamps_ms || !new_w || !new_h || !dist_rgb_dev || !undist_rgb_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
+    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall");
+    Combo combo;
+    if (!make_combo(GF_PIX_LUMA8, distortion_model, digital_lens, GF_INTERP_BILINEAR, &combo) || !combo.kernels[KV_GENERAL] ||
+        !point_path_supported(distortion_model, digital_lens))
+        return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "no ST-map kernels for this (lens, digital lens) pair");
+    // every argument is checked before the first launch
+    int max_w = 0, max_h = 0;
+    size_t max_px = 0;
+    for (size_t i = 0; i < n; ++i) {
+        const std::string at = " at entry " + std::to_string(i);
+        if (!dist_rgb_dev[i] || !undist_rgb_dev[i]) return fail(nullptr, GF_ERR_BAD_PARAMS, "null map buffer" + at);
+        if (!stmap_size_ok(new_w[i], new_h[i])) return fail(nullptr, GF_ERR_SIZE_MISMATCH, "ST map: undistorted frame size out of range" + at);
+        if (new_w[i] > 16384) return fail(nullptr, GF_ERR_BAD_PARAMS, "ST map: undistorted width beyond the warp's 16384" + at);
+        const size_t px = (size_t)new_w[i] * (size_t)new_h[i];
+        if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < px * 3)
+            return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "ST map output buffers too small" + at);
+        max_w = std::max(max_w, new_w[i]); max_h = std::max(max_h, new_h[i]); max_px = std::max(max_px, px);
+    }
+    CK(nullptr, cudaSetDevice(g->device));
+    const cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    if (!g->stmap_done) CK(nullptr, create_event(g->stmap_done));
+    // The context is the previous job's: this stream waits for that job on the device.  A context too small or of another lens pair is
+    // replaced, which waits for the previous job on the host.
+    CK(nullptr, cudaStreamWaitEvent(st, g->stmap_done.get(), 0));
+    if (!g->stmap_ctx || g->stmap_ctx->combo.lens != distortion_model || g->stmap_ctx->combo.digital != digital_lens ||
+        g->stmap_ctx->max_rows < (size_t)std::max(max_w, max_h)) {
+        CK(nullptr, cudaEventSynchronize(g->stmap_done.get()));
+        g->stmap_ctx.reset();
+        gf_cuda_ctx* raw = nullptr;
+        const int rc = create_stmap_ctx(g->device, distortion_model, digital_lens, max_w, max_h, undist_rgb_dev[0], &raw);
+        if (rc != GF_OK) return rc;
+        g->stmap_ctx.reset(raw);
+    }
+    gf_cuda_ctx* const ctx = g->stmap_ctx.get();
+    CK(nullptr, ctx->coords.reserve(max_px, st));             // sized once for the largest frame (growing waits for the stream)
+    int rc = GF_OK;
+    for (size_t i = 0; i < n && rc == GF_OK; ++i)
+        rc = enqueue_stmap_frame(ctx, g, cp, distortion_model, digital_lens, frames[i], timestamps_ms[i], new_w[i], new_h[i],
+                                 dist_rgb_dev[i], undist_rgb_dev[i], st);
+    CK(nullptr, cudaEventRecord(g->stmap_done.get(), st));    // also after a failure: whatever was enqueued still uses the context
     return rc;
 }
 

@@ -103,6 +103,20 @@ FrameTiming frame_timing(const gf_compute_params* cp, size_t frame, double times
 CameraStab camera_stab_at(const gf_compute_params* cp, size_t frame, bool framebuffer_inverted, const StabSplines* splines);
 // the lens model is the identity for these coefficients (c_abi.cu)
 bool lens_noop(int lens, const float* k);
+// the point path (zoom_kernel.cu) compiles this (lens, digital lens) pair
+bool point_path_supported(int lens, int digital);
+
+// What generate_stmaps does to the user's ComputeParams before either map (stmap.rs:24-35, :44-46): rotation suppressed, fovs cleared,
+// no readout time unless per_frame, fov_scale 1 and the output size the frame size.
+inline gf_compute_params stmap_params(const gf_compute_params& user, int per_frame) {
+    gf_compute_params cp = user;
+    if (!per_frame) cp.frame_readout_time = 0.0;
+    cp.suppress_rotation = 1; cp.fovs = nullptr; cp.n_fovs = 0; cp.minimal_fovs = nullptr; cp.n_minimal_fovs = 0;
+    cp.fov_scale = 1.0; cp.output_width = cp.width; cp.output_height = cp.height;
+    return cp;
+}
+// The undistorted sizes gf_cuda_generate_stmap accepts (the warp that renders the undistort map takes widths up to 16384 besides)
+inline bool stmap_size_ok(int w, int h) { return w >= 4 && h >= 4 && w <= 32768 && h <= 32768; }
 
 } // namespace gf
 

@@ -380,6 +380,7 @@ GF_API void gf_cuda_gyro_free(gf_cuda_gyro* g) {
     if (!g) return;
     cudaSetDevice(g->device);
     if (g->stream) cudaStreamSynchronize(g->stream.get());
+    if (g->stmap_done) cudaEventSynchronize(g->stmap_done.get());     // the last ST-map job, which may run on a caller's stream
     delete g;
     (void)cudaGetLastError();       // a failed teardown call must not fail the thread's next call
 }

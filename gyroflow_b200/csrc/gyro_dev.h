@@ -22,6 +22,9 @@ struct gf_cuda_gyro {
     static constexpr unsigned kScratchPairs = 64;
     gf::GrowBuf<unsigned> d_scratch; unsigned next_scratch = 0;
     gf::Stream stream;
+    // ST-map jobs (gf_cuda_generate_stmaps_dev): the coordinate-mode warp context they share, and the end of the last job on its stream
+    std::unique_ptr<gf_cuda_ctx, gf::Deleter<gf_cuda_destroy>> stmap_ctx;
+    gf::Event stmap_done;
 
     gf::Track org_track() const { return gf::Track{ d_org_ts.ptr, d_org_q.ptr, n_org }; }
     // the uploaded multi-point sync offsets; `scalar_ms` (gyro_offset_ms) applies when there are none

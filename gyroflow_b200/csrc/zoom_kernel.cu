@@ -232,13 +232,43 @@ __global__ void __launch_bounds__(128) points_kernel(const ZoomArgs A, const Zoo
     if (pts) { out[2 * i] = ox; out[2 * i + 1] = oy; }
     else     { out[3 * i] = ox / (float)grid_w; out[3 * i + 1] = 1.0f - (oy / (float)grid_h); out[3 * i + 2] = 0.0f; }
 }
-// Both kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye
+// One frame of gf_cuda_stmap_sizes: what gf_cuda_undistort_points derives for it.  The lens may change per frame (lens_per_frame), so
+// the call-wide values are per frame here.
+struct StmapFrame { ZoomArgs A; ZoomFrame F; };
+
+// The undistorted size of one frame per CTA — stmap.rs:58-77: the 120 points_around_rect(w, h, 31, 31) edge points with margin 0
+// (fov_iterative.rs:154-175) through undistort_points, their bounding box folded in order from 0 with f32::min / max (NaN is
+// ignored, :62-71), then `ceil(max - min) as usize` for each extent.
+template <int LENS, int DIGITAL>
+__global__ void __launch_bounds__(128) stmap_size_kernel(const StmapFrame* __restrict__ frames, float w, float h, int2* __restrict__ out) {
+    __shared__ float und[2 * RECT_POINTS];
+    const StmapFrame& S = frames[blockIdx.x];
+    const int tid = threadIdx.x;
+    if (tid < RECT_POINTS) {
+        float x, y; rect_point(w, h, 0.0f, tid, x, y);
+        undistort_point_rs<LENS, DIGITAL>(S.A, S.F, x, y, (size_t)tid, und[2 * tid], und[2 * tid + 1]);
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    float min_x = 0.0f, min_y = 0.0f, max_x = 0.0f, max_y = 0.0f;
+    for (int i = 0; i < RECT_POINTS; ++i) {
+        min_x = fminf(und[2 * i], min_x); min_y = fminf(und[2 * i + 1], min_y);
+        max_x = fmaxf(und[2 * i], max_x); max_y = fmaxf(und[2 * i + 1], max_y);
+    }
+    const float fw = ceilf(max_x - min_x), fh = ceilf(max_y - min_y);
+    // `as usize`: truncating, saturating, NaN -> 0 (kept within int32; anything that large is out of range anyway)
+    auto as_size = [](float v) { return v != v ? 0 : (v <= 0.0f ? 0 : (v >= 2147483647.0f ? 2147483647 : (int)v)); };
+    out[blockIdx.x] = make_int2(as_size(fw), as_size(fh));
+}
+
+// The kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye
 // model, GoPro warp the GoPro model).
 struct ZoomKernels {
     void (*find_fov)(const ZoomArgs, const ZoomFrame*, double*);
     void (*points)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
+    void (*stmap_size)(const StmapFrame*, float, float, int2*);
 };
-template <int LENS, int DIGITAL> ZoomKernels kernels_of() { return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL> }; }
+template <int LENS, int DIGITAL> ZoomKernels kernels_of() { return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL> }; }
 template <int LENS> ZoomKernels pick_digital(int digital) {
     switch (digital) {
     case GF_LENS_NONE:             return kernels_of<LENS, GF_LENS_NONE>();
@@ -249,7 +279,7 @@ template <int LENS> ZoomKernels pick_digital(int digital) {
     case GF_LENS_GOPRO_WARP:       if (LENS == GF_LENS_GOPRO) return kernels_of<LENS, GF_LENS_GOPRO_WARP>();                break;
     default: break;
     }
-    return { nullptr, nullptr };
+    return { nullptr, nullptr, nullptr };
 }
 ZoomKernels pick_kernels(int lens, int digital) {
     switch (lens) {
@@ -262,7 +292,7 @@ ZoomKernels pick_kernels(int lens, int digital) {
     case GF_LENS_SONY:               return pick_digital<GF_LENS_SONY>(digital);
     case GF_LENS_GENERIC_POLYNOMIAL: return pick_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
     case GF_LENS_GOPRO:              return pick_digital<GF_LENS_GOPRO>(digital);
-    default: return { nullptr, nullptr };
+    default: return { nullptr, nullptr, nullptr };
     }
 }
 
@@ -333,6 +363,8 @@ static gf_compute_params resolve_point_lens(const gf_compute_params& cp, size_t 
     }
     return r;
 }
+
+bool gf::point_path_supported(int lens, int digital) { return pick_kernels(lens, digital).points != nullptr; }
 
 // ---- the temporal filters of zoom_dynamic.rs, on the host like in the reference ----
 
@@ -466,6 +498,47 @@ GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* c
     const size_t n = (size_t)cp->width * (size_t)cp->height;
     k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);
     CK(nullptr, cudaGetLastError());
+    return GF_OK;
+}
+
+// The undistorted size of every frame of an ST-map job (stmap.rs:58-77), one CTA per frame.  Each frame's record is what
+// gf_cuda_undistort_points(use_fovs = 0, lens_correction_amount = 1) builds for it, so the sizes are those of gf_cuda_generate_stmap.
+GF_API int gf_cuda_stmap_sizes(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens, int per_frame,
+                               const size_t* frames, const double* timestamps_ms, size_t n,
+                               int32_t* out_new_width, int32_t* out_new_height, void* cu_stream) {
+    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    if (n == 0) return GF_OK;
+    if (!frames || !timestamps_ms || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    if (n > 0x7fffffffu) return fail(nullptr, GF_ERR_BAD_PARAMS, "too many frames");
+    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
+    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall");
+    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
+    if (!k.stmap_size) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "no point-path kernel for this (lens, digital lens) pair");
+    CK(nullptr, cudaSetDevice(g->device));
+    std::vector<StmapFrame> hf(n);
+    for (size_t i = 0; i < n; ++i) {
+        const gf_compute_params rcp = resolve_point_lens(cp, frames[i]);
+        setup_points_args(g, rcp, distortion_model, points_fov(&rcp, frames[i], false, timestamps_ms[i]), hf[i].A);
+        hf[i].F = frame_uniforms(g, rcp, hf[i].A, timestamps_ms[i], frames[i], 1.0, false);
+    }
+    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    GrowBuf<StmapFrame> d_frames; GrowBuf<int2> d_out;
+    CK(nullptr, d_frames.reserve(n, st));
+    CK(nullptr, d_out.reserve(n, st));
+    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(StmapFrame), cudaMemcpyHostToDevice, st));
+    k.stmap_size<<<(unsigned)n, 128, 0, st>>>(d_frames.ptr, (float)cp.width, (float)cp.height, d_out.ptr);
+    CK(nullptr, cudaGetLastError());
+    std::vector<int2> sizes(n);
+    CK(nullptr, cudaMemcpyAsync(sizes.data(), d_out.ptr, n * sizeof(int2), cudaMemcpyDeviceToHost, st));
+    CK(nullptr, cudaStreamSynchronize(st));
+    size_t bad = n;
+    for (size_t i = 0; i < n; ++i) {
+        out_new_width[i] = sizes[i].x; out_new_height[i] = sizes[i].y;
+        if (bad == n && !stmap_size_ok(sizes[i].x, sizes[i].y)) bad = i;
+    }
+    if (bad < n)
+        return fail(nullptr, GF_ERR_SIZE_MISMATCH, "ST map: undistorted frame size out of range: " + std::to_string(sizes[bad].x) + "x" +
+                    std::to_string(sizes[bad].y) + " at entry " + std::to_string(bad) + " (frame " + std::to_string(frames[bad]) + ")");
     return GF_OK;
 }
 

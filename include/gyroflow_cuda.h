@@ -481,6 +481,25 @@ GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp, 
                                   int per_frame, size_t frame, double timestamp_ms, int32_t* out_new_width, int32_t* out_new_height,
                                   float* dist_rgb_dev, size_t dist_capacity_floats, float* undist_rgb_dev, size_t undist_capacity_floats,
                                   void* cu_stream);
+/* ST maps of a whole clip — generate_stmaps(stab, per_frame = true), stmap.rs:6-146, for `n` frames (frames[i] at timestamps_ms[i]), in
+ * two calls, each map byte-identical to gf_cuda_generate_stmap of the same frame.
+ * gf_cuda_stmap_sizes: new_width / new_height of every frame (the bounding box of :58-77), one CTA per frame.  Synchronous: it returns
+ *   the sizes.  Every output entry is written; a frame whose size is outside 4..32768 fails the call with GF_ERR_SIZE_MISMATCH and
+ *   gf_cuda_last_error(NULL) names the first such frame.  Size the buffers from the largest entries.
+ * gf_cuda_generate_stmaps_dev: both maps of every frame into dist_rgb_dev[i] (width x height, >= dist_capacity_floats floats) and
+ *   undist_rgb_dev[i] (new_w[i] x new_h[i], >= undist_capacity_floats floats), as the single-frame call writes them.  Every argument is
+ *   checked before anything is enqueued (a new_w wider than the warp's 16384 is GF_ERR_BAD_PARAMS).  The work runs on cu_stream (NULL:
+ *   the gyro object's stream) and the call returns once it is enqueued: the per-frame tables go through a ring of four page-locked
+ *   slots, so the host may wait for frame i - 4 before it stages frame i, never for the last frames.  The warp context of the job is
+ *   kept by the gyro object for the next job; a later job on another stream is ordered after this one on the device.
+ * n == 0: nothing is written, GF_OK.  `cp` is the user's ComputeParams, as for gf_cuda_generate_stmap. */
+GF_API int gf_cuda_stmap_sizes(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, int per_frame,
+                               const size_t* frames, const double* timestamps_ms, size_t n,
+                               int32_t* out_new_width, int32_t* out_new_height, void* cu_stream);
+GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, int per_frame,
+                                       const size_t* frames, const double* timestamps_ms, size_t n,
+                                       const int32_t* new_w, const int32_t* new_h, float* const* dist_rgb_dev, float* const* undist_rgb_dev,
+                                       size_t dist_capacity_floats, size_t undist_capacity_floats, void* cu_stream);
 
 GF_API int gf_zoom_dynamic_compute(const double* fov_minimal, size_t n, double window_s, double fps, int method, double* out);
 
