@@ -259,7 +259,12 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     };
     if (!(int_map_ok(A.omap_x) && int_map_ok(A.omap_y))) A.feat |= F_WILD;
     // integer prologue of the packed kernel: identity maps -> opx = (x - in_min) + add with integer in_min / add
-    A.hot.rect[0] = A.src_rect[0]; A.hot.rect[1] = A.src_rect[1]; A.hot.rect[2] = A.interior_span[0]; A.hot.rect[3] = A.interior_span[1];
+    // the packed kernel's 8-bit sampler (it only runs without F_WILD: then 0 <= rx0, ry0 <= 2^16 and span < 2^17, far from overflow):
+    // the source rect's origin folded into the rounding word and into the gather's base address
+    const bool tame_rect = (A.feat & F_WILD) == 0;
+    A.hot.wbias[0] = 0x4affffff + (tame_rect ? 64 * A.src_rect[0] : 0); A.hot.wbias[1] = 0x4affffff + (tame_rect ? 64 * A.src_rect[1] : 0);
+    A.hot.wlim[0] = 64u * (unsigned)A.interior_span[0] + 63u; A.hot.wlim[1] = 64u * (unsigned)A.interior_span[1] + 63u;
+    A.hot.src = tame_rect ? src + ((long long)A.src_rect[1] * (long long)p->stride + (long long)A.src_rect[0] * (long long)bpp) : src;
     if (A.omap_x.identity && A.omap_y.identity && A.omap_x.add == truncf(A.omap_x.add) && A.omap_y.add == truncf(A.omap_y.add) &&
         fabsf(A.omap_x.add) < 0x1p20f && fabsf(A.omap_y.add) < 0x1p20f && fabsf(A.omap_x.in_min) < 0x1p20f && fabsf(A.omap_y.in_min) < 0x1p20f) {
         A.hot.x_off = (int)A.omap_x.add - (int)A.omap_x.in_min; A.hot.y_off = (int)A.omap_y.add - (int)A.omap_y.in_min;

@@ -134,10 +134,14 @@ struct WarpArgs {
     // packed kernel: per-frame integers that replace the float rect map + bounds test of :546-551 when both output maps are the
     // identity (F_INTPRO), and the sampler's rect constants side by side (one 128-bit constant load)
     struct X2Hot {
+        const uint8_t* src;         // the source pixel (rx0, ry0): base address of the interior 8-bit gather
         int x_off, y_off;           // opx == (float)(x + x_off), opy likewise (exact: integers below 2^24)
         int x0, x1, y0, y1;         // pixel (x, y) is written iff x0 <= x < x1 and y0 <= y < y1 (rows that do not fit the buffer folded in) ...
         int full_rows, last_cols;   // ... and, with F_SHORTROW only, it fits the buffer: y < full_rows, or y == full_rows and x < last_cols
-        int rect[4];                // rx0, ry0, span_x, span_y
+        // 8-bit sampler, per axis: wbias = 0x4affffff + 64 * rx0 turns bits(RZ(64 u + 2^23)) into w - 64 * rx0 (w: round_half_away_w
+        // in warp_kernel_x2.cuh), and the footprint is interior iff that word, unsigned, is <= wlim = 64 * span + 63
+        int wbias[2];
+        unsigned wlim[2];
     } hot;
 };
 

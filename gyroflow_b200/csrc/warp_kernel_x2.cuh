@@ -521,10 +521,9 @@ GF_DEV int round_away_i32(float t) {
 // whenever the exact result is < 0 (it may also be -1 where the exact result is 0);  t >= 2^22 (or +inf): some value >= 2^22.
 // Callers either clamp to [0, lim] with lim < 2^22 (then the result is exact for every input except NaN -> 0, which is also
 // what the reference gives) or treat every negative / huge result as "not interior" and recompute exactly out of line.
-template <bool BOUNDED = false>     // BOUNDED: the caller guarantees |a2| < 2^23 (no NaN), the max() is not needed
 GF_DEV void round_half_away_w(f2 a2, int& wa, int& wb) {
-    const float sa = __fadd_rz(BOUNDED ? a2.x : fmaxf(a2.x, -4.0f), 8388608.0f);
-    const float sb = __fadd_rz(BOUNDED ? a2.y : fmaxf(a2.y, -4.0f), 8388608.0f);
+    const float sa = __fadd_rz(fmaxf(a2.x, -4.0f), 8388608.0f);
+    const float sb = __fadd_rz(fmaxf(a2.y, -4.0f), 8388608.0f);
     wa = __float_as_int(sa) - 0x4affffff; wb = __float_as_int(sb) - 0x4affffff;
 }
 // max(min(round(t) as i32, lim), 0) for both lanes, lim < 2^22
@@ -563,21 +562,46 @@ static __device__ __noinline__ void shade_cold(bool ok, float u, float v, const 
     PIX::store(out, true, pixel);
 }
 
+// The 8-bit sampler's rounding word for |t| < 2^16: bits(RZ(64 t + 2^23)) - bias, i.e. round_half_away_w(64 t) - 64 * r0 with the
+// source rect's origin r0 folded into bias (X2Hot::wbias).  64 t is exact, so one FFMA.RZ rounds the same sum as FMUL + FADD.RZ.
+GF_DEV int hot_w(float t, int bias) { return __float_as_int(__fmaf_rz(t, 64.0f, 8388608.0f)) - bias; }
+GF_DEV bool hot_interior(int wu, int wv, const WarpArgs& A) { return ((unsigned)wu <= A.hot.wlim[0]) & ((unsigned)wv <= A.hot.wlim[1]); }
+
+// sample_u8_bilinear from the words of hot_w, with both weights doubled: w & 62 is 2 * fx straight from the word, and the row weights
+// (64 - 2 fy, 2 fy) pack into one dp2a operand as 64 + 255 * (2 fy).  Every product and sum is an integer below 2^16 per 16-bit lane
+// (255 * 64) and 4 N < 2^20 in total, so 4 N >> 12 == N >> 10 bit for bit.  Returns trunc(sum / 1024) per channel.
+template <class PIX>
+GF_DEV void sample_u8_hot(int wu, int wv, const WarpArgs& A, uint32_t (&s)[PIX::COUNT]) {
+    constexpr int C = PIX::COUNT;
+    const uint32_t fx2 = (uint32_t)wu & 62u, fy2 = (uint32_t)wv & 62u;
+    const uint32_t wx0 = 64u - fx2, wx1 = fx2;
+    const uint32_t wy = 64u + 255u * fy2;                                            // dp2a bytes: 64 - 2 fy, 2 fy
+    const uint8_t* row0 = A.hot.src + ((long long)(wv >> 6) * (long long)A.p.stride + (long long)(wu >> 6) * (long long)C);
+    const uint8_t* row1 = row0 + A.p.stride;
+    const uint32_t p00 = PIX::load_packed(row0), p01 = PIX::load_packed(row0 + C);
+    const uint32_t p10 = PIX::load_packed(row1), p11 = PIX::load_packed(row1 + C);
+    const uint32_t he0 = (p00 & 0x00ff00ffu) * wx0 + (p01 & 0x00ff00ffu) * wx1;      // row 0: ch0 | ch2 << 16
+    const uint32_t he1 = (p10 & 0x00ff00ffu) * wx0 + (p11 & 0x00ff00ffu) * wx1;      // row 1
+    s[0] = __dp2a_lo(__byte_perm(he0, he1, 0x5410), wy, 0u) >> 12;
+    if (C > 2) s[C > 2 ? 2 : 0] = __dp2a_lo(__byte_perm(he0, he1, 0x7632), wy, 0u) >> 12;
+    if (C > 1) {
+        const uint32_t ho0 = __byte_perm(p00, 0u, 0x4341) * wx0 + __byte_perm(p01, 0u, 0x4341) * wx1;   // ch1 | ch3 << 16
+        const uint32_t ho1 = __byte_perm(p10, 0u, 0x4341) * wx0 + __byte_perm(p11, 0u, 0x4341) * wx1;
+        s[1] = __dp2a_lo(__byte_perm(ho0, ho1, 0x5410), wy, 0u) >> 12;
+        if (C > 3) s[C > 3 ? 3 : 0] = __dp2a_lo(__byte_perm(ho0, ho1, 0x7632), wy, 0u) >> 12;
+    }
+}
+
 // sampling + conversion + store of one pixel, lean feature set (no fix_range, background mode 0, pixel_value_limit >= max).
-// wu, wv: round_half_away_w of 64 * u, 64 * v (8-bit formats only).
+// wu, wv: hot_w of u, v (8-bit formats only).
 template <class PIX>
 GF_DEV void shade_lean(bool ok, bool far, float u, float v, int wu, int wv, const WarpArgs& A, uint8_t* __restrict__ out) {
     constexpr int C = PIX::COUNT;
     if (PIX::SCALAR == SC_U8) {
-        const int sx0 = wu >> 1, sy0 = wv >> 1;
-        const int sx = sx0 >> 5, sy = sy0 >> 5;
         // interior_span < 2^17 (host): negative and >= 2^22 results of the rounding shortcut can never pass
-        const bool interior = ok & !far & ((unsigned)(sx - A.hot.rect[0]) <= (unsigned)A.hot.rect[2]) & ((unsigned)(sy - A.hot.rect[1]) <= (unsigned)A.hot.rect[3]);
-        if (interior) {
-            uint32_t N[C], s[C];
-            sample_u8_bilinear<PIX>(sx0, sy0, A, N);
-            #pragma unroll
-            for (int ch = 0; ch < C; ++ch) s[ch] = N[ch] >> 10;      // trunc(N / 1024); N / 1024 <= 255 <= pixel_value_limit
+        if (ok & !far & hot_interior(wu, wv, A)) {
+            uint32_t s[C];
+            sample_u8_hot<PIX>(wu, wv, A, s);      // trunc(N / 1024) <= 255 <= pixel_value_limit
             PIX::store_scalars(out, true, s);
         } else {
             shade_cold<PIX>(ok, u, v, A, out);
@@ -613,8 +637,8 @@ static __device__ __noinline__ void finish_pair_cold(const WarpArgs& A, int x, i
     const unsigned long long off_a = (unsigned long long)y0 * (unsigned long long)A.p.output_stride + (unsigned long long)x * (unsigned long long)PIX::BYTES;
     int wu_a = 0, wu_b = 0, wv_a = 0, wv_b = 0;
     if (PIX::SCALAR == SC_U8) {      // as on the hot path; the value of a far lane is not used (`interior` is false for it)
-        round_half_away_w<true>(p2::mul(p2::mk(c.ua, c.ub), p2::bc(64.0f)), wu_a, wu_b);
-        round_half_away_w<true>(p2::mul(p2::mk(c.va, c.vb), p2::bc(64.0f)), wv_a, wv_b);
+        wu_a = hot_w(c.ua, A.hot.wbias[0]); wv_a = hot_w(c.va, A.hot.wbias[1]);
+        wu_b = hot_w(c.ub, A.hot.wbias[0]); wv_b = hot_w(c.vb, A.hot.wbias[1]);
     }
     if (wr_a) shade_lean<PIX>(ok_a, (c.ok & 4) != 0, c.ua, c.va, wu_a, wv_a, A, A.dst + off_a);
     if (wr_b) shade_lean<PIX>(ok_b, (c.ok & 8) != 0, c.ub, c.vb, wu_b, wv_b, A, A.dst + off_a + (unsigned long long)A.p.output_stride);
@@ -722,9 +746,18 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
         return;
     }
     int wu_a = 0, wu_b = 0, wv_a = 0, wv_b = 0;
-    if (PIX::SCALAR == SC_U8) {                          // (u * 32).round() for both pixels: 64 * u == 2 * (32 * u) exactly, inside the
-        round_half_away_w<true>(mul(u, bc(64.0f)), wu_a, wu_b);                    // unguarded shortcut's domain
-        round_half_away_w<true>(mul(v, bc(64.0f)), wv_a, wv_b);
+    if (PIX::SCALAR == SC_U8) {                          // (u * 32).round() for both pixels, inside the unguarded shortcut's domain
+        wu_a = hot_w(u.x, A.hot.wbias[0]); wv_a = hot_w(v.x, A.hot.wbias[1]);
+        wu_b = hot_w(u.y, A.hot.wbias[0]); wv_b = hot_w(v.y, A.hot.wbias[1]);
+        if (wr_a & wr_b & hot_interior(wu_a, wv_a, A) & hot_interior(wu_b, wv_b, A)) {     // nearly every pair: one straight block
+            constexpr int C = PIX::COUNT;
+            uint32_t sa[C], sb[C];
+            sample_u8_hot<PIX>(wu_a, wv_a, A, sa);
+            sample_u8_hot<PIX>(wu_b, wv_b, A, sb);
+            PIX::store_scalars(A.dst + off_a, true, sa);
+            PIX::store_scalars(A.dst + off_b, true, sb);
+            return;
+        }
     }
     if (wr_a) shade_lean<PIX>(true, false, u.x, v.x, wu_a, wv_a, A, A.dst + off_a);                     // :615-622
     if (wr_b) shade_lean<PIX>(true, false, u.y, v.y, wu_b, wv_b, A, A.dst + off_b);
