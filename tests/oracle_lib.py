@@ -85,6 +85,17 @@ def undistort_point(lens, x, y, params):
     return (ox.value, oy.value) if ok else None
 
 
+def undistort_coord(x, y, params, matrices, lens, digital_lens, mesh=None):
+    """undistort_coord of cpu_undistort.rs:421-517 for output buffer position (x, y) (float32): the source position in buffer
+    coordinates, or None."""
+    lib = load(); ou, ov = C.c_float(), C.c_float()
+    m = np.ascontiguousarray(matrices, dtype=np.float32)
+    mesh = np.zeros(0, np.float32) if mesh is None else np.ascontiguousarray(mesh, dtype=np.float32)
+    ok = lib.gf_oracle_undistort_coord(float(x), float(y), C.byref(params), m.ctypes.data, abi.LENS[lens], abi.LENS[digital_lens] if digital_lens else 0,
+                                       mesh.ctypes.data if mesh.size else None, mesh.size, C.byref(ou), C.byref(ov))
+    return (np.float32(ou.value), np.float32(ov.value)) if ok else None
+
+
 def find_fovs(cp, lens, digital_lens, timestamps_ms, margin=2.0):
     """FovIterative::compute with the calculate_fovs adjustments (zooming/mod.rs:41-49): oracle, one frame at a time."""
     lib = load()

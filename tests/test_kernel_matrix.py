@@ -1,8 +1,9 @@
 """Every compiled warp kernel against the CPU oracle, cell by cell.
 
 A cell is one (lens pair, pixel type, kernel variant).  The pairs are the ones the library compiles (the 21 the reference
-pre-compiles), the pixel types all 13, and the variants the seven ways a frame can be rendered (MODES): the packed kernel on its
-trusted and on its guarded path, the lean and the general kernel, and the three coordinate passes of the two-pass path.  A switch
+pre-compiles), the pixel types all 13, and the variants the nine ways a frame can be rendered (MODES): the packed kernel on its
+trusted and on its guarded path, the lean and the general kernel, the three coordinate passes of the two-pass path, and the lean and
+general coordinate passes with EWA's two Jacobian probe passes.  A switch
 (GF_DISABLE_X2, GF_DISABLE_LEAN) or the tables' provenance selects the variant; gf_cuda_plan, which shares the planner with the
 rendering call, says which one a frame takes.
 
@@ -38,8 +39,16 @@ MODES = [
     ("packed-coords", None, "Lanczos4", "host", 0x13),
     ("lean-coords", "GF_DISABLE_X2", "Lanczos4", "host", 0x11),
     ("general-coords", "GF_DISABLE_LEAN", "Lanczos4", "host", 0x10),
+    # EWA: three coordinate maps (the pixel and its two Jacobian probes) and no packed form.  The kernel reads the filter only as
+    # KernelParams::ewa_coeffs, so the two variants take two different filters rather than all four each.
+    ("lean-ewa", None, "EWA: RobidouxSharp", "host", 0x11),
+    ("general-ewa", "GF_DISABLE_LEAN", "EWA: Catmull-Rom", "host", 0x10),
 ]
-W, H = 75, 43           # not a multiple of the 32-wide block nor of the packed kernel's 8-row tile: a lone last row is left over
+# (lens, digital, geometry) cells EWA cannot be compared in: in geometry B, next to its NaN centres, (opencv_fisheye, gopro_hyperview)
+# has written pixels whose Jacobian probes give footprints past the kernel's 2^22-tap guard, up to a saturated i32 box that the oracle
+# would sum ~1e19 taps for (test_ewa_resampler.test_geometry_b_footprints pins both)
+EWA_UNCOMPARABLE = {("opencv_fisheye", "gopro_hyperview", "B")}
+W, H = 75, 43          # not a multiple of the 32-wide block nor of the packed kernel's 8-row tile: a lone last row is left over
 CUT = 29                # the short output buffers end inside this pixel of the last row (at its first byte for 1-byte pixels)
 GUARD = 2048            # bytes after the output's described length that must stay untouched (more than one output row)
 
@@ -154,7 +163,7 @@ def test_library_pairs_are_the_reference_pairs():
 
 
 def test_plan_matrix(monkeypatch):
-    """gf_cuda_plan for every cell in every geometry the GPU matrix renders: 21 pairs x 13 pixel types x 7 variants."""
+    """gf_cuda_plan for every cell in every geometry the GPU matrix renders: 21 pairs x 13 pixel types x 9 variants."""
     lib = g.load_library()
     checked = set()
     for lens, digital in library_pairs():
@@ -168,7 +177,7 @@ def test_plan_matrix(monkeypatch):
                     got = plan(p, pix, lens, digital, descs(case, p, src, dst, out_len), flags)
                     assert got == code, (lens, digital, pix, name, mode, got, code)
                     checked.add((lens, digital, pix, mode))
-    assert len(checked) == 21 * 13 * 7
+    assert len(checked) == 21 * 13 * 9
 
 
 @pytest.mark.parametrize("pix", PIXEL_TYPES)
@@ -258,7 +267,7 @@ def run_matrix(request, monkeypatch, geometry_names, kinds, pairs=None, pixel_ty
     """Render every cell of pairs x pixel_types x modes in the named geometries with every buffer kind of `kinds`; reports the count,
     the time and every failing cell, fails with the first bad render, returns the set of cells rendered."""
     t0 = time.perf_counter()
-    rendered, bad, bad_cells, renders = set(), [], set(), 0
+    rendered, skipped, bad, bad_cells, renders = set(), set(), [], set(), 0
     pairs = pairs or library_pairs()
     for lens, digital in pairs:
         for pix in pixel_types or PIXEL_TYPES:
@@ -270,6 +279,9 @@ def run_matrix(request, monkeypatch, geometry_names, kinds, pairs=None, pixel_ty
                 for mode, switch, interp, tables, code in modes or MODES:
                     set_switch(monkeypatch, switch)
                     cell = (lens, digital, pix, mode)
+                    if interp.startswith("EWA") and (lens, digital, name[0]) in EWA_UNCOMPARABLE:
+                        skipped.add(cell)
+                        continue
                     want, outs, got_code = render(case, pix, lens, digital, interp, tables, out_len, kinds)
                     assert got_code == code, (cell, name, got_code, code)
                     for kind, got, launches in outs:
@@ -285,12 +297,13 @@ def run_matrix(request, monkeypatch, geometry_names, kinds, pairs=None, pixel_ty
                             bad_cells.add(cell)
                     rendered.add(cell)
     n_modes = len(modes or MODES)
-    report(request, "%s: %d cells (%d pairs x %d pixel types x %d variants), %d renders, %d failing renders in %d cells, %.1f s" %
-           (label or request.node.name, len(rendered), len(pairs), len(pixel_types or PIXEL_TYPES), n_modes, renders, len(bad), len(bad_cells), time.perf_counter() - t0))
+    report(request, "%s: %d cells (%d pairs x %d pixel types x %d variants, %d EWA cells not comparable), %d renders, %d failing renders in %d cells, %.1f s" %
+           (label or request.node.name, len(rendered), len(pairs), len(pixel_types or PIXEL_TYPES), n_modes, len(skipped), renders, len(bad), len(bad_cells),
+            time.perf_counter() - t0))
     for c in sorted(bad_cells, key=str)[:64]:
         report(request, "  failing cell: %s %s %s %s" % c)
     assert not bad, "%d failing renders; first: %s" % (len(bad), bad[0])
-    assert len(rendered) == len(pairs) * len(pixel_types or PIXEL_TYPES) * n_modes
+    assert len(rendered) + len(skipped) == len(pairs) * len(pixel_types or PIXEL_TYPES) * n_modes
     return rendered
 
 
@@ -299,7 +312,7 @@ def test_matrix_identity_maps_odd_size(request, monkeypatch):
     """Geometry A: 75 x 43, identity output maps, a stride that is a multiple of 8 with the whole buffer, one that is not with
     buffers ending at the last pixel and part-way through the last row; HOST and DEVICE outputs, guard bytes untouched."""
     rendered = run_matrix(request, monkeypatch, ("A/stride8", "A/ends-at-last-pixel", "A/ends-mid-row"), ("host", "device"))
-    assert len(rendered) == 21 * 13 * 7
+    assert len(rendered) == 21 * 13 * 9
 
 
 @pytest.mark.gpu
@@ -307,21 +320,22 @@ def test_matrix_rects_and_short_output(request, monkeypatch):
     """Geometry B: source rect, output rect and size, fov 1.3, output buffers ending at the last (written) pixel and part-way through
     the last row; HOST and DEVICE outputs, guard bytes after the described length untouched."""
     rendered = run_matrix(request, monkeypatch, ("B/ends-at-last-pixel", "B/ends-mid-row"), ("host", "device"))
-    assert len(rendered) == 21 * 13 * 7
+    assert len(rendered) == 21 * 13 * 9 - 13 * 2          # EWA_UNCOMPARABLE: one pair in both EWA variants
 
 
 # ---- value-domain edges ----------------------------------------------------------------------------------------------------------
 EDGE_PAIRS = [("opencv_fisheye", None), ("sony", "digital_stretch")]
 EDGE_PIXEL_TYPES = ["R32f", "RGBAf", "RGBAf16", "Luma16", "RGBA16"]
 RESAMPLERS = ("Bilinear", "Bicubic", "Lanczos4", "EWA: Mitchell")
+EWA_FILTERS = ("EWA: RobidouxSharp", "EWA: Robidoux", "EWA: Mitchell", "EWA: Catmull-Rom")
 
 
 def edge_modes():
-    """Every variant of MODES with every resampler it can run: bilinear the four fused variants; bicubic, Lanczos4 and EWA the
-    coordinate variants, EWA having no packed one."""
+    """Every variant of MODES with every resampler it can run: bilinear the four fused variants; bicubic, Lanczos4 and the four EWA
+    filters the coordinate variants, EWA having no packed one."""
     out = [m for m in MODES if m[2] == "Bilinear"]
-    for interp in RESAMPLERS[1:]:
-        for mode, switch, _, tables, code in MODES[4:]:
+    for interp in RESAMPLERS[1:3] + EWA_FILTERS:
+        for mode, switch, _, tables, code in MODES[4:7]:
             if interp.startswith("EWA") and mode == "packed-coords":
                 continue
             out.append((mode + "/" + interp, switch, interp, tables, code))
@@ -342,7 +356,7 @@ def test_edge_values(request, monkeypatch):
     edge = dict(edge_values=True, fov=1.3)
     rendered = run_matrix(request, monkeypatch, ("A/stride8",), ("host",), pairs=EDGE_PAIRS, pixel_types=EDGE_PIXEL_TYPES,
                           modes=edge_modes(), extra=edge, label="test_edge_values, variants")
-    assert len(rendered) == 2 * 5 * 12
+    assert len(rendered) == 2 * 5 * (4 + 3 + 3 + 4 * 2)
     for what, params in GENERAL_OPTIONS:
         modes = [(what + "/" + interp, None, interp, "host", 0 if interp == "Bilinear" else 0x10) for interp in RESAMPLERS]
         rendered = run_matrix(request, monkeypatch, ("A/stride8",), ("host",), pairs=EDGE_PAIRS, pixel_types=EDGE_PIXEL_TYPES,
