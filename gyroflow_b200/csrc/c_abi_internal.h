@@ -105,6 +105,11 @@ CameraStab camera_stab_at(const gf_compute_params* cp, size_t frame, bool frameb
 bool lens_noop(int lens, const float* k);
 // the point path (zoom_kernel.cu) compiles this (lens, digital lens) pair
 bool point_path_supported(int lens, int digital);
+// Filtered rolling-shutter pre-pass of the packed fisheye kernel (c_abi.cu): the conditioning cap on r^2 for fisheye coefficients
+// k[0..3] (0: no filter), and the lens's radial table below it — GF_RADIAL_ROWS rows, returns the cap rounded down to a row boundary
+// (NaN rows from there on), or 0 when the table misses its error budget.
+float filter_a_cap(const float* k);
+float build_radial_table(const float* k, float a_cap, float4* rows);
 
 // What generate_stmaps does to the user's ComputeParams before either map (stmap.rs:24-35, :44-46): rotation suppressed, fovs cleared,
 // no readout time unless per_frame, fov_scale 1 and the output size the frame size.

@@ -128,11 +128,17 @@ __global__ void sweep_kernel(uint32_t lo, uint32_t hi, int which, unsigned long 
 // rotation of up to ~25 degrees with random translation terms, frame sizes 1280..8192) every pixel of a sampled grid is evaluated both
 // ways.  out[0] = pixels inside the regime, out[1] = pixels whose |tv_approx - tv_exact| EXCEEDS the certificate's bound (must be 0),
 // out[2] = pixels the certificate calls uncertain (distance to the rounding boundary <= bound), out[3] = max |diff| / bound in 1e-6 units.
-struct FilterCfg { float m[9]; float k[4]; float f1, c1; float a_cap; int w, h; };
-__global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, int n_cfg, int step, float rho, unsigned long long* out) {
+// Each configuration's lens has its own radial table (build_radial_table, as the warp builds it); a lens whose table misses the error
+// budget would run without the filter and is skipped.
+struct FilterCfg { float m[9]; float k[4]; float f1, c1; int on; int w, h; };
+__global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, const float4* __restrict__ tabs, int n_cfg, int step, float rho,
+                                    unsigned long long* out) {
     unsigned long long in_regime = 0, violations = 0, uncertain = 0; unsigned worst = 0;
     for (int ci = blockIdx.y; ci < n_cfg; ci += gridDim.y) {
         const FilterCfg C = cfgs[ci];
+        if (!C.on) continue;
+        const float4* const rtab = tabs + (size_t)ci * GF_RADIAL_ROWS;
+        const float eps_rel = rho + 0x1p-22f, eps_abs = 0x1p-22f * fabsf(C.c1);     // the kernel's certificate tolerance
         gf_kernel_params P; memset(&P, 0, sizeof(P));
         for (int i = 0; i < 4; ++i) P.k[i] = C.k[i];
         P.f[0] = C.f1; P.f[1] = C.f1; P.c[0] = 0.5f * (float)C.w; P.c[1] = C.c1;
@@ -142,14 +148,15 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, int n_cf
             const float _x = (px * C.m[0] + py * C.m[1]) + C.m[2];
             const float _y = (px * C.m[3] + py * C.m[4]) + C.m[5];
             const float _w = (px * C.m[6] + py * C.m[7]) + C.m[8];
-            float tvc;
-            if (!Lens2<GF_LENS_OPENCV_FISHEYE>::approx_v(_x, _y, _w, P, C.a_cap, tvc)) continue;
+            using L = Lens2<GF_LENS_OPENCV_FISHEYE>;
+            if (!(__float_as_uint(_w) - L::kWLo < L::kWSpan)) continue;
+            const float tvc = L::approx_v(_x, _y, _w, P, rtab);
             const float tv = tvc + P.c[1];
-            if (!(fabsf(tv) < 0x1p20f)) continue;
+            if (!(fabsf(tv) < 0x1p20f)) continue;                                     // also r^2 at or above the cap: NaN rows
             float ex, ey;
             Lens<GF_LENS_OPENCV_FISHEYE>::distort(_x, _y, _w, P, false, ex, ey);       // the reference's arithmetic (scalar exact code)
             const float tv_exact = ey * P.f[1] + P.c[1];
-            const float bound = __fmaf_rn(fabsf(tvc), rho, fabsf(tv) * 0x1p-22f);
+            const float bound = __fmaf_rn(fabsf(tvc), eps_rel, eps_abs);
             const float diff = fabsf(tv - tv_exact);
             ++in_regime;
             if (!(diff <= bound)) ++violations;
@@ -170,6 +177,7 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
     if (!out4 || n_cfg < 1 || step < 1) return GF_ERR_BAD_PARAMS;
     CK(nullptr, cudaSetDevice(device));
     std::vector<FilterCfg> cfgs((size_t)n_cfg);
+    std::vector<float4> tabs((size_t)n_cfg * GF_RADIAL_ROWS);
     uint64_t st = seed * 0x9E3779B97F4A7C15ULL + 12345u;
     auto rnd = [&]() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return (double)(st >> 11) * (1.0 / 9007199254740992.0); };   // [0, 1)
     for (int i = 0; i < n_cfg; ++i) {
@@ -182,9 +190,8 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
         const double B = t2 * (fabs(k[0]) + t2 * (fabs(k[1]) + t2 * (fabs(k[2]) + t2 * fabs(k[3]))));
         const double sc = (i % 7 == 0) ? 0.02 / B : 0.25 / B;                 // every 7th: a weak lens (cap at 1.55 rad)
         for (int j = 0; j < 4; ++j) C.k[j] = (float)(k[j] * sc);
-        auto Bf = [&](double t) { const double q = t * t; return q * (fabs((double)C.k[0]) + q * (fabs((double)C.k[1]) + q * (fabs((double)C.k[2]) + q * fabs((double)C.k[3])))); };
-        double lo = 0.0, hi = 1.55; if (Bf(hi) > 0.25) { for (int it = 0; it < 60; ++it) { const double mid = 0.5 * (lo + hi); if (Bf(mid) <= 0.25) lo = mid; else hi = mid; } } else lo = hi;
-        C.a_cap = (float)fmin(tan(lo) * tan(lo) * 0.999, 16000.0);
+        const float a_cap = filter_a_cap(C.k);
+        C.on = a_cap > 0.0f && build_radial_table(C.k, a_cap, &tabs[(size_t)i * GF_RADIAL_ROWS]) > 0.0f;
         // mid-row matrix: (K_new R)^-1 with focal length 0.3..1.2 widths and a rotation of up to ~25 degrees about a random axis
         const double f = (0.3 + 0.9 * rnd()) * C.w, cx = 0.5 * C.w, cy = 0.5 * C.h;
         double ax[3] = { rnd() - 0.5, rnd() - 0.5, rnd() - 0.5 }; const double an = sqrt(ax[0]*ax[0] + ax[1]*ax[1] + ax[2]*ax[2]) + 1e-12;
@@ -198,12 +205,14 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
         for (int r = 0; r < 3; ++r) for (int q = 0; q < 3; ++q) C.m[r * 3 + q] = (float)(R[0 * 3 + r] * Ki[0 * 3 + q] + R[1 * 3 + r] * Ki[1 * 3 + q] + R[2 * 3 + r] * Ki[2 * 3 + q]);
         C.f1 = (float)((0.3 + 0.9 * rnd()) * C.w); C.c1 = (float)(cy + (rnd() - 0.5) * 40.0);
     }
-    GrowBuf<FilterCfg> d_cfg; GrowBuf<unsigned long long> d_out;
+    GrowBuf<FilterCfg> d_cfg; GrowBuf<float4> d_tab; GrowBuf<unsigned long long> d_out;
     CK(nullptr, d_cfg.reserve(cfgs.size(), nullptr));
+    CK(nullptr, d_tab.reserve(tabs.size(), nullptr));
     CK(nullptr, d_out.reserve(4, nullptr));
     CK(nullptr, cudaMemcpy(d_cfg.ptr, cfgs.data(), cfgs.size() * sizeof(FilterCfg), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemcpy(d_tab.ptr, tabs.data(), tabs.size() * sizeof(float4), cudaMemcpyHostToDevice));
     CK(nullptr, cudaMemset(d_out.ptr, 0, 4 * sizeof(unsigned long long)));
-    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg.ptr, n_cfg, step, 0x1p-17f, d_out.ptr);
+    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg.ptr, d_tab.ptr, n_cfg, step, 0x1p-17f, d_out.ptr);
     CK(nullptr, cudaGetLastError());
     CK(nullptr, cudaDeviceSynchronize());
     CK(nullptr, cudaMemcpy(out4, d_out.ptr, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));

@@ -88,6 +88,13 @@ template <bool GEN> __device__ __forceinline__ bool has(uint32_t feat, uint32_t 
     return (feat & bit) != 0;        // F_RS, F_IS_Y stay dynamic
 }
 
+// Radial table of the filtered pre-pass (approx_v): the row of a = r^2 is bits(a) >> 19, one row per 1/16 octave and one for every
+// bit pattern, so that no index needs a clamp.  Rows [GF_RADIAL_FIT, GF_RADIAL_FIT + GF_RADIAL_FIT_ROWS) cover [2^-30, 2^14) and are
+// fitted; the rows below repeat the first fitted row, the rows above hold NaN.
+constexpr int GF_RADIAL_ROWS = 8192;
+constexpr int GF_RADIAL_FIT = (127 - 30) << 4;
+constexpr int GF_RADIAL_FIT_ROWS = (14 + 30) * 16;
+
 struct WarpArgs {
     gf_kernel_params p;             // verbatim KernelParams
     const uint8_t* src;
@@ -107,8 +114,9 @@ struct WarpArgs {
         unsigned* count_next;       // the next frame's counter, zeroed by this frame's tail launch
         uint32_t  cap;              // capacity of q (a full queue makes the thread take the exact pre-pass inline)
         int       tail;             // 1 = this launch renders the queue
-        float     rho;              // relative tolerance of the certificate
-        float     a_cap;            // r^2 below which the tolerance holds for this lens (polynomial conditioning), <= 2^14
+        const float4* rtab;         // the lens's radial table (GF_RADIAL_ROWS rows, approx_v in warp_kernel_x2.cuh)
+        const float*  mid_row;      // the matrix table's middle row, matrices + (matrix_count / 2) * GF_MATRIX_STRIDE
+        float     eps_rel, eps_abs; // tolerance of the certificate: eps = eps_rel |t - c_y| + eps_abs = (rho + 2^-22) |t - c_y| + 2^-22 |c_y|
     } flt;
     int            coord_shift;     // pass 1: 0 = pixel (x, y); 1 = (x + 0.01, y); 2 = (x, y + 0.01) — the EWA Jacobian probes of :567-572
     int            coord_maps;      // pass 2: 1, or 3 when the two probe maps follow the first one (stride out_cols * out_rows)

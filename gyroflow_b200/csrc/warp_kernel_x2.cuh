@@ -18,7 +18,6 @@
 // Behavioural source: src/core/stabilization/cpu_undistort.rs:133-228, :421-517, :543-625 (as warp_kernel.cuh).
 #pragma once
 #include "warp_kernel.cuh"
-#include "approx_atan_table.inc"
 
 namespace gf {
 
@@ -50,28 +49,25 @@ template <> struct Lens2<GF_LENS_OPENCV_FISHEYE> {
     static constexpr bool kHas = true;
     // FILTERED PRE-PASS.  The mid-row evaluation of cpu_undistort.rs:470-479 only decides which matrix row a pixel uses:
     // idx = clamp(round(v_mid), 0, H).  This is v_mid - c_y computed CHEAPLY — one MUFU.RCP instead of two refined divisions, no
-    // square root, atan(r) / r from a cubic table in r^2 (approx_atan_table.inc), fused multiply-adds — together with a proven bound
-    // on its distance from the reference's own float result (DESIGN.md §4 "filtered pre-pass"):
-    //     |tv_approx - tv_exact| <= rho * |tv - c_y| + 2^-22 * |tv|,   rho = 2^-17,
-    // valid while the divisor w is in the window of the exact sequences and r^2 < a_cap (the host derives a_cap from k so that the
-    // polynomial 1 + k0 t^2 + ... stays within [3/4, 5/4], which bounds its cancellation).  (_x, _y, _w) are the reference's own
-    // unfused products — bit-identical to the exact chain — so only relative perturbations enter after them.
-    // Returns false outside that regime; tvc = (v - c_y) otherwise.
-    static GF_DEV bool approx_v(float _x, float _y, float _w, const gf_kernel_params& P, float a_cap, float& tvc) {
-        const bool ok_w = (_w >= 0x1p-56f) & (_w < 0x1p48f);
+    // square root, the whole radial factor R(a) = (atan(r) / r) * (1 + k0 theta^2 + ... + k3 theta^8) from the lens's cubic table in
+    // a = r^2 (`rtab`, built and checked by the host: build_radial_table in c_abi.cu), fused multiply-adds — together with a proven
+    // bound on its distance from the reference's own float result (profiles/FILTER_ANALYSIS.md):
+    //     |tv_approx - tv_exact| <= (rho + 2^-22) * |tv - c_y| + 2^-22 * |c_y|,   rho = 2^-17,
+    // valid while the divisor w is in the window of the exact sequences and r^2 is below the host's conditioning cap (the polynomial
+    // stays within [3/4, 5/4]).  The table's rows from that cap on hold NaN, so tvc is NaN there and fails the certificate.
+    // (_x, _y, _w) are the reference's own unfused products — bit-identical to the exact chain — so only relative perturbations enter
+    // after them.  Returns tvc = (v - c_y), or NaN; the caller checks _w against the window kWLo / kWSpan.
+    static constexpr uint32_t kWLo = 0x23800000u, kWSpan = 0x57800000u - 0x23800000u;   // 2^-56 <= w < 2^48 <=> bits(w) - kWLo < kWSpan
+                                                                                        // (unsigned: NaN, zeros and negatives fail)
+    static GF_DEV float approx_v(float _x, float _y, float _w, const gf_kernel_params& P, const float4* __restrict__ rtab) {
         const float iw = p2::rcp_approx(_w);
         const float x = _x * iw, y = _y * iw;
         const float a = __fmaf_rn(x, x, y * y);
         const uint32_t ab = __float_as_uint(a);
-        const int idx = __vimin_s32_relu((int)(ab >> 19) - (int)GF_APX_BASE, GF_APX_ROWS - 1);     // max(min(., ROWS - 1), 0): any a, NaN included
-        const float a0 = __uint_as_float((ab & 0xfff80000u) | 0x00040000u);      // midpoint of a's 1/16-octave interval
-        const float4 c = __ldg(&GF_APX_TAB[idx]);
-        const float d = a - a0;
-        const float T = __fmaf_rn(d, __fmaf_rn(d, __fmaf_rn(d, c.w, c.z), c.y), c.x);   // atan(r) / r
-        const float t2 = (a * T) * T;                                                     // theta^2
-        const float s = __fmaf_rn(t2, __fmaf_rn(t2, __fmaf_rn(t2, __fmaf_rn(t2, P.k[3], P.k[2]), P.k[1]), P.k[0]), 1.0f);
-        tvc = ((y * T) * s) * P.f[1];
-        return ok_w & (a < a_cap);              // NaN compares false
+        const float4 c = __ldg(&rtab[ab >> 19]);                                   // a's 1/16-octave interval: every bit pattern has a row
+        const float d = a - __uint_as_float(ab & 0xfff80000u);                    // from the interval's start (exact)
+        const float R = __fmaf_rn(d, __fmaf_rn(d, __fmaf_rn(d, c.w, c.z), c.y), c.x);
+        return (y * R) * P.f[1];
     }
     template <bool TRUSTED>
     static GF_DEV void distort(f2 x, f2 y, f2 z, const gf_kernel_params& P, f2& ox, f2& oy, bool& bad) {
@@ -697,18 +693,18 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
         if constexpr (TRUSTED && LensApprox<LENS>::value && DIGITAL == GF_LENS_NONE) {
             if (!exact_prepass) {                        // F_FILTER, which implies F_RS (host)
                 // :470-479, filtered: certify round(v_mid) from the approximate evaluation, defer the pair when it cannot be
-                const MatRow9 rm = load_row9(A.matrices, (uint32_t)P.matrix_count / 2u);
+                const MatRow9 rm = load_row9(A.flt.mid_row, 0u);
                 const float bx = pxs * rm.m01.x, by = pxs * rm.m23.y, bw = pxs * rm.m67.x;              // the reference's products and sums, unfused
                 const float xa = (bx + py.x * rm.m01.y) + rm.m23.x, xb = (bx + py.y * rm.m01.y) + rm.m23.x;
                 const float ya = (by + py.x * rm.m45.x) + rm.m45.y, yb = (by + py.y * rm.m45.x) + rm.m45.y;
                 const float wa = (bw + py.x * rm.m67.y) + rm.m8,    wb = (bw + py.y * rm.m67.y) + rm.m8;
-                float ca, cb;
-                const bool ra = Lens2<LENS>::approx_v(xa, ya, wa, P, A.flt.a_cap, ca);
-                const bool rb = Lens2<LENS>::approx_v(xb, yb, wb, P, A.flt.a_cap, cb);
+                const float ca = Lens2<LENS>::approx_v(xa, ya, wa, P, A.flt.rtab), cb = Lens2<LENS>::approx_v(xb, yb, wb, P, A.flt.rtab);
+                constexpr uint32_t wlo = Lens2<LENS>::kWLo;                   // both divisors in the window: the larger offset, unsigned
+                const bool w_ok = __viaddmax_u32(__float_as_uint(wa), 0u - wlo, __float_as_uint(wb) - wlo) < Lens2<LENS>::kWSpan;
                 const float ta = ca + P.c[1], tb = cb + P.c[1];
-                const float ea = __fmaf_rn(fabsf(ca), A.flt.rho, fabsf(ta) * 0x1p-22f), eb = __fmaf_rn(fabsf(cb), A.flt.rho, fabsf(tb) * 0x1p-22f);
+                const float ea = __fmaf_rn(fabsf(ca), A.flt.eps_rel, A.flt.eps_abs), eb = __fmaf_rn(fabsf(cb), A.flt.eps_rel, A.flt.eps_abs);
                 const bool ca_ok = certify_row(ta, ea, lim, sy_a), cb_ok = certify_row(tb, eb, lim, sy_b);
-                if (ra & rb & ca_ok & cb_ok) break;
+                if (w_ok & ca_ok & cb_ok) break;
                 // append the pair to the frame's queue (warp-aggregated), rendered by the tail launch
                 const unsigned m = __activemask();
                 const unsigned lane = threadIdx.x & 31u;

@@ -307,6 +307,11 @@ GF_API int         gf_cuda_plan(const gf_kernel_params* params, int pixel_type, 
 GF_API int         gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
                                          const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags,
                                          size_t n_planes, uint32_t* feat_out);
+/* The filtered pre-pass's radial table for opencv_fisheye coefficients k[0..3], as the warp builds it (host only, no CUDA call): 8192
+ * rows of four floats into rows_out (rows_cap >= 8192; row bits(r^2) >> 19 holds the cubic c0 + d (c1 + d (c2 + d c3)) in d = r^2 minus the
+ * start of its 1/16-octave interval), and the r^2 cap the filter runs with, rounded down to a row boundary (rows from there on are NaN);
+ * 0 when the lens runs without the filter.  Returns the number of rows, or < 0 on error.  Test hook. */
+GF_API int         gf_filter_radial_table(const float* k, float* rows_out, size_t rows_cap, float* a_cap_out);
 
 /* Preview overlays of the reference's GPU kernels — draw_pixel + draw_safe_area, src/core/gpu/opencl_undistort.cl:109-154, buffer
  * produced by gpu/drawing.rs:8-50 (SURVEY §8 f4).  OFF by default: the CPU path, the parity target, draws none
