@@ -223,6 +223,7 @@ EXPORTS = [
     ("gf_cuda_plan_features", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t,
                                         _P(C.c_uint32)]),
     ("gf_filter_radial_table", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_float)]),
+    ("gf_cuda_filter_stats", C.c_int, [C.c_void_p, _P(C.c_uint64)]),
     ("gf_cuda_synchronize", C.c_int, [C.c_void_p]),
     ("gf_cuda_set_overlays", C.c_int, [C.c_void_p, C.c_int]),
     ("gf_cuda_last_error", C.c_char_p, [C.c_void_p]),

@@ -203,6 +203,16 @@ class CudaWrapper:
         if rc != 0:
             raise self._err(rc)
 
+    def filter_stats(self):
+        """The filtered pre-pass's bookkeeping (gf_cuda_filter_stats, a test hook), after waiting like synchronize(): filtered frames so
+        far, the latest one's raw deferral count (above `cap`: the excess took the exact pre-pass inline), the queue capacity, the tail
+        launch's thread count, radial tables built and lookups served from the cache."""
+        out = (C.c_uint64 * 6)()
+        rc = self._lib.gf_cuda_filter_stats(self._h, out)
+        if rc != 0:
+            raise self._err(rc)
+        return dict(zip(("frames", "count", "cap", "tail_threads", "radial_builds", "radial_hits"), (int(v) for v in out)))
+
     @property
     def launch_count(self):
         return int(self._lib.gf_cuda_launch_count(self._h))

@@ -33,20 +33,24 @@ struct Slot {                                   // one in-flight set of per-fram
 };
 constexpr int kSlots = 4;
 // A lens's radial table for the filtered pre-pass (build_radial_table), cached by the bit pattern of k[0..3].  An entry is rebuilt for
-// another lens only once `done` has passed: it is recorded after every launch that reads the table, and a launch on another stream
-// than the previous reader's waits for it first, so the latest record follows every earlier reader and no frame in flight sees its
-// table change.
+// another lens only once `done` has passed: it is recorded after every launch that reads the table, and every call on the context is
+// ordered after the previous one (run_warp), so the latest record follows every earlier reader and its upload from the pinned copy `h`,
+// and no frame in flight sees its table change.
 struct RadialTable {
     uint32_t key[4] = {};
     bool filled = false, uploaded = false;
     float a_cap = 0.0f;                         // rounded to an interval boundary; 0: the fit missed its budget, no filter for this lens
     unsigned long long last_use = 0;            // least recently used entry is rebuilt
-    cudaStream_t stream = nullptr;              // of the latest launch that read it
     GrowBuf<float4, true> h;
     GrowBuf<float4> d;
     Event done;
 };
 constexpr int kRadialTables = 4;
+// The deferred-pair queue of the filtered pre-pass holds this many pairs (4 MB: a quarter of a 4K frame's pairs); a pair that finds it
+// full is rendered inline by the main launch.  Packed-kernel blocks are GF_BLOCK_X x kPackedBlockY threads; the tail launch has
+// kTailBlocksPerSM of them per multiprocessor.
+constexpr unsigned kDeferCap = 1u << 20;
+constexpr int kPackedBlockY = 4, kTailBlocksPerSM = 16;
 
 // Per pixel layout (LAY_*): bytes per pixel, channels, scalar kind (SC_*), the maximum value pixel_value_limit is compared against
 struct LayoutInfo { int bpp, channels, scalar; float max_value; };
@@ -78,10 +82,14 @@ struct gf_cuda_ctx {
     KernelFn fn_shade = nullptr;         // pass 2 of the two-pass path
     GrowBuf<uint32_t> const_flags;       // two device words {0, 1}: the verdict of the host scan of host tables, as the kernel wants it
     GrowBuf<uint32_t> vflags;            // scratch verdict word of gf_cuda_validate_tables_dev
-    cudaStream_t last_stream = nullptr;  // the stream of the most recent call (gf_cuda_synchronize waits for it too)
+    // Every call is ordered after the previous one on the device, whatever streams they name: `last_call` is recorded at the end of each
+    // call, and a call on another stream than `last_stream` waits for it first (order_after_last_call).  The calls share the state
+    // below (deferred-pair queue and counters, coordinate maps, staging), and gf_cuda_synchronize waits for `last_stream` only.
+    cudaStream_t last_stream = nullptr;
+    Event last_call;
     // filtered rolling-shutter pre-pass (packed fisheye kernel): queue of deferred pixel pairs + two ping-pong counters
     GrowBuf<uint32_t> defer_q; GrowBuf<unsigned> defer_count; unsigned long long filter_frames = 0;
-    RadialTable radial[kRadialTables]; unsigned long long radial_uses = 0;
+    RadialTable radial[kRadialTables]; unsigned long long radial_uses = 0, radial_builds = 0;
     int sm_count = 1;                    // the device's multiprocessors (sizes the filtered pre-pass's tail launch)
     // preview overlays (overlay.cu), off unless gf_cuda_set_overlays: device copy of the drawing buffer, private copy of a DEVICE input
     int overlays = 0;
@@ -586,6 +594,7 @@ struct FrameRun {
                 CK(err, radial->h.reserve(GF_RADIAL_ROWS, st)); CK(err, radial->d.reserve(GF_RADIAL_ROWS, st));
                 radial->a_cap = build_radial_table(A.p.k, plan.a_cap, radial->h.ptr);
                 memcpy(radial->key, key, sizeof(key)); radial->filled = true; radial->uploaded = false;
+                ctx->radial_builds++;
             }
             radial->last_use = ++ctx->radial_uses;
             plan.a_cap = radial->a_cap;
@@ -603,11 +612,10 @@ struct FrameRun {
         const KernelFn fn = ctx->combo.kernels[plan.kernel];
         if (plan.kernel == KV_PACKED || plan.kernel == KV_PACKED_COORDS) {
             // 32 x 4 threads (4 x 8 output rows... 32 x 8 pixels) per block measured 2 % faster than 32 x 8 threads (finer tail)
-            constexpr int kPackedBlockY = 4;
             const dim3 block2(GF_BLOCK_X, kPackedBlockY), grid2(grid.x, (A.out_rows + 2 * kPackedBlockY - 1) / (2 * kPackedBlockY));
             if (plan.a_cap > 0.0f) {
-                if (!ctx->defer_q.ptr) {                       // 4 MB: 1 M pairs = a quarter of a 4K frame's pairs; a full queue falls back inline
-                    CK(err, ctx->defer_q.reserve(1u << 20, st)); CK(err, ctx->defer_count.reserve(2, st));
+                if (!ctx->defer_q.ptr) {
+                    CK(err, ctx->defer_q.reserve(kDeferCap, st)); CK(err, ctx->defer_count.reserve(2, st));
                     CK(err, cudaMemsetAsync(ctx->defer_count.ptr, 0, 2 * sizeof(unsigned), st));
                 }
                 const unsigned cur = (unsigned)(ctx->filter_frames & 1ull);
@@ -619,18 +627,17 @@ struct FrameRun {
                 if (!rt.uploaded) {
                     CK(err, cudaMemcpyAsync(rt.d.ptr, rt.h.ptr, GF_RADIAL_ROWS * sizeof(float4), cudaMemcpyHostToDevice, st));
                     rt.uploaded = true;
-                } else if (rt.stream != st) CK(err, cudaStreamWaitEvent(st, rt.done.get(), 0));   // after the upload and the earlier readers
+                }
                 // eps = (rho + 2^-22) |t - c_y| + 2^-22 |c_y| with rho = 2^-17 (profiles/FILTER_ANALYSIS.md; |c_y| >= 2^-10 without F_WILD)
                 A.flt.mid_row = A.matrices + (size_t)(A.p.matrix_count / 2) * GF_MATRIX_STRIDE;
                 A.flt.rtab = rt.d.ptr; A.flt.eps_rel = 0x1p-17f + 0x1p-22f; A.flt.eps_abs = 0x1p-22f * fabsf(A.p.c[1]);
                 A.flt.tail = 0;
                 CK(err, launch_pdl(fn, grid2, block2, A, st));
                 CK(err, cudaEventRecord(rt.done.get(), st));   // the tail launch runs the exact pre-pass and does not read the table
-                rt.stream = st;
                 A.flt.tail = 1;                                // the deferred pairs, exact pre-pass; also re-arms the other counter
                 // one thread per deferred pair for up to 2 % of a 4K frame's pairs in a single wave of tiny blocks (idle blocks exit at once);
                 // more entries than threads are covered by the grid-stride loop
-                CK(err, launch_pdl(fn, dim3(ctx->sm_count * 16, 1), block2, A, st));
+                CK(err, launch_pdl(fn, dim3(ctx->sm_count * kTailBlocksPerSM, 1), block2, A, st));
                 ctx->launches++;
             } else CK(err, launch_pdl(fn, grid2, block2, A, st));
         } else {
@@ -684,6 +691,13 @@ struct FrameRun {
     }
 };
 
+// The start of every call that enqueues work for a context on `st`: after the previous call on the device (see gf_cuda_ctx::last_call).
+int order_after_last_call(gf_cuda_ctx* ctx, cudaStream_t st) {
+    if (ctx->last_stream && ctx->last_stream != st) CK(&ctx->last_error, cudaStreamWaitEvent(st, ctx->last_call.get(), 0));
+    ctx->last_stream = st;
+    return GF_OK;
+}
+
 int run_warp(gf_cuda_ctx* ctx, const FrameJob& job) {
     if (!ctx) return fail(nullptr, GF_ERR_BAD_PARAMS, "ctx is null");
     std::string* const err = &ctx->last_error;
@@ -705,13 +719,15 @@ int run_warp(gf_cuda_ctx* ctx, const FrameJob& job) {
     if (job.tables_on_device && (reinterpret_cast<uintptr_t>(job.matrices) & 7u)) return fail(err, GF_ERR_BAD_PARAMS, "device matrices must be 8-byte aligned");
     CK(err, cudaSetDevice(ctx->device));
     FrameRun F{ctx, job};
-    ctx->last_stream = F.st;
+    if ((rc = order_after_last_call(ctx, F.st)) != GF_OK) return rc;
     memset(&F.A, 0, sizeof(F.A));
     F.A.p = *job.p;
-    if ((rc = F.stage()) != GF_OK || (rc = F.draw_input_overlays()) != GF_OK || (rc = F.plan_launch()) != GF_OK) return rc;
-    nvtxRangePushA("gf_warp_launch");
-    if ((rc = F.launch()) == GF_OK) rc = F.finish();
-    nvtxRangePop();
+    if ((rc = F.stage()) == GF_OK && (rc = F.draw_input_overlays()) == GF_OK && (rc = F.plan_launch()) == GF_OK) {
+        nvtxRangePushA("gf_warp_launch");
+        if ((rc = F.launch()) == GF_OK) rc = F.finish();
+        nvtxRangePop();
+    }
+    CK(err, cudaEventRecord(ctx->last_call.get(), F.st));    // also after a failure: whatever was enqueued still uses the context
     return rc;
 }
 
@@ -811,6 +827,7 @@ GF_API int gf_cuda_create(gf_cuda_ctx** out_ctx, int device, const gf_kernel_par
     CK(nullptr, cudaSetDevice(device));
     CK(nullptr, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
     CK(nullptr, create_stream(ctx->stream));
+    CK(nullptr, create_event(ctx->last_call));
     const cudaStream_t st = ctx->stream.get();
     // matrices: 14 * max(W, H) f32 (rows = height, or width for horizontal rolling shutter) — opencl.rs:268, wgpu.rs:260
     size_t rows = (size_t)std::max(std::max(params->width, params->height), std::max(params->output_width, params->output_height));
@@ -1061,7 +1078,7 @@ GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_
     }
     CK(err, cudaSetDevice(ctx->device));
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
-    ctx->last_stream = st;
+    { int rc = order_after_last_call(ctx, st); if (rc != GF_OK) return rc; }   // the staging copies below reuse the context's buffers
     if (ctx->plane_src.size() < n_planes) { ctx->plane_src.resize(n_planes); ctx->plane_dst.resize(n_planes); }
     std::vector<gf_buffer_desc> din(in, in + n_planes), dout(out, out + n_planes);
     for (size_t i = 0; i < n_planes; ++i) {
@@ -1144,6 +1161,22 @@ GF_API int gf_cuda_synchronize(gf_cuda_ctx* ctx) {
     CK(err, cudaSetDevice(ctx->device));
     CK(err, cudaStreamSynchronize(ctx->stream.get()));
     if (ctx->last_stream && ctx->last_stream != ctx->stream.get()) CK(err, cudaStreamSynchronize(ctx->last_stream));   // calls made with a caller-supplied stream
+    return GF_OK;
+}
+
+GF_API int gf_cuda_filter_stats(gf_cuda_ctx* ctx, uint64_t* out6) {
+    if (!ctx || !out6) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    std::string* const err = &ctx->last_error;
+    int rc = gf_cuda_synchronize(ctx);
+    if (rc != GF_OK) return rc;
+    unsigned count = 0;
+    if (ctx->filter_frames > 0) {
+        CK(err, cudaMemcpyAsync(&count, ctx->defer_count.ptr + ((ctx->filter_frames - 1) & 1ull), sizeof(count), cudaMemcpyDeviceToHost, ctx->stream.get()));
+        CK(err, cudaStreamSynchronize(ctx->stream.get()));
+    }
+    out6[0] = ctx->filter_frames; out6[1] = count; out6[2] = kDeferCap;
+    out6[3] = (uint64_t)ctx->sm_count * kTailBlocksPerSM * GF_BLOCK_X * kPackedBlockY;
+    out6[4] = ctx->radial_builds; out6[5] = ctx->radial_uses - ctx->radial_builds;
     return GF_OK;
 }
 

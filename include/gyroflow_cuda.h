@@ -195,7 +195,10 @@ typedef struct gf_buffer_desc {
     size_t   len;                    /* bytes reachable from ptr */
 } gf_buffer_desc;
 
-typedef struct gf_cuda_ctx gf_cuda_ctx;   /* opaque; one per host thread / stream, like the thread-local LRU (mod.rs:62-66) */
+/* Opaque; like the thread-local LRU (mod.rs:62-66), one per host thread: a context is not thread-safe.  Every call takes a stream, and
+ * the work of each call on a context runs on the device after the work of the previous call on that context, whatever streams the two
+ * name (the calls share the context's device buffers).  Independent frames in flight at once want one context each. */
+typedef struct gf_cuda_ctx gf_cuda_ctx;
 
 /* ---- capability probe: OclWrapper::list_devices opencl.rs:60, wgpu.rs:77,99,113 ---------- */
 GF_API int         gf_cuda_device_count(void);
@@ -312,6 +315,12 @@ GF_API int         gf_cuda_plan_features(const gf_kernel_params* params, int pix
  * start of its 1/16-octave interval), and the r^2 cap the filter runs with, rounded down to a row boundary (rows from there on are NaN);
  * 0 when the lens runs without the filter.  Returns the number of rows, or < 0 on error.  Test hook. */
 GF_API int         gf_filter_radial_table(const float* k, float* rows_out, size_t rows_cap, float* a_cap_out);
+/* The filtered pre-pass's bookkeeping on a context, after waiting like gf_cuda_synchronize: out6[0] frames rendered with the filter so
+ * far; [1] the deferral counter of the latest of them, raw: it counts every pair the main launch could not certify, and what exceeds the
+ * queue's capacity took the exact pre-pass inline (the value stays until the next filtered frame's tail launch); [2] the queue's capacity
+ * in pairs; [3] the tail launch's thread count; [4] radial tables built; [5] radial-table lookups served from the context's cache.
+ * Returns GF_OK or < 0.  Test hook. */
+GF_API int         gf_cuda_filter_stats(gf_cuda_ctx* ctx, uint64_t* out6);
 
 /* Preview overlays of the reference's GPU kernels — draw_pixel + draw_safe_area, src/core/gpu/opencl_undistort.cl:109-154, buffer
  * produced by gpu/drawing.rs:8-50 (SURVEY §8 f4).  OFF by default: the CPU path, the parity target, draws none
@@ -321,7 +330,7 @@ GF_API int         gf_filter_radial_table(const float* k, float* rows_out, size_
  * modified.  Single-plane calls only. */
 GF_API int         gf_cuda_set_overlays(gf_cuda_ctx* ctx, int enabled);
 
-/* Waits for the context's own stream AND for the stream of the most recent call that named one. */
+/* Waits for the context's own stream AND for the stream of the most recent call that named one (which follows every earlier call). */
 GF_API int         gf_cuda_synchronize(gf_cuda_ctx* ctx);
 GF_API const char* gf_cuda_last_error(gf_cuda_ctx* ctx);     /* ctx may be NULL: last global error */
 GF_API const char* gf_cuda_backend_name(void);               /* ProcessedInfo.backend: "CUDA" (mod.rs:195-201) */

@@ -451,7 +451,8 @@ def test_filtered_prepass_certificate_on_device():
 def test_filtered_prepass_queue_overflow_and_extremes(monkeypatch):
     """Frames where the certificate fails for MANY pairs — strong roll (the row boundaries run diagonally through every warp), a lens at
     its conditioning cap, a view zoomed out past the cap, translation — still match the oracle: deferred pairs go through the tail
-    launch, a full queue falls back to the exact pre-pass inline."""
+    launch.  None of these frames defers more pairs than the queue holds (1920 x 1080 has fewer pairs in all); the full queue's inline
+    fallback and the tail's grid-stride loop are tested in tests/test_filter_queue.py, on frames proven to reach them."""
     for c in (dict(w=1920, h=1080, video_rotation=33.0), dict(w=1920, h=1080, fov=3.5, ts=1234.0), dict(w=1280, h=720, params=dict(k=[0.18, -0.06, 0.02, -0.004] + [0.0] * 8)),
               dict(w=1280, h=720, params=dict(k=[-0.21, 0.0, 0.0, 0.0] + [0.0] * 8), fov=1.7), dict(w=1280, h=720, params=dict(translation2d=[13.5, -7.25]), readout=33.0),
               dict(w=3840, h=2160, ts=3456.7, pix="Luma8"), dict(w=2048, h=1152, ow=1024, oh=576), dict(w=640, h=360, out_size=(700, 400), out_rect=(30, 20, 640, 360))):

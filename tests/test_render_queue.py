@@ -77,12 +77,19 @@ def test_queue_device_buffers_every_frame_matches_oracle():
     ("Luma16", "opencv_fisheye", "gopro_superview", {}),
     ("RGBAf", "sony", None, dict(stab=True, mesh=True)),          # IBIS rows from the spline producer + per-frame mesh: guarded / general kernel
     ("RGBA8", "opencv_fisheye", None, dict(stab="alternate")),     # packed kernel, consecutive slots alternate between verdicts 2 and 0
+    # five fisheye lenses in turn: each slot's context sees all five (one radial-table eviction) and then its first lens again (a rebuild)
+    ("RGBA8", "opencv_fisheye", None, dict(lenses=5, n=18)),
 ])
 def test_queue_host_buffers_pipelined(pix, lens, digital, extra):
     import torch
     from tests.test_frame_transform import _stab
-    n = 9
+    n = extra.get("n", 9)
     kw = {}
+    if extra.get("lenses"):
+        p0 = synth.base_kernel_params(W, H)
+        K = [p0.f[0], 0.0, p0.c[0], 0.0, p0.f[1], p0.c[1], 0.0, 0.0, 1.0]
+        L = [dict(camera_matrix=K, distortion_coeffs=[0.05 - 0.03 * i, 0.01 * (i % 2), -0.002, 0.0005 * i] + [0.0] * 8) for i in range(extra["lenses"])]
+        kw = dict(lens_per_frame=[L[f % len(L)] for f in range(n)])
     if extra.get("stab") == "alternate":      # spline points on even frames (counts differ), none on odd ones, frames 7 and 8 past the end
         stab = producer_cases.spline_stab([12, 0, 31, 0, 6, 0, 19], seed=8)
         kw = dict(camera_stab=stab, sync_offsets={500_000: 3.0, 800_000: -1.5, 1_200_000: 2.5})
