@@ -32,25 +32,7 @@ struct Slot {                                   // one in-flight set of per-fram
     Event done;
 };
 constexpr int kSlots = 4;
-// A lens's radial table for the filtered pre-pass (build_radial_table), cached by the bit pattern of k[0..3].  An entry is rebuilt for
-// another lens only once `done` has passed: it is recorded after every launch that reads the table, and every call on the context is
-// ordered after the previous one (run_warp), so the latest record follows every earlier reader and its upload from the pinned copy `h`,
-// and no frame in flight sees its table change.
-struct RadialTable {
-    uint32_t key[4] = {};
-    bool filled = false, uploaded = false;
-    float a_cap = 0.0f;                         // rounded to an interval boundary; 0: the fit missed its budget, no filter for this lens
-    unsigned long long last_use = 0;            // least recently used entry is rebuilt
-    GrowBuf<float4, true> h;
-    GrowBuf<float4> d;
-    Event done;
-};
-constexpr int kRadialTables = 4;
-// The deferred-pair queue of the filtered pre-pass holds this many pairs (4 MB: a quarter of a 4K frame's pairs); a pair that finds it
-// full is rendered inline by the main launch.  Packed-kernel blocks are GF_BLOCK_X x kPackedBlockY threads; the tail launch has
-// kTailBlocksPerSM of them per multiprocessor.
-constexpr unsigned kDeferCap = 1u << 20;
-constexpr int kPackedBlockY = 4, kTailBlocksPerSM = 16;
+constexpr int kPackedBlockY = 4;                // packed-kernel blocks are GF_BLOCK_X x kPackedBlockY threads
 
 // Per pixel layout (LAY_*): bytes per pixel, channels, scalar kind (SC_*), the maximum value pixel_value_limit is compared against
 struct LayoutInfo { int bpp, channels, scalar; float max_value; };
@@ -87,10 +69,7 @@ struct gf_cuda_ctx {
     // below (deferred-pair queue and counters, coordinate maps, staging), and gf_cuda_synchronize waits for `last_stream` only.
     cudaStream_t last_stream = nullptr;
     Event last_call;
-    // filtered rolling-shutter pre-pass (packed fisheye kernel): queue of deferred pixel pairs + two ping-pong counters
-    GrowBuf<uint32_t> defer_q; GrowBuf<unsigned> defer_count; unsigned long long filter_frames = 0;
-    RadialTable radial[kRadialTables]; unsigned long long radial_uses = 0, radial_builds = 0;
-    int sm_count = 1;                    // the device's multiprocessors (sizes the filtered pre-pass's tail launch)
+    FilterPrepass filter;
     // preview overlays (overlay.cu), off unless gf_cuda_set_overlays: device copy of the drawing buffer, private copy of a DEVICE input
     int overlays = 0;
     GrowBuf<uint8_t, true> h_drawing;
@@ -309,96 +288,6 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     }
 }
 
-} // namespace
-
-// Filtered rolling-shutter pre-pass (warp_kernel_x2.cuh, Lens2<opencv_fisheye>::approx_v): the host side of its contract.
-// The certificate |tv_approx - tv_exact| <= (rho + 2^-22) |tv - c_y| + 2^-22 |c_y| assumes that the polynomial s = 1 + k0 t^2 + k1 t^4 +
-// k2 t^6 + k3 t^8 stays within [3/4, 5/4] (its rounding error and its sensitivity to the error of t are then bounded,
-// profiles/FILTER_ANALYSIS.md): a_cap = tan^2(t_cap) with t_cap the largest angle (<= 1.55 rad) for which sum |k_i| t^(2i+2) <= 1/4.
-// Returns 0 when the lens is too strongly curved for the filter to be worth it (t_cap < 0.5 rad).
-float gf::filter_a_cap(const float* k) {
-    auto B = [&](double t) { const double t2 = t * t; return t2 * (fabs((double)k[0]) + t2 * (fabs((double)k[1]) + t2 * (fabs((double)k[2]) + t2 * fabs((double)k[3])))); };
-    for (int i = 0; i < 4; ++i) if (!std::isfinite(k[i])) return 0.0f;
-    double lo = 0.0, hi = 1.55;
-    if (B(hi) > 0.25) { for (int it = 0; it < 60; ++it) { const double mid = 0.5 * (lo + hi); if (B(mid) <= 0.25) lo = mid; else hi = mid; } }
-    else lo = hi;
-    if (lo < 0.5) return 0.0f;
-    const double a = tan(lo) * tan(lo);
-    return (float)std::min(a * 0.999, 16000.0);                 // stay inside the table (r^2 < 2^14) and below the exact bound
-}
-
-namespace {
-// T(a) = atan(sqrt a) / sqrt a in f64
-double radial_T(double a) { const double r = sqrt(a); return r < 1e-4 ? 1.0 - a / 3.0 + a * a / 5.0 : atan(r) / r; }
-// What every lens's table shares, computed once for the fitted rows: the intervals, T at their Chebyshev nodes, and the check points
-// with T there
-struct RadialGrid {
-    static constexpr int N = GF_RADIAL_FIT_ROWS, kChk = 65;     // 64 steps per interval, both ends included
-    double lo[N], hi[N], h[N];
-    double node_a[N][4], node_T[N][4];
-    double chk_a[N][kChk], chk_T[N][kChk];
-    double vinv[4][4];              // inverse of the Vandermonde matrix of the nodes 1 + t_q, t_q = cos((2q + 1) pi / 8), in units of h
-    RadialGrid() {
-        double t[4], V[4][8];
-        for (int q = 0; q < 4; ++q) t[q] = cos((2 * q + 1) * 3.14159265358979323846 / 8.0);
-        for (int r = 0; r < 4; ++r) for (int c = 0; c < 8; ++c) V[r][c] = c < 4 ? pow(1.0 + t[r], c) : (c - 4 == r ? 1.0 : 0.0);
-        for (int c = 0; c < 4; ++c) {               // Gauss-Jordan with partial pivoting
-            int p = c;
-            for (int r = c + 1; r < 4; ++r) if (fabs(V[r][c]) > fabs(V[p][c])) p = r;
-            for (int j = 0; j < 8; ++j) std::swap(V[c][j], V[p][j]);
-            const double d = V[c][c];
-            for (int j = 0; j < 8; ++j) V[c][j] /= d;
-            for (int r = 0; r < 4; ++r) if (r != c) { const double f = V[r][c]; for (int j = 0; j < 8; ++j) V[r][j] -= f * V[c][j]; }
-        }
-        for (int r = 0; r < 4; ++r) for (int c = 0; c < 4; ++c) vinv[r][c] = V[r][c + 4];
-        for (int i = 0; i < N; ++i) {
-            const int e = i / 16, j = i % 16;
-            lo[i] = ldexp(1.0 + j / 16.0, e - 30); hi[i] = ldexp(1.0 + (j + 1) / 16.0, e - 30);
-            h[i] = 0.5 * (hi[i] - lo[i]);
-            for (int q = 0; q < 4; ++q) { node_a[i][q] = lo[i] + h[i] * (1.0 + t[q]); node_T[i][q] = radial_T(node_a[i][q]); }
-            for (int q = 0; q < kChk; ++q) { chk_a[i][q] = (double)(float)(lo[i] + (hi[i] - lo[i]) * q / 64.0); chk_T[i][q] = radial_T(chk_a[i][q]); }
-        }
-    }
-};
-} // namespace
-
-// The filtered pre-pass's radial table (approx_v): R(a) = T(a) s(theta) with theta^2 = a T(a)^2 and s = 1 + k0 theta^2 + ... + k3 theta^8,
-// one cubic c0 + d (c1 + d (c2 + d c3)) in d = a - lo per 1/16-octave interval [lo, hi) of a over [2^-30, 2^14), fitted in f64 at the
-// interval's four Chebyshev nodes and rounded to f32.  The rows below 2^-30 repeat the first fitted row (R changes by less than 2^-29
-// relative there); a_cap (filter_a_cap) is rounded down to an interval boundary, and the rows from there on hold NaN, up to the last of
-// the GF_RADIAL_ROWS bit patterns.  Every fitted row is checked on 65 points: the f32 coefficients' cubic, evaluated in f64, must stay
-// within kRadialBudget (relative) of R, the table error of profiles/FILTER_ANALYSIS.md step 3.  Returns the rounded a_cap, or 0 when
-// some row misses the budget: then the lens runs without the filter.
-float gf::build_radial_table(const float* k, float a_cap, float4* rows) {
-    static const RadialGrid* const G = new RadialGrid();
-    constexpr double kRadialBudget = 0x1p-23;
-    uint32_t cap_bits; memcpy(&cap_bits, &a_cap, 4);
-    const int n_valid = std::max(0, std::min(GF_RADIAL_FIT_ROWS, (int)(cap_bits >> 19) - GF_RADIAL_FIT));
-    const double k0 = k[0], k1 = k[1], k2 = k[2], k3 = k[3];
-    auto R = [&](double a, double T) { const double q = a * T * T; return T * (1.0 + q * (k0 + q * (k1 + q * (k2 + q * k3)))); };
-    bool ok = n_valid > 0;
-    for (int i = 0; i < GF_RADIAL_ROWS; ++i) rows[i] = make_float4(NAN, NAN, NAN, NAN);
-    for (int i = 0; i < n_valid; ++i) {
-        double f[4], c[4];
-        for (int q = 0; q < 4; ++q) f[q] = R(G->node_a[i][q], G->node_T[i][q]);
-        for (int r = 0; r < 4; ++r) c[r] = G->vinv[r][0] * f[0] + G->vinv[r][1] * f[1] + G->vinv[r][2] * f[2] + G->vinv[r][3] * f[3];
-        const double hh = G->h[i];
-        const float4 row = make_float4((float)c[0], (float)(c[1] / hh), (float)(c[2] / (hh * hh)), (float)(c[3] / (hh * hh * hh)));
-        rows[GF_RADIAL_FIT + i] = row;
-        for (int q = 0; q < RadialGrid::kChk; ++q) {
-            const double a = G->chk_a[i][q], d = a - G->lo[i];
-            const double v = row.x + d * (row.y + d * (row.z + d * (double)row.w));
-            const double want = R(a, G->chk_T[i][q]);
-            if (!(fabs(v - want) <= kRadialBudget * fabs(want))) ok = false;
-        }
-    }
-    for (int i = 0; i < GF_RADIAL_FIT; ++i) rows[i] = rows[GF_RADIAL_FIT];
-    uint32_t r_bits = cap_bits & 0xfff80000u; float a_cap_r; memcpy(&a_cap_r, &r_bits, 4);
-    return ok ? a_cap_r : 0.0f;
-}
-
-namespace {
-
 // One frame through the warp: `FrameJob job{in, out, p, matrices, rows, mesh, mesh_len, stream}`, then the options a call needs.
 struct FrameJob {
     const gf_buffer_desc* in; const gf_buffer_desc* out; const gf_kernel_params* p;   // arrays of 1 + more_planes planes
@@ -420,7 +309,7 @@ struct Plan {
     bool two_pass;                  // coordinates into a map (pass 1), then one sampling launch per plane (pass 2)
     int n_maps;                     // coordinate maps of pass 1: 1, or 3 for EWA (pixel + two Jacobian probes)
     KernelVariant kernel;           // what renders pass 1 (or the whole frame)
-    float a_cap;                    // > 0: the packed kernel runs the filtered rolling-shutter pre-pass with this bound
+    bool filter;                    // the packed kernel runs the filtered rolling-shutter pre-pass if the lens has a radial table
 };
 // A holds the frame's filled uniforms; table_flags is what the HOST knows of the matrix table (0 = tame and IBIS-free, non-zero =
 // anything else, including device tables not scanned on the host).  Of the job only its shape is read.
@@ -440,24 +329,11 @@ Plan plan_frame(const Combo& c, const WarpArgs& A, uint32_t table_flags, const F
     const KernelVariant packed = pl.two_pass ? KV_PACKED_COORDS : KV_PACKED;
     const bool packed_ok = lean_ok && c.kernels[packed] && (A.feat & F_WILD) == 0 && pl.n_maps == 1;
     pl.kernel = packed_ok ? packed : (lean_ok ? KV_LEAN : KV_GENERAL);
-    // filtered pre-pass: fisheye without a digital lens, rolling shutter on, geometry that fits the queue's 16 + 16 bit entries; host
-    // tables known to be wild / IBIS take the guarded path, which has no tail launch
-    pl.a_cap = (packed_ok && c.lens == GF_LENS_OPENCV_FISHEYE && c.digital == GF_LENS_NONE && (A.feat & F_RS) && !c.no_filter &&
-                A.out_cols <= 65536 && A.out_rows <= 131072 && (s.tables_on_device || table_flags == 0)) ? filter_a_cap(A.p.k) : 0.0f;
+    // filtered pre-pass: rolling shutter on, geometry that fits the queue's entries; host tables known to be wild / IBIS take the
+    // guarded path, which has no tail launch
+    pl.filter = packed_ok && filter_pair(c.lens, c.digital) && (A.feat & F_RS) && !c.no_filter && A.out_cols <= WarpArgs::X2Filter::kMaxCols &&
+                A.out_rows <= WarpArgs::X2Filter::kMaxRows && (s.tables_on_device || table_flags == 0);
     return pl;
-}
-
-// Packed-kernel launches use programmatic stream serialization: the grid may be scheduled while the previous kernel on the stream
-// (the frame's producer kernel, the previous frame's tail, ...) is still draining; every CTA executes griddepcontrol.wait before it
-// touches memory, so the dependency itself is unchanged and only the kernel-to-kernel launch gap disappears.
-cudaError_t launch_pdl(KernelFn fn, dim3 g, dim3 b, const WarpArgs& args, cudaStream_t st) {
-    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    void* kargs[1] = { (void*)&args };
-    return cudaLaunchKernelExC(&cfg, (const void*)fn, kargs);
 }
 
 // Planes of one frame that share their geometry (GBRAPF32's four R32f planes, the U and V planes of planar YUV, ...):
@@ -492,7 +368,7 @@ struct FrameRun {
     bool full_cover = false;                // the kernel writes every output byte that travels back
     const uint8_t* drawing_dev = nullptr;
     Plan plan;
-    RadialTable* radial = nullptr;          // the filtered pre-pass's table for this frame's lens (plan.a_cap > 0)
+    const FilterPrepass::Table* radial = nullptr;   // the lens's radial table when the frame runs the filtered pre-pass
     dim3 grid;                              // of the scalar kernels and the sampling pass (blocks of kBlock)
 
     // Tables and mesh: host tables are copied through a slot and scanned on the host; a mesh is widened to f64 on the device.
@@ -579,26 +455,7 @@ struct FrameRun {
         grid = dim3((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);
         if (grid.x == 0 || grid.y == 0 || grid.y > 65535) return fail(err, GF_ERR_BAD_PARAMS, "output buffer geometry out of range");
         plan = plan_frame(ctx->combo, A, table_flags, job);
-        if (plan.a_cap > 0.0f) {                               // the lens's radial table: cached, or rebuilt in the least recently used entry
-            uint32_t key[4]; memcpy(key, A.p.k, sizeof(key));
-            RadialTable* lru = &ctx->radial[0];
-            for (RadialTable& t : ctx->radial) {
-                if (t.filled && memcmp(t.key, key, sizeof(key)) == 0) radial = &t;
-                if (t.last_use < lru->last_use) lru = &t;
-            }
-            if (!radial) {
-                radial = lru;
-                radial->filled = false;
-                if (!radial->done) CK(err, create_event(radial->done));
-                CK(err, cudaEventSynchronize(radial->done.get()));       // every frame that read this entry has finished
-                CK(err, radial->h.reserve(GF_RADIAL_ROWS, st)); CK(err, radial->d.reserve(GF_RADIAL_ROWS, st));
-                radial->a_cap = build_radial_table(A.p.k, plan.a_cap, radial->h.ptr);
-                memcpy(radial->key, key, sizeof(key)); radial->filled = true; radial->uploaded = false;
-                ctx->radial_builds++;
-            }
-            radial->last_use = ++ctx->radial_uses;
-            plan.a_cap = radial->a_cap;
-        }
+        if (plan.filter) { const int rc = ctx->filter.table(A.p.k, st, err, &radial); if (rc != GF_OK) return rc; }
         if (plan.two_pass) {
             if (!ctx->fn_shade && !job.coord_only) return fail(err, GF_ERR_UNSUPPORTED_COMBO, "no sampling kernel for this pixel layout");
             CK(err, ctx->coords.reserve((size_t)A.out_cols * (size_t)A.out_rows * (size_t)plan.n_maps, st));
@@ -613,33 +470,8 @@ struct FrameRun {
         if (plan.kernel == KV_PACKED || plan.kernel == KV_PACKED_COORDS) {
             // 32 x 4 threads (4 x 8 output rows... 32 x 8 pixels) per block measured 2 % faster than 32 x 8 threads (finer tail)
             const dim3 block2(GF_BLOCK_X, kPackedBlockY), grid2(grid.x, (A.out_rows + 2 * kPackedBlockY - 1) / (2 * kPackedBlockY));
-            if (plan.a_cap > 0.0f) {
-                if (!ctx->defer_q.ptr) {
-                    CK(err, ctx->defer_q.reserve(kDeferCap, st)); CK(err, ctx->defer_count.reserve(2, st));
-                    CK(err, cudaMemsetAsync(ctx->defer_count.ptr, 0, 2 * sizeof(unsigned), st));
-                }
-                const unsigned cur = (unsigned)(ctx->filter_frames & 1ull);
-                ctx->filter_frames++;
-                A.feat |= F_FILTER;
-                A.flt.q = ctx->defer_q.ptr; A.flt.cap = (uint32_t)ctx->defer_q.len;
-                A.flt.count = ctx->defer_count.ptr + cur; A.flt.count_next = ctx->defer_count.ptr + (cur ^ 1u);
-                RadialTable& rt = *radial;
-                if (!rt.uploaded) {
-                    CK(err, cudaMemcpyAsync(rt.d.ptr, rt.h.ptr, GF_RADIAL_ROWS * sizeof(float4), cudaMemcpyHostToDevice, st));
-                    rt.uploaded = true;
-                }
-                // eps = (rho + 2^-22) |t - c_y| + 2^-22 |c_y| with rho = 2^-17 (profiles/FILTER_ANALYSIS.md; |c_y| >= 2^-10 without F_WILD)
-                A.flt.mid_row = A.matrices + (size_t)(A.p.matrix_count / 2) * GF_MATRIX_STRIDE;
-                A.flt.rtab = rt.d.ptr; A.flt.eps_rel = 0x1p-17f + 0x1p-22f; A.flt.eps_abs = 0x1p-22f * fabsf(A.p.c[1]);
-                A.flt.tail = 0;
-                CK(err, launch_pdl(fn, grid2, block2, A, st));
-                CK(err, cudaEventRecord(rt.done.get(), st));   // the tail launch runs the exact pre-pass and does not read the table
-                A.flt.tail = 1;                                // the deferred pairs, exact pre-pass; also re-arms the other counter
-                // one thread per deferred pair for up to 2 % of a 4K frame's pairs in a single wave of tiny blocks (idle blocks exit at once);
-                // more entries than threads are covered by the grid-stride loop
-                CK(err, launch_pdl(fn, dim3(ctx->sm_count * kTailBlocksPerSM, 1), block2, A, st));
-                ctx->launches++;
-            } else CK(err, launch_pdl(fn, grid2, block2, A, st));
+            if (radial) { const int rc = ctx->filter.launch(fn, grid2, block2, A, *radial, st, err, ctx->launches); if (rc != GF_OK) return rc; }
+            else CK(err, launch_pdl(fn, grid2, block2, A, st));
         } else {
             const size_t map_len = (size_t)A.out_cols * (size_t)A.out_rows;
             for (int mi = 0; mi < plan.n_maps; ++mi) {        // one launch, or three for EWA (pixel, x-probe, y-probe)
@@ -752,6 +584,19 @@ int gf_internal_run_frame(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_b
     return run_warp(ctx, job);
 }
 
+// Packed-kernel launches use programmatic stream serialization: the grid may be scheduled while the previous kernel on the stream
+// (the frame's producer kernel, the previous frame's tail, ...) is still draining; every CTA executes griddepcontrol.wait before it
+// touches memory, so the dependency itself is unchanged and only the kernel-to-kernel launch gap disappears.
+cudaError_t gf::launch_pdl(KernelFn fn, dim3 g, dim3 b, const WarpArgs& args, cudaStream_t st) {
+    cudaLaunchConfig_t cfg; memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = g; cfg.blockDim = b; cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    void* kargs[1] = { (void*)&args };
+    return cudaLaunchKernelExC(&cfg, (const void*)fn, kargs);
+}
+
 bool gf::lens_noop(int lens, const float* k) {
     switch (lens) {
     case GF_LENS_OPENCV_FISHEYE:
@@ -825,7 +670,7 @@ GF_API int gf_cuda_create(gf_cuda_ctx** out_ctx, int device, const gf_kernel_par
     ctx->width = params->width; ctx->height = params->height; ctx->output_width = params->output_width; ctx->output_height = params->output_height;
 
     CK(nullptr, cudaSetDevice(device));
-    CK(nullptr, cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device));
+    CK(nullptr, ctx->filter.init(device));
     CK(nullptr, create_stream(ctx->stream));
     CK(nullptr, create_event(ctx->last_call));
     const cudaStream_t st = ctx->stream.get();
@@ -1101,7 +946,7 @@ GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_
 // IBIS rows, non-zero = anything else.  Returns 0 general, 1 lean, 2 packed, 3 packed + trusted tables, | 0x10 two-pass (plan_frame,
 // the planner run_warp uses), or a negative GF_ERR_*.  A planning aid for integrators and the hook the CPU-only tests use to check
 // the host logic.  gf_cuda_plan_features also writes the frame's feature word (F_* of warp_kernel.cuh) to *feat_out: the bits
-// fill_uniforms computes, plus F_FILTER when the plan runs the filtered pre-pass (launch() sets that bit at launch time).
+// fill_uniforms computes, plus F_FILTER when the plan runs the filtered pre-pass (FilterPrepass::launch sets that bit at launch time).
 GF_API int gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
                                  const gf_buffer_desc* in, const gf_buffer_desc* out, size_t mesh_len, uint32_t table_flags, size_t n_planes,
                                  uint32_t* feat_out) {
@@ -1118,18 +963,17 @@ GF_API int gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type,
     FrameJob job{in, out, params, nullptr, 0, nullptr, mesh_len, nullptr};
     job.more_planes = n_planes > 1 ? n_planes - 1 : 0;
     Plan pl = plan_frame(c, A, table_flags, job);
-    if (pl.a_cap > 0.0f) { std::vector<float4> rows(GF_RADIAL_ROWS); pl.a_cap = build_radial_table(A.p.k, pl.a_cap, rows.data()); }   // as plan_launch
+    if (pl.filter) { std::vector<float4> rows(GF_RADIAL_ROWS); pl.filter = radial_table_cap(A.p.k, rows.data()) > 0.0f; }   // as FilterPrepass::table
     // packed: the trusted path runs when the table's verdict word is 0, which the host knows only for tables it scanned
     const int v = pl.kernel == KV_GENERAL ? 0 : (pl.kernel == KV_LEAN ? 1 : (table_flags == 0 ? 3 : 2));
-    if (feat_out) *feat_out = A.feat | (pl.a_cap > 0.0f ? (uint32_t)F_FILTER : 0u);
+    if (feat_out) *feat_out = A.feat | (pl.filter ? (uint32_t)F_FILTER : 0u);
     return v | (pl.two_pass ? 0x10 : 0);
 }
 
 GF_API int gf_filter_radial_table(const float* k, float* rows_out, size_t rows_cap, float* a_cap_out) {
     if (!k || !rows_out || !a_cap_out || rows_cap < (size_t)GF_RADIAL_ROWS) return GF_ERR_BAD_PARAMS;
-    const float cap = filter_a_cap(k);
-    std::vector<float4> rows(GF_RADIAL_ROWS, make_float4(NAN, NAN, NAN, NAN));
-    *a_cap_out = cap > 0.0f ? build_radial_table(k, cap, rows.data()) : 0.0f;
+    std::vector<float4> rows(GF_RADIAL_ROWS);
+    *a_cap_out = radial_table_cap(k, rows.data());
     memcpy(rows_out, rows.data(), rows.size() * sizeof(float4));
     return GF_RADIAL_ROWS;
 }
@@ -1166,18 +1010,9 @@ GF_API int gf_cuda_synchronize(gf_cuda_ctx* ctx) {
 
 GF_API int gf_cuda_filter_stats(gf_cuda_ctx* ctx, uint64_t* out6) {
     if (!ctx || !out6) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    std::string* const err = &ctx->last_error;
     int rc = gf_cuda_synchronize(ctx);
     if (rc != GF_OK) return rc;
-    unsigned count = 0;
-    if (ctx->filter_frames > 0) {
-        CK(err, cudaMemcpyAsync(&count, ctx->defer_count.ptr + ((ctx->filter_frames - 1) & 1ull), sizeof(count), cudaMemcpyDeviceToHost, ctx->stream.get()));
-        CK(err, cudaStreamSynchronize(ctx->stream.get()));
-    }
-    out6[0] = ctx->filter_frames; out6[1] = count; out6[2] = kDeferCap;
-    out6[3] = (uint64_t)ctx->sm_count * kTailBlocksPerSM * GF_BLOCK_X * kPackedBlockY;
-    out6[4] = ctx->radial_builds; out6[5] = ctx->radial_uses - ctx->radial_builds;
-    return GF_OK;
+    return ctx->filter.stats(ctx->stream.get(), &ctx->last_error, out6);
 }
 
 GF_API int gf_cuda_set_overlays(gf_cuda_ctx* ctx, int enabled) {

@@ -105,11 +105,36 @@ CameraStab camera_stab_at(const gf_compute_params* cp, size_t frame, bool frameb
 bool lens_noop(int lens, const float* k);
 // the point path (zoom_kernel.cu) compiles this (lens, digital lens) pair
 bool point_path_supported(int lens, int digital);
-// Filtered rolling-shutter pre-pass of the packed fisheye kernel (c_abi.cu): the conditioning cap on r^2 for fisheye coefficients
-// k[0..3] (0: no filter), and the lens's radial table below it — GF_RADIAL_ROWS rows, returns the cap rounded down to a row boundary
-// (NaN rows from there on), or 0 when the table misses its error budget.
-float filter_a_cap(const float* k);
-float build_radial_table(const float* k, float a_cap, float4* rows);
+
+// ---- Filtered rolling-shutter pre-pass of the packed fisheye kernel (filter_prepass.cu) ----
+struct WarpArgs;
+typedef void (*KernelFn)(const WarpArgs);      // as kernel_registry.h
+cudaError_t launch_pdl(KernelFn fn, dim3 g, dim3 b, const WarpArgs& args, cudaStream_t st);    // c_abi.cu
+// The radial table (GF_RADIAL_ROWS rows, Lens2<opencv_fisheye>::approx_v) of fisheye coefficients k[0..3]: returns the conditioning cap
+// on r^2 rounded down to a row boundary (NaN rows from there on), or 0 when the lens runs without the filter.
+float radial_table_cap(const float* k, float4* rows);
+// One per context: the radial tables of the last four lenses, the deferred-pair queue with its two ping-pong counters, and the launches
+// of a filtered frame.  They rely on the context's calls being ordered on the device (gf_cuda_ctx::last_call).
+class FilterPrepass {
+public:
+    struct Table {                             // rebuilt only once `done` has passed: it is recorded after the upload and every reader
+        uint32_t key[4] = {};
+        float a_cap = 0.0f;                    // radial_table_cap
+        unsigned long long last_use = 0;       // 0: empty
+        GrowBuf<float4, true> h; GrowBuf<float4> d; Event done;
+    };
+    cudaError_t init(int device) { return cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, device); }
+    // The lens's table, cached by the bits of k[0..3] or built in the least recently used entry and uploaded on `st`; nullptr: no filter.
+    int table(const float* k, cudaStream_t st, std::string* err, const Table** out);
+    // The main launch, which defers the pairs it cannot certify, and the tail launch, which renders them; the tail is added to `launches`.
+    int launch(KernelFn fn, dim3 grid, dim3 block, WarpArgs& A, const Table& t, cudaStream_t st, std::string* err, unsigned long long& launches);
+    int stats(cudaStream_t st, std::string* err, uint64_t* out6) const;    // gf_cuda_filter_stats, once `st` has every frame behind it
+private:
+    Table tables[4];
+    GrowBuf<uint32_t> queue; GrowBuf<unsigned> counts;
+    unsigned long long frames = 0, uses = 0, builds = 0;
+    int sm_count = 1;
+};
 
 // What generate_stmaps does to the user's ComputeParams before either map (stmap.rs:24-35, :44-46): rotation suppressed, fovs cleared,
 // no readout time unless per_frame, fov_scale 1 and the output size the frame size.

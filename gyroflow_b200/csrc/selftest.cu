@@ -128,7 +128,7 @@ __global__ void sweep_kernel(uint32_t lo, uint32_t hi, int which, unsigned long 
 // rotation of up to ~25 degrees with random translation terms, frame sizes 1280..8192) every pixel of a sampled grid is evaluated both
 // ways.  out[0] = pixels inside the regime, out[1] = pixels whose |tv_approx - tv_exact| EXCEEDS the certificate's bound (must be 0),
 // out[2] = pixels the certificate calls uncertain (distance to the rounding boundary <= bound), out[3] = max |diff| / bound in 1e-6 units.
-// Each configuration's lens has its own radial table (build_radial_table, as the warp builds it); a lens whose table misses the error
+// Each configuration's lens has its own radial table (radial_table_cap, as the warp builds it); a lens whose table misses the error
 // budget would run without the filter and is skipped.
 struct FilterCfg { float m[9]; float k[4]; float f1, c1; int on; int w, h; };
 __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, const float4* __restrict__ tabs, int n_cfg, int step, float rho,
@@ -138,7 +138,7 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, const fl
         const FilterCfg C = cfgs[ci];
         if (!C.on) continue;
         const float4* const rtab = tabs + (size_t)ci * GF_RADIAL_ROWS;
-        const float eps_rel = rho + 0x1p-22f, eps_abs = 0x1p-22f * fabsf(C.c1);     // the kernel's certificate tolerance
+        const FilterEps eps = filter_eps(C.c1, rho);                                  // the kernel's certificate tolerance
         gf_kernel_params P; memset(&P, 0, sizeof(P));
         for (int i = 0; i < 4; ++i) P.k[i] = C.k[i];
         P.f[0] = C.f1; P.f[1] = C.f1; P.c[0] = 0.5f * (float)C.w; P.c[1] = C.c1;
@@ -156,7 +156,7 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, const fl
             float ex, ey;
             Lens<GF_LENS_OPENCV_FISHEYE>::distort(_x, _y, _w, P, false, ex, ey);       // the reference's arithmetic (scalar exact code)
             const float tv_exact = ey * P.f[1] + P.c[1];
-            const float bound = __fmaf_rn(fabsf(tvc), eps_rel, eps_abs);
+            const float bound = __fmaf_rn(fabsf(tvc), eps.rel, eps.abs);
             const float diff = fabsf(tv - tv_exact);
             ++in_regime;
             if (!(diff <= bound)) ++violations;
@@ -190,8 +190,7 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
         const double B = t2 * (fabs(k[0]) + t2 * (fabs(k[1]) + t2 * (fabs(k[2]) + t2 * fabs(k[3]))));
         const double sc = (i % 7 == 0) ? 0.02 / B : 0.25 / B;                 // every 7th: a weak lens (cap at 1.55 rad)
         for (int j = 0; j < 4; ++j) C.k[j] = (float)(k[j] * sc);
-        const float a_cap = filter_a_cap(C.k);
-        C.on = a_cap > 0.0f && build_radial_table(C.k, a_cap, &tabs[(size_t)i * GF_RADIAL_ROWS]) > 0.0f;
+        C.on = radial_table_cap(C.k, &tabs[(size_t)i * GF_RADIAL_ROWS]) > 0.0f;
         // mid-row matrix: (K_new R)^-1 with focal length 0.3..1.2 widths and a rotation of up to ~25 degrees about a random axis
         const double f = (0.3 + 0.9 * rnd()) * C.w, cx = 0.5 * C.w, cy = 0.5 * C.h;
         double ax[3] = { rnd() - 0.5, rnd() - 0.5, rnd() - 0.5 }; const double an = sqrt(ax[0]*ax[0] + ax[1]*ax[1] + ax[2]*ax[2]) + 1e-12;
@@ -212,7 +211,7 @@ extern "C" GF_API int gf_cuda_selftest_filter(int device, unsigned long long see
     CK(nullptr, cudaMemcpy(d_cfg.ptr, cfgs.data(), cfgs.size() * sizeof(FilterCfg), cudaMemcpyHostToDevice));
     CK(nullptr, cudaMemcpy(d_tab.ptr, tabs.data(), tabs.size() * sizeof(float4), cudaMemcpyHostToDevice));
     CK(nullptr, cudaMemset(d_out.ptr, 0, 4 * sizeof(unsigned long long)));
-    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg.ptr, d_tab.ptr, n_cfg, step, 0x1p-17f, d_out.ptr);
+    filter_check_kernel<<<dim3(132, (unsigned)(n_cfg < 64 ? n_cfg : 64)), 256>>>(d_cfg.ptr, d_tab.ptr, n_cfg, step, kFilterRho, d_out.ptr);
     CK(nullptr, cudaGetLastError());
     CK(nullptr, cudaDeviceSynchronize());
     CK(nullptr, cudaMemcpy(out4, d_out.ptr, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));

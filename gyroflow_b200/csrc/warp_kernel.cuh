@@ -95,6 +95,12 @@ constexpr int GF_RADIAL_ROWS = 8192;
 constexpr int GF_RADIAL_FIT = (127 - 30) << 4;
 constexpr int GF_RADIAL_FIT_ROWS = (14 + 30) * 16;
 
+// Tolerance of the filtered pre-pass's certificate (profiles/FILTER_ANALYSIS.md): eps = (rho + 2^-22) |t - c_y| + 2^-22 |c_y|, as
+// X2Filter's eps_rel and eps_abs.
+constexpr float kFilterRho = 0x1p-17f;
+struct FilterEps { float rel, abs; };
+GF_HD FilterEps filter_eps(float c_y, float rho = kFilterRho) { return { rho + 0x1p-22f, 0x1p-22f * fabsf(c_y) }; }
+
 struct WarpArgs {
     gf_kernel_params p;             // verbatim KernelParams
     const uint8_t* src;
@@ -109,6 +115,7 @@ struct WarpArgs {
     // filtered rolling-shutter pre-pass of the packed kernel (F_FILTER): pairs whose row choice the approximate evaluation cannot
     // certify are appended to `q` and rendered by a second launch of the same kernel in tail mode
     struct X2Filter {
+        static constexpr int kMaxCols = 1 << 16, kMaxRows = 2 << 16;   // the output geometry a queue entry can address
         uint32_t* q;                // deferred pairs: x | (y0 / 2) << 16
         unsigned* count;            // number of entries appended by this frame's main launch
         unsigned* count_next;       // the next frame's counter, zeroed by this frame's tail launch
@@ -116,7 +123,7 @@ struct WarpArgs {
         int       tail;             // 1 = this launch renders the queue
         const float4* rtab;         // the lens's radial table (GF_RADIAL_ROWS rows, approx_v in warp_kernel_x2.cuh)
         const float*  mid_row;      // the matrix table's middle row, matrices + (matrix_count / 2) * GF_MATRIX_STRIDE
-        float     eps_rel, eps_abs; // tolerance of the certificate: eps = eps_rel |t - c_y| + eps_abs = (rho + 2^-22) |t - c_y| + 2^-22 |c_y|
+        float     eps_rel, eps_abs; // tolerance of the certificate: eps = eps_rel |t - c_y| + eps_abs (filter_eps)
     } flt;
     int            coord_shift;     // pass 1: 0 = pixel (x, y); 1 = (x + 0.01, y); 2 = (x, y + 0.01) — the EWA Jacobian probes of :567-572
     int            coord_maps;      // pass 2: 1, or 3 when the two probe maps follow the first one (stride out_cols * out_rows)

@@ -40,9 +40,8 @@ GF_DEV bool zero_or_in_window(float v) {
 // All predicates are combined with & and | (never && / ||) so that no branch is generated for them.
 // ------------------------------------------------------------------------------------------
 template <int M> struct Lens2 { static constexpr bool kHas = false; };
-// lens models with an approximate v evaluation for the filtered rolling-shutter pre-pass (Lens2<M>::approx_v)
-template <int M> struct LensApprox { static constexpr bool value = false; };
-template <> struct LensApprox<GF_LENS_OPENCV_FISHEYE> { static constexpr bool value = true; };
+// lens pairs whose packed kernel has the filtered rolling-shutter pre-pass (an approximate v evaluation, Lens2<M>::approx_v)
+__host__ __device__ constexpr bool filter_pair(int lens, int digital) { return lens == GF_LENS_OPENCV_FISHEYE && digital == GF_LENS_NONE; }
 
 // opencv_fisheye.rs:72-93 (k != 0: the lean kernel is only chosen when F_LENS_NOOP is clear; |k| bounded by the host)
 template <> struct Lens2<GF_LENS_OPENCV_FISHEYE> {
@@ -50,9 +49,9 @@ template <> struct Lens2<GF_LENS_OPENCV_FISHEYE> {
     // FILTERED PRE-PASS.  The mid-row evaluation of cpu_undistort.rs:470-479 only decides which matrix row a pixel uses:
     // idx = clamp(round(v_mid), 0, H).  This is v_mid - c_y computed CHEAPLY — one MUFU.RCP instead of two refined divisions, no
     // square root, the whole radial factor R(a) = (atan(r) / r) * (1 + k0 theta^2 + ... + k3 theta^8) from the lens's cubic table in
-    // a = r^2 (`rtab`, built and checked by the host: build_radial_table in c_abi.cu), fused multiply-adds — together with a proven
-    // bound on its distance from the reference's own float result (profiles/FILTER_ANALYSIS.md):
-    //     |tv_approx - tv_exact| <= (rho + 2^-22) * |tv - c_y| + 2^-22 * |c_y|,   rho = 2^-17,
+    // a = r^2 (`rtab`, built and checked by the host: build_radial_table in filter_prepass.cu), fused multiply-adds — together with a
+    // proven bound on its distance from the reference's own float result (profiles/FILTER_ANALYSIS.md):
+    //     |tv_approx - tv_exact| <= (rho + 2^-22) * |tv - c_y| + 2^-22 * |c_y|,   rho = kFilterRho (filter_eps),
     // valid while the divisor w is in the window of the exact sequences and r^2 is below the host's conditioning cap (the polynomial
     // stays within [3/4, 5/4]).  The table's rows from that cap on hold NaN, so tvc is NaN there and fails the certificate.
     // (_x, _y, _w) are the reference's own unfused products — bit-identical to the exact chain — so only relative perturbations enter
@@ -690,7 +689,7 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
     const int lim = A.row_lim;
     int sy_a = 0, sy_b = 0;
     do {      // `break`: the rows are known
-        if constexpr (TRUSTED && LensApprox<LENS>::value && DIGITAL == GF_LENS_NONE) {
+        if constexpr (TRUSTED && filter_pair(LENS, DIGITAL)) {
             if (!exact_prepass) {                        // F_FILTER, which implies F_RS (host)
                 // :470-479, filtered: certify round(v_mid) from the approximate evaluation, defer the pair when it cannot be
                 const MatRow9 rm = load_row9(A.flt.mid_row, 0u);
@@ -771,7 +770,7 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
 template <int LENS, int DIGITAL, class PIX, int MINB, bool COORD = false>
 __global__ void __launch_bounds__(GF_BLOCK_X * GF_BLOCK_Y, MINB)
 warp_kernel_x2(const __grid_constant__ WarpArgs A) {
-    constexpr bool kFilter = LensApprox<LENS>::value && DIGITAL == GF_LENS_NONE;
+    constexpr bool kFilter = filter_pair(LENS, DIGITAL);
     // launched with programmatic stream serialization (c_abi.cu: launch_pdl): nothing of the previous kernel on the stream — the matrix
     // table and its verdict word, the deferred-pair queue and its counters, the previous frame's output — may be read or written before this
     asm volatile("griddepcontrol.wait;" ::: "memory");

@@ -1,4 +1,4 @@
-"""The bookkeeping around the packed fisheye kernel's filtered rolling-shutter pre-pass (c_abi.cu: plan_launch / launch; warp_kernel_x2.cuh:
+"""The bookkeeping around the packed fisheye kernel's filtered rolling-shutter pre-pass (FilterPrepass in filter_prepass.cu; warp_kernel_x2.cuh:
 the deferral in warp_x2_body and the tail branch of warp_kernel_x2): the deferred-pair queue and its inline fallback when it is full, the
 tail launch's grid-stride loop, the ping-pong counters across frames of every kind, the per-context radial-table cache, and the ordering of
 calls on one context that name different streams.
@@ -18,7 +18,7 @@ from tests import cases, oracle_lib
 QUEUE_CAP = 1 << 20
 K_SMALLEST_CAP = [-0.25 / 0.5 ** 2 * 0.999, 0.0, 0.0, 0.0] + [0.0] * 8      # one-term lens at the smallest cap the filter accepts (0.5 rad)
 K_BAND = [-0.42, 0.0, 0.0, 0.0] + [0.0] * 8                                # cap inside a 4K frame: a band of corners defers
-K_NO_FILTER = [40.0, 0.0, 0.0, 0.0] + [0.0] * 8                            # conditioning cap below 0.5 rad: no table, no filter
+K_NO_FILTER = [40.0, 0.0, 0.0, 0.0] + [0.0] * 8                            # conditioning cap below 0.5 rad: no filter
 
 
 def radial_cap(k):

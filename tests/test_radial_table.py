@@ -1,4 +1,4 @@
-"""The filtered pre-pass's per-lens radial table (build_radial_table in c_abi.cu, read by Lens2<opencv_fisheye>::approx_v), replayed on the
+"""The filtered pre-pass's per-lens radial table (build_radial_table in filter_prepass.cu, read by Lens2<opencv_fisheye>::approx_v), replayed on the
 host through gf_filter_radial_table: which rows are fitted, which repeat the first fitted row and which are NaN, the rounded r^2 cap, and
 the fit error against R(a) = T(a) s(theta) off the 65 points per row the host checks."""
 import ctypes as C
