@@ -148,6 +148,18 @@ class QueueConfig(C.Structure):
     ]
 
 
+class QueuePlane(C.Structure):
+    """gf_queue_plane: one plane of a planes queue's layout (pixel type, size fraction of the frame, max value, background in the
+    plane's components)."""
+    _fields_ = [("pixel_type", C.c_int32), ("w_div", C.c_int32), ("h_div", C.c_int32), ("max_value", C.c_float),
+                ("background", C.c_float * 4)]
+
+
+class ChecksumPlane(C.Structure):
+    """gf_checksum_plane: `rows` rows of `row_bytes` bytes, `stride` bytes apart, summed by gf_cuda_checksum_planes_dev."""
+    _fields_ = [("ptr", C.c_void_p), ("row_bytes", C.c_size_t), ("stride", C.c_size_t), ("rows", C.c_size_t)]
+
+
 # KernelParamsFlags — stabilization/mod.rs:85-98
 FLAG_FIX_COLOR_RANGE, FLAG_HAS_DIGITAL_LENS, FLAG_FILL_WITH_BACKGROUND, FLAG_DRAWING_ENABLED = 1, 2, 4, 8
 FLAG_HORIZONTAL_RS, FLAG_HAS_SOURCE_RECT, FLAG_HAS_OUTPUT_RECT, FLAG_FRAMEBUFFER_INVERTED = 16, 32, 64, 128
@@ -262,6 +274,11 @@ EXPORTS = [
     ("gf_cuda_queue_last_error", C.c_char_p, [C.c_void_p]),
     ("gf_cuda_bind_thread_to_device", C.c_int, [C.c_int]),
     ("gf_cuda_checksum_dev", C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("gf_cuda_queue_create_planes", C.c_int, [_P(C.c_void_p), _P(QueueConfig), _P(ComputeParams), C.c_size_t, _P(QueuePlane),
+                                              _P(BufferDesc), _P(BufferDesc)]),
+    ("gf_cuda_queue_submit_planes", C.c_int, [C.c_void_p, C.c_size_t, C.c_double, C.c_size_t, _P(BufferDesc), _P(BufferDesc),
+                                              C.c_void_p, C.c_size_t, C.c_int]),
+    ("gf_cuda_checksum_planes_dev", C.c_int, [_P(ChecksumPlane), C.c_size_t, C.c_void_p, C.c_void_p]),
     ("gf_cuda_host_register", C.c_int, [C.c_void_p, C.c_size_t]),
     ("gf_cuda_host_unregister", C.c_int, [C.c_void_p]),
 ]

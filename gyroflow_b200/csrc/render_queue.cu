@@ -12,6 +12,10 @@
 //     ->  [checksum kernel]  ->  [frame D2H]  ->  event
 // Slots are used round-robin; submit() waits for a slot's previous frame only when it comes round again, wait() hands finished
 // frames back in submission order (output order restored by frame index on the host, as §8e asks).
+// A planes queue (gf_cuda_queue_create_planes) renders decoder frames of 1-4 planes (create_planes_proc!, rendering/mod.rs:483-651):
+// every plane's Stabilization has the frame's size and ComputeParams, so one producer launch serves all planes; per plane only the
+// per-buffer half of KernelParams differs.  Per frame: producer -> [H2D of every plane into the slot's staging] -> one planes call per
+// group (planes of one pixel type and size fraction, one context each) -> [one checksum launch over all planes] -> [D2H of every plane].
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
 #include <sched.h>
@@ -38,6 +42,9 @@ struct QSlot {
     GrowBuf<uint64_t> d_sum; GrowBuf<uint64_t, true> h_sum;  // checksum (device word, pinned host copy)
     bool busy = false;
     size_t frame = 0;
+    // planes queue only: one warp context per plane group, device copies of every plane when the frames are HOST
+    std::vector<std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>>> group_ctx;
+    std::vector<GrowBuf<uint8_t>> plane_in, plane_out;
 };
 
 // sum(word[i] * (2 i + 1)) mod 2^64: order-independent, so blocks may add their partial sums in any order
@@ -49,6 +56,51 @@ __global__ void checksum_kernel(const uint32_t* __restrict__ w, size_t n, unsign
     for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
     if ((threadIdx.x & 31u) == 0u && s) atomicAdd(out, s);
 }
+
+// The same sum over the rows of up to four descriptors read as one byte string (gf_cuda_checksum_planes_dev).  A block takes whole rows;
+// its threads take the string's 32-bit words that the row touches.  A word cut by a row boundary gets its bytes from both rows, each
+// row adding its own bytes times the word's weight, which sums to the whole word's term.
+struct ChecksumRows {
+    const uint8_t* ptr[4];
+    unsigned long long row_bytes[4], stride[4];
+    unsigned long long first_row[5];       // rows of the descriptors before k (first_row[n]: all rows)
+    unsigned long long first_byte[4];      // string offset of descriptor k's first byte
+    unsigned long long end;                // bytes summed: 4 * (string length / 4)
+    int n;
+};
+__global__ void checksum_rows_kernel(const ChecksumRows P, unsigned long long* __restrict__ out) {
+    unsigned long long s = 0;
+    for (unsigned long long r = blockIdx.x; r < P.first_row[P.n]; r += gridDim.x) {
+        int k = 0;
+        while (k + 1 < P.n && r >= P.first_row[k + 1]) ++k;
+        const unsigned long long lr = r - P.first_row[k];
+        const uint8_t* const row = P.ptr[k] + lr * P.stride[k];
+        const unsigned long long g0 = P.first_byte[k] + lr * P.row_bytes[k];                 // string offset of the row's first byte
+        const unsigned long long g1 = min(g0 + P.row_bytes[k], P.end);                       // past its last summed byte
+        if (g0 >= g1) continue;
+        for (unsigned long long w = (g0 >> 2) + threadIdx.x; w < ((g1 + 3) >> 2); w += blockDim.x) {
+            const unsigned long long b0 = max(4ull * w, g0), b1 = min(4ull * w + 4ull, g1);
+            uint32_t v = 0;
+            if (b0 == 4ull * w && b1 == b0 + 4ull && (reinterpret_cast<uintptr_t>(row + (b0 - g0)) & 3u) == 0u) {
+                v = *reinterpret_cast<const uint32_t*>(row + (b0 - g0));
+            } else {
+                for (unsigned long long b = b0; b < b1; ++b) v |= (uint32_t)row[b - g0] << (8u * (unsigned)(b - 4ull * w));
+            }
+            s += (unsigned long long)v * (2ull * w + 1ull);
+        }
+    }
+    #pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31u) == 0u && s) atomicAdd(out, s);
+}
+
+// A planes queue's layout: the planes, their prototypes and per-plane stab configs, and the groups that share a context.
+struct QPlane {
+    gf_queue_plane spec;
+    gf_buffer_desc in_proto, out_proto;
+    gf_stab_config stab;                  // the queue's, with the plane's pixel type and background
+    int group;
+};
 
 } // namespace
 
@@ -62,6 +114,9 @@ struct gf_cuda_queue {
     size_t max_rows = 0;
     unsigned long long launches = 0;
     std::string last_error;
+    std::vector<QPlane> planes;           // empty: a gf_cuda_queue_create queue
+    std::vector<std::vector<size_t>> groups;   // plane indices of each group, in plane order
+    bool host_frames = false;
 };
 
 namespace {
@@ -70,6 +125,46 @@ int finish_slot(gf_cuda_queue* q, QSlot& s) {
     CK(&q->last_error, cudaEventSynchronize(s.done.get()));
     s.busy = false;
     return GF_OK;
+}
+
+// A slot's stream, event, device table + verdict word, mesh staging and checksum word.
+int init_slot(QSlot& s, size_t max_rows) {
+    CK(nullptr, create_stream(s.stream));
+    CK(nullptr, create_event(s.done));
+    const cudaStream_t st = s.stream.get();
+    CK(nullptr, s.d_mat.reserve(max_rows * GF_MATRIX_STRIDE, st));
+    CK(nullptr, s.d_flags.reserve(1, st));
+    CK(nullptr, s.h_mesh.reserve(GF_MESH_MAX_LEN, st));
+    CK(nullptr, s.d_mesh.reserve(GF_MESH_MAX_LEN, st));
+    CK(nullptr, s.d_sum.reserve(1, st));
+    CK(nullptr, s.h_sum.reserve(1, st));
+    *s.h_sum.ptr = 0;
+    return GF_OK;
+}
+
+int enqueue_checksum_rows(const gf_checksum_plane* d, size_t n, uint64_t* out_dev, cudaStream_t st, std::string* err) {
+    if (!d || !out_dev || n < 1 || n > 4) return fail(err, GF_ERR_BAD_PARAMS, "checksum: 1..4 descriptors and an output word");
+    ChecksumRows P; memset(&P, 0, sizeof(P));
+    P.n = (int)n;
+    unsigned long long bytes = 0;
+    for (size_t k = 0; k < n; ++k) {
+        if (!d[k].ptr && d[k].rows && d[k].row_bytes) return fail(err, GF_ERR_BAD_PARAMS, "checksum: descriptor " + std::to_string(k) + " has no pointer");
+        P.ptr[k] = static_cast<const uint8_t*>(d[k].ptr);
+        P.row_bytes[k] = d[k].row_bytes; P.stride[k] = d[k].stride;
+        P.first_row[k + 1] = P.first_row[k] + d[k].rows;
+        P.first_byte[k] = bytes;
+        bytes += (unsigned long long)d[k].rows * d[k].row_bytes;
+    }
+    P.end = bytes & ~3ull;
+    CK(err, cudaMemsetAsync(out_dev, 0, sizeof(uint64_t), st));
+    if (P.end) checksum_rows_kernel<<<132 * 4, 256, 0, st>>>(P, reinterpret_cast<unsigned long long*>(out_dev));
+    CK(err, cudaGetLastError());
+    return GF_OK;
+}
+
+int ceil_div(int a, int b) { return (a + b - 1) / b; }
+bool same_shape(const gf_buffer_desc& a, const gf_buffer_desc& b) {
+    return a.width == b.width && a.height == b.height && a.stride == b.stride && a.kind == b.kind;
 }
 } // namespace
 
@@ -159,16 +254,79 @@ GF_API int gf_cuda_queue_create(gf_cuda_queue** out, const gf_queue_config* cfg,
         rc = gf_cuda_create(&ctx, cfg->device, &kp, cfg->stab.pixel_type, cfg->distortion_model, cfg->digital_lens, in_proto, out_proto, 0);
         if (rc != GF_OK) return rc;
         s.ctx.reset(ctx);
-        CK(nullptr, create_stream(s.stream));
-        CK(nullptr, create_event(s.done));
-        const cudaStream_t st = s.stream.get();
-        CK(nullptr, s.d_mat.reserve(q->max_rows * GF_MATRIX_STRIDE, st));
-        CK(nullptr, s.d_flags.reserve(1, st));
-        CK(nullptr, s.h_mesh.reserve(GF_MESH_MAX_LEN, st));
-        CK(nullptr, s.d_mesh.reserve(GF_MESH_MAX_LEN, st));
-        CK(nullptr, s.d_sum.reserve(1, st));
-        CK(nullptr, s.h_sum.reserve(1, st));
-        *s.h_sum.ptr = 0;
+        if ((rc = init_slot(s, q->max_rows)) != GF_OK) return rc;
+    }
+    *out = q.release();
+    return GF_OK;
+}
+
+GF_API int gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_config* cfg, const gf_compute_params* cp, size_t n_planes,
+                                       const gf_queue_plane* planes, const gf_buffer_desc* in_protos, const gf_buffer_desc* out_protos) {
+    if (!out || !cfg || !cp || !planes || !in_protos || !out_protos) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    *out = nullptr;
+    if (n_planes < 1 || n_planes > 4) return fail(nullptr, GF_ERR_BAD_PARAMS, "n_planes must be 1..4");
+    if (cfg->depth < 1 || cfg->depth > 16) return fail(nullptr, GF_ERR_BAD_PARAMS, "depth must be 1..16");
+    std::unique_ptr<gf_cuda_queue, Deleter<gf_cuda_queue_destroy>> q(new gf_cuda_queue());
+    q->cfg = *cfg; q->cp = *cp;
+    q->host_frames = in_protos[0].kind == GF_BUF_HOST;
+    // everything checkable on the host first: nothing touches the device before the layout is known to be good
+    for (size_t i = 0; i < n_planes; ++i) {
+        const gf_queue_plane& pl = planes[i];
+        const gf_buffer_desc& bi = in_protos[i], &bo = out_protos[i];
+        const std::string name = "plane " + std::to_string(i) + ": ";
+        if ((pl.w_div != 1 && pl.w_div != 2) || (pl.h_div != 1 && pl.h_div != 2)) return fail(nullptr, GF_ERR_BAD_PARAMS, name + "w_div and h_div must be 1 or 2");
+        if (!gf_combo_supported(pl.pixel_type, cfg->distortion_model, cfg->digital_lens, cfg->stab.interpolation))
+            return fail(nullptr, GF_ERR_BAD_PARAMS, name + "no kernel for this (pixel type, lens, digital lens, interpolation)");
+        if ((bi.kind != GF_BUF_HOST && bi.kind != GF_BUF_DEVICE) || bi.kind != in_protos[0].kind || bo.kind != bi.kind || !bi.ptr || !bo.ptr)
+            return fail(nullptr, GF_ERR_BAD_PARAMS, name + "buffers must all be HOST or all DEVICE, with a pointer");
+        if ((pl.pixel_type == GF_PIX_UV8 || pl.pixel_type == GF_PIX_UV16) &&
+            (bi.width != ceil_div(cfg->stab.width, pl.w_div) || bo.width != ceil_div(cfg->stab.output_width, pl.w_div)))
+            return fail(nullptr, GF_ERR_BAD_PARAMS, name + "a UV plane is ceil(W / w_div) pixels wide");
+        if (bo.stride < 1 || bo.height < 1 || bo.len < (size_t)bo.height * (size_t)bo.stride)
+            return fail(nullptr, GF_ERR_BAD_PARAMS, name + "the output buffer holds fewer than height rows of stride bytes");
+        QPlane qp;
+        qp.spec = pl; qp.in_proto = bi; qp.out_proto = bo;
+        qp.stab = cfg->stab; qp.stab.pixel_type = pl.pixel_type;
+        for (int c = 0; c < 4; ++c) qp.stab.background[c] = pl.background[c];
+        qp.group = -1;
+        for (size_t k = 0; k < q->groups.size() && qp.group < 0; ++k) {
+            const gf_queue_plane& o = q->planes[q->groups[k][0]].spec;
+            if (o.pixel_type == pl.pixel_type && o.w_div == pl.w_div && o.h_div == pl.h_div) qp.group = (int)k;
+        }
+        if (qp.group < 0) { qp.group = (int)q->groups.size(); q->groups.emplace_back(); }
+        q->groups[(size_t)qp.group].push_back(i);
+        q->planes.push_back(qp);
+    }
+    CK(nullptr, cudaSetDevice(cfg->device));
+    if (cfg->pin_numa) (void)gf_cuda_bind_thread_to_device(cfg->device);
+    gf_cuda_gyro* gyro = nullptr;
+    int rc = gf_cuda_gyro_upload(&gyro, cfg->device, cp);
+    if (rc != GF_OK) return rc;
+    q->gyro.reset(gyro);
+    q->max_rows = (size_t)(cp->width > cp->height ? cp->width : cp->height);
+    q->slots.resize((size_t)cfg->depth);
+    for (QSlot& s : q->slots) {
+        if ((rc = init_slot(s, q->max_rows)) != GF_OK) return rc;
+        for (const std::vector<size_t>& grp : q->groups) {            // one context per group, created for its first plane's buffers
+            const QPlane& qp = q->planes[grp[0]];
+            gf_buffer_desc bi = qp.in_proto, bo = qp.out_proto;
+            bi.kind = bo.kind = GF_BUF_DEVICE;                         // HOST frames are staged by the queue, the context sees device copies
+            gf_kernel_params kp; memset(&kp, 0, sizeof(kp));
+            kp.matrix_count = 1;
+            rc = gf_get_frame_transform_at(&qp.stab, cp, &bi, &bo, nullptr, 0, 0.0, 0, 1.0, &kp);
+            if (rc != GF_OK) return fail(nullptr, rc, "plane " + std::to_string(grp[0]) + ": gf_get_frame_transform_at failed");
+            gf_cuda_ctx* ctx = nullptr;
+            rc = gf_cuda_create(&ctx, cfg->device, &kp, qp.spec.pixel_type, cfg->distortion_model, cfg->digital_lens, &bi, &bo, 0);
+            if (rc != GF_OK) return rc;
+            s.group_ctx.emplace_back(ctx);
+        }
+        if (q->host_frames) {
+            s.plane_in.resize(n_planes); s.plane_out.resize(n_planes);
+            for (size_t i = 0; i < n_planes; ++i) {
+                CK(nullptr, s.plane_in[i].reserve(q->planes[i].in_proto.len, s.stream.get()));
+                CK(nullptr, s.plane_out[i].reserve(q->planes[i].out_proto.len, s.stream.get()));
+            }
+        }
     }
     *out = q.release();
     return GF_OK;
@@ -178,6 +336,7 @@ GF_API int gf_cuda_queue_submit(gf_cuda_queue* q, size_t frame, double timestamp
                                 const float* mesh, size_t mesh_len) {
     if (!q || !in || !out) return fail(q ? &q->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
     std::string* const err = &q->last_error;
+    if (!q->planes.empty()) return fail(err, GF_ERR_BAD_PARAMS, "a planes queue takes gf_cuda_queue_submit_planes");
     if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
     CK(err, cudaSetDevice(q->cfg.device));
     QSlot& s = q->slots[(size_t)q->next];
@@ -215,6 +374,92 @@ GF_API int gf_cuda_queue_submit(gf_cuda_queue* q, size_t frame, double timestamp
     q->fifo.push_back(q->next);
     q->next = (q->next + 1) % (int)q->slots.size();
     return GF_OK;
+}
+
+GF_API int gf_cuda_queue_submit_planes(gf_cuda_queue* q, size_t frame, double timestamp_ms, size_t n_planes, const gf_buffer_desc* in,
+                                       const gf_buffer_desc* out, const float* mesh, size_t mesh_len, int fill_with_background) {
+    if (!q || !in || !out) return fail(q ? &q->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    std::string* const err = &q->last_error;
+    if (q->planes.empty()) return fail(err, GF_ERR_BAD_PARAMS, "a one-plane queue takes gf_cuda_queue_submit");
+    if (n_planes != q->planes.size()) return fail(err, GF_ERR_BAD_PARAMS, "n_planes differs from the queue's layout (" + std::to_string(q->planes.size()) + ")");
+    if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
+    for (size_t i = 0; i < n_planes; ++i) {
+        const QPlane& qp = q->planes[i];
+        const std::string name = "plane " + std::to_string(i) + ": ";
+        if (in[i].kind != in[0].kind || out[i].kind != in[0].kind) return fail(err, GF_ERR_BAD_PARAMS, name + "HOST and DEVICE buffers mixed in one frame");
+        if (!same_shape(in[i], qp.in_proto) || !same_shape(out[i], qp.out_proto) || !in[i].ptr || !out[i].ptr)
+            return fail(err, GF_ERR_BAD_PARAMS, name + "buffer size, stride or kind differs from the prototype's");
+        if (out[i].len < (size_t)out[i].height * (size_t)out[i].stride)
+            return fail(err, GF_ERR_BAD_PARAMS, name + "the output buffer holds fewer than height rows of stride bytes");
+        if (q->host_frames && (in[i].len > qp.in_proto.len || out[i].len > qp.out_proto.len))
+            return fail(err, GF_ERR_BUFFER_TOO_SMALL, name + "HOST buffer longer than the prototype's (the staging size)");
+    }
+    CK(err, cudaSetDevice(q->cfg.device));
+    QSlot& s = q->slots[(size_t)q->next];
+    if (s.busy) return fail(err, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
+    const cudaStream_t st = s.stream.get();
+    nvtxRangePushA("gf_queue_submit_planes");
+    struct PopRange { ~PopRange() { nvtxRangePop(); } } pop_range;
+    // one table + verdict for every plane: each plane's Stabilization is sized with the frame (rendering/mod.rs:514)
+    gf_kernel_params kp0; size_t rows = 0; double fov = 1.0, minimal_fov = 1.0;
+    int rc = gf_cuda_frame_transform_dev_flagged(q->gyro.get(), &q->cp, timestamp_ms, frame, &kp0, s.d_mat.ptr, q->max_rows, s.d_flags.ptr,
+                                                 &rows, &fov, &minimal_fov, (void*)st);
+    if (rc != GF_OK) return fail(err, rc, "gf_cuda_frame_transform_dev_flagged failed");
+    q->launches++;
+    const float* mesh_dev = nullptr;
+    if (mesh && mesh_len) {
+        memcpy(s.h_mesh.ptr, mesh, mesh_len * sizeof(float));
+        CK(err, cudaMemcpyAsync(s.d_mesh.ptr, s.h_mesh.ptr, mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
+        mesh_dev = s.d_mesh.ptr;
+    }
+    // the per-buffer half, per plane, as rendering/mod.rs:531-541 completes it before process_pixels
+    gf_kernel_params kp[4];
+    gf_buffer_desc din[4], dout[4];
+    for (size_t i = 0; i < n_planes; ++i) {
+        const QPlane& qp = q->planes[i];
+        kp[i] = kp0;
+        rc = gf_get_frame_transform_at(&qp.stab, &q->cp, &in[i], &out[i], mesh, mesh_len, timestamp_ms, frame, minimal_fov, &kp[i]);
+        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(i) + ": gf_get_frame_transform_at failed");
+        kp[i].pixel_value_limit = kp[i].max_pixel_value = qp.spec.max_value;
+        kp[i].plane_index = (int32_t)i;
+        if (fill_with_background) kp[i].flags |= GF_FLAG_FILL_WITH_BACKGROUND;
+        din[i] = in[i]; dout[i] = out[i];
+        if (q->host_frames) {                  // the output too: pixels the warp leaves alone keep their content, like on the CPU path
+            CK(err, cudaMemcpyAsync(s.plane_in[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
+            CK(err, cudaMemcpyAsync(s.plane_out[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));
+            din[i].kind = dout[i].kind = GF_BUF_DEVICE;
+            din[i].ptr = s.plane_in[i].ptr; dout[i].ptr = s.plane_out[i].ptr;
+        }
+    }
+    // each group through the planes path: its planner fuses the planes whose KernelParams agree, the rest get a warp each
+    for (size_t g = 0; g < q->groups.size(); ++g) {
+        const std::vector<size_t>& grp = q->groups[g];
+        gf_buffer_desc gi[4], go[4]; gf_kernel_params gp[4];
+        for (size_t j = 0; j < grp.size(); ++j) { gi[j] = din[grp[j]]; go[j] = dout[grp[j]]; gp[j] = kp[grp[j]]; }
+        gf_cuda_ctx* const ctx = s.group_ctx[g].get();
+        const unsigned long long l0 = gf_cuda_launch_count(ctx);
+        rc = gf_cuda_undistort_planes_dev_flagged(ctx, grp.size(), gi, go, gp, s.d_mat.ptr, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags.ptr, (void*)st);
+        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(grp[0]) + ": " + gf_cuda_last_error(ctx));
+        q->launches += gf_cuda_launch_count(ctx) - l0;
+    }
+    if (q->cfg.checksum) {
+        gf_checksum_plane d[4];
+        for (size_t i = 0; i < n_planes; ++i) d[i] = { dout[i].ptr, (size_t)dout[i].stride, (size_t)dout[i].stride, (size_t)dout[i].height };
+        if ((rc = enqueue_checksum_rows(d, n_planes, s.d_sum.ptr, st, err)) != GF_OK) return rc;
+        q->launches++;
+        CK(err, cudaMemcpyAsync(s.h_sum.ptr, s.d_sum.ptr, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    }
+    if (q->host_frames)
+        for (size_t i = 0; i < n_planes; ++i) CK(err, cudaMemcpyAsync(out[i].ptr, s.plane_out[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
+    CK(err, cudaEventRecord(s.done.get(), st));
+    s.busy = true; s.frame = frame;
+    q->fifo.push_back(q->next);
+    q->next = (q->next + 1) % (int)q->slots.size();
+    return GF_OK;
+}
+
+GF_API int gf_cuda_checksum_planes_dev(const gf_checksum_plane* planes, size_t n, uint64_t* out_dev, void* cu_stream) {
+    return enqueue_checksum_rows(planes, n, out_dev, (cudaStream_t)cu_stream, nullptr);
 }
 
 GF_API int gf_cuda_queue_wait(gf_cuda_queue* q, size_t* out_frame, uint64_t* out_checksum) {

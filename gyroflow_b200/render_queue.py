@@ -8,6 +8,8 @@ tests.  The reference has no counterpart: its render queue runs whole jobs in pa
 but each job is a sequential decode -> warp -> encode loop on one device (rendering/mod.rs:451).
 """
 import ctypes as C
+from dataclasses import dataclass
+from typing import Tuple
 
 import numpy as np
 
@@ -23,7 +25,7 @@ class RenderQueue:
     (shard_frames) and the per-frame checksums are gathered in frame order (gather_results)."""
 
     def __init__(self, compute_params, stab: abi.StabConfig, distortion_model: str, digital_lens, in_proto, out_proto,
-                 device=0, depth=4, pin_numa=True, checksum=False):
+                 device=0, depth=4, pin_numa=True, checksum=False, planes=None):
         self._lib = abi.load_library()
         self.cp = compute_params                      # keeps the arrays alive
         cfg = abi.QueueConfig()
@@ -34,24 +36,52 @@ class RenderQueue:
         cfg.stab = stab
         self.depth = depth
         self.in_flight = 0
+        self.n_planes = 0 if planes is None else len(planes)
         h = C.c_void_p()
-        i, o = in_proto.to_c(), out_proto.to_c()
-        rc = self._lib.gf_cuda_queue_create(C.byref(h), C.byref(cfg), C.byref(compute_params.c), C.byref(i), C.byref(o))
+        if planes is None:
+            i, o = in_proto.to_c(), out_proto.to_c()
+            rc = self._lib.gf_cuda_queue_create(C.byref(h), C.byref(cfg), C.byref(compute_params.c), C.byref(i), C.byref(o))
+            what = "gf_cuda_queue_create"
+        else:
+            n = len(planes)
+            specs = (abi.QueuePlane * n)(*planes)
+            ins = (abi.BufferDesc * n)(*[b.to_c() for b in in_proto])
+            outs = (abi.BufferDesc * n)(*[b.to_c() for b in out_proto])
+            rc = self._lib.gf_cuda_queue_create_planes(C.byref(h), C.byref(cfg), C.byref(compute_params.c), n, specs, ins, outs)
+            what = "gf_cuda_queue_create_planes"
         if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_queue_create: " + (self._lib.gf_cuda_last_error(None) or b"").decode())
+            raise GyroflowCoreError(rc, what + ": " + (self._lib.gf_cuda_last_error(None) or b"").decode())
         self._h = h
+
+    @classmethod
+    def for_planes(cls, compute_params, stab: abi.StabConfig, distortion_model: str, digital_lens, planes, in_protos, out_protos, **kw):
+        """A queue for decoder frames of 1-4 planes (gf_cuda_queue_create_planes): `planes` are abi.QueuePlane (PlaneLayout.to_c of
+        layout()), `in_protos` / `out_protos` one BufferDescription per plane.  submit() then takes a list of Buffers per frame."""
+        return cls(compute_params, stab, distortion_model, digital_lens, in_protos, out_protos, planes=planes, **kw)
 
     def _err(self, rc, what):
         return GyroflowCoreError(rc, what + ": " + (self._lib.gf_cuda_queue_last_error(self._h) or b"").decode())
 
-    def submit(self, frame: int, timestamp_ms: float, buffers, mesh=None):
-        """Enqueue one frame.  The queue must have a free slot (in_flight < depth): call wait() first otherwise."""
-        i, o = buffers.input.to_c(), buffers.output.to_c()
+    def submit(self, frame: int, timestamp_ms: float, buffers, mesh=None, fill_with_background=False):
+        """Enqueue one frame (a planes queue: a list of Buffers, one per plane).  The queue must have a free slot (in_flight < depth):
+        call wait() first otherwise.  fill_with_background: the render loop's per-frame flag, planes queues only (a one-plane queue
+        takes FILL_WITH_BACKGROUND through StabConfig.base_flags)."""
         m = None if mesh is None else np.ascontiguousarray(mesh, dtype=np.float32)
-        rc = self._lib.gf_cuda_queue_submit(self._h, frame, timestamp_ms, C.byref(i), C.byref(o),
-                                            m.ctypes.data if m is not None and m.size else None, m.size if m is not None else 0)
+        mp, mn = (m.ctypes.data if m is not None and m.size else None), (m.size if m is not None else 0)
+        if self.n_planes:
+            n = len(buffers)
+            ins = (abi.BufferDesc * n)(*[b.input.to_c() for b in buffers])
+            outs = (abi.BufferDesc * n)(*[b.output.to_c() for b in buffers])
+            rc = self._lib.gf_cuda_queue_submit_planes(self._h, frame, timestamp_ms, n, ins, outs, mp, mn, int(fill_with_background))
+            what = "gf_cuda_queue_submit_planes"
+        else:
+            if fill_with_background:
+                raise ValueError("a one-plane queue takes FILL_WITH_BACKGROUND through StabConfig.base_flags")
+            i, o = buffers.input.to_c(), buffers.output.to_c()
+            rc = self._lib.gf_cuda_queue_submit(self._h, frame, timestamp_ms, C.byref(i), C.byref(o), mp, mn)
+            what = "gf_cuda_queue_submit"
         if rc != 0:
-            raise self._err(rc, "gf_cuda_queue_submit")
+            raise self._err(rc, what)
         self.in_flight += 1
 
     def wait(self):
@@ -63,13 +93,14 @@ class RenderQueue:
         self.in_flight -= 1
         return int(f.value), int(s.value)
 
-    def render(self, frames, timestamp_of, buffers_of, mesh_of=None):
-        """Run `frames` (an iterable of frame indices) through the queue keeping it full; returns {frame: checksum} in frame order."""
+    def render(self, frames, timestamp_of, buffers_of, mesh_of=None, fill_with_background=False):
+        """Run `frames` (an iterable of frame indices) through the queue keeping it full; returns {frame: checksum} in frame order.
+        buffers_of(f): the frame's Buffers, or for a planes queue its list of per-plane Buffers."""
         out = {}
         for f in frames:
             if self.in_flight == self.depth:
                 k, v = self.wait(); out[k] = v
-            self.submit(f, timestamp_of(f), buffers_of(f), mesh_of(f) if mesh_of else None)
+            self.submit(f, timestamp_of(f), buffers_of(f), mesh_of(f) if mesh_of else None, fill_with_background)
         while self.in_flight:
             k, v = self.wait(); out[k] = v
         return dict(sorted(out.items()))
@@ -100,6 +131,80 @@ def checksum_host(buf: np.ndarray) -> int:
     k = np.arange(w.size, dtype=np.uint64) * np.uint64(2) + np.uint64(1)
     with np.errstate(over="ignore"):
         return int((w * k).sum(dtype=np.uint64))
+
+
+def plane_rows(buf: np.ndarray, row_bytes: int, stride: int, rows: int) -> np.ndarray:
+    """The bytes a gf_checksum_plane descriptor names: `rows` rows of `row_bytes` bytes, `stride` bytes apart, concatenated."""
+    b = np.ascontiguousarray(buf).view(np.uint8).reshape(-1)
+    if rows == 0 or row_bytes == 0:
+        return np.zeros(0, np.uint8)
+    idx = np.arange(rows, dtype=np.int64)[:, None] * stride + np.arange(row_bytes, dtype=np.int64)[None, :]
+    return b[idx.reshape(-1)]
+
+
+def checksum_planes_host(descs) -> int:
+    """The multi-plane checksum (gf_cuda_checksum_planes_dev, a planes queue's frame checksum) on the host: descs = [(buffer,
+    row_bytes, stride, rows)]; checksum_host of their rows concatenated in order.  One (buf, stride, stride, rows) descriptor is
+    checksum_host of the buffer's first rows * stride bytes."""
+    parts = [plane_rows(b, rb, st, r) for b, rb, st, r in descs]
+    return checksum_host(np.concatenate(parts) if parts else np.zeros(0, np.uint8))
+
+
+# ---- decoder formats -> plane layouts: create_planes_proc! in the reference's rendering/mod.rs:563-651 -------------------------------
+@dataclass(frozen=True)
+class PlaneLayout:
+    """One plane of a decoder format: its pixel type, size fraction of the frame (ceil(W / w_div) x ceil(H / h_div)), the value the
+    render loop writes to pixel_value_limit / max_pixel_value, and the component list (`$yuvi`) from_rgb_color converts the background
+    with — that conversion stays with the caller."""
+    pixel_type: str
+    w_div: int
+    h_div: int
+    max_value: float
+    components: Tuple[int, ...]
+
+    def size(self, width, height):
+        return (-(-width // self.w_div), -(-height // self.h_div))
+
+    def to_c(self, background=(0.0, 0.0, 0.0, 0.0)) -> abi.QueuePlane:
+        p = abi.QueuePlane()
+        p.pixel_type, p.w_div, p.h_div, p.max_value = abi.PIXEL_TYPES[self.pixel_type][0], self.w_div, self.h_div, self.max_value
+        p.background[:] = [float(v) for v in background]
+        return p
+
+
+def _yuv(luma, chroma, w_div, h_div, max_value, uv_components=None, alpha=False):
+    if chroma.startswith("UV"):
+        return (PlaneLayout(luma, 1, 1, max_value, (0,)), PlaneLayout(chroma, w_div, h_div, max_value, uv_components))
+    planes = [PlaneLayout(luma, 1, 1, max_value, (0,))] + [PlaneLayout(chroma, w_div, h_div, max_value, (c,)) for c in (1, 2)]
+    return tuple(planes + ([PlaneLayout(luma, 1, 1, max_value, (3,))] if alpha else []))
+
+
+DECODER_FORMATS = {
+    "nv12": _yuv("Luma8", "UV8", 2, 2, 255.0, (1, 2)),
+    "nv21": _yuv("Luma8", "UV8", 2, 2, 255.0, (2, 1)),
+    "yuv420p": _yuv("Luma8", "Luma8", 2, 2, 255.0),
+    "yuvj420p": _yuv("Luma8", "Luma8", 2, 2, 255.0),
+    # the reference keeps 65535 for the 10-bit P0xx formats too (their samples sit in the high bits)
+    **{"p%s%s" % (s, b): _yuv("Luma16", "UV16", wd, hd, 65535.0, (1, 2))
+       for s, (wd, hd) in (("0", (2, 2)), ("2", (2, 1)), ("4", (1, 1))) for b in ("10", "16")},
+    **{"yuv4%sp%s" % (s, b): _yuv("Luma16", "Luma16", wd, hd, float((1 << int(b)) - 1))
+       for s, (wd, hd) in (("20", (2, 2)), ("22", (2, 1)), ("44", (1, 1))) for b in ("10", "12", "14", "16")},
+    **{"yuva444p%s" % b: _yuv("Luma16", "Luma16", 1, 1, float((1 << int(b)) - 1), alpha=True) for b in ("10", "12", "16")},
+    # planes G, B, R(, A) in ffmpeg's order; from_rgb_color takes background components 2, 0, 1(, 3) for them
+    "gbrapf32": tuple(PlaneLayout("R32f", 1, 1, 255.0, (c,)) for c in (2, 0, 1, 3)),
+    "gbrpf32": tuple(PlaneLayout("R32f", 1, 1, 255.0, (c,)) for c in (2, 0, 1)),
+}
+
+
+def layout(fmt: str, width: int, height: int):
+    """The planes of a decoder frame of format `fmt` (ffmpeg's name, case-insensitive, "le" suffix optional) and size width x height:
+    a list of (PlaneLayout, (plane width, plane height)) in plane order."""
+    key = fmt.lower()
+    if key not in DECODER_FORMATS and key.endswith("le"):
+        key = key[:-2]
+    if key not in DECODER_FORMATS:
+        raise KeyError("no plane layout for decoder format %r" % fmt)
+    return [(pl, pl.size(width, height)) for pl in DECODER_FORMATS[key]]
 
 
 def shard_frames(n_frames, world, rank):

@@ -207,7 +207,7 @@ GF_API int         gf_cuda_supports(const gf_buffer_desc* in, const gf_buffer_de
 GF_API const char* gf_cuda_version(void);
 /* sizeof() of the structs that cross this ABI, for binding generators and their tests: 0 gf_kernel_params, 1 gf_buffer_desc,
  * 2 gf_compute_params, 3 gf_camera_stab, 4 gf_keyframe_track, 5 gf_stab_config, 6 gf_queue_config, 7 gf_lens_data, 8 gf_mesh_f64,
- * 9 gf_zoom_params; 0 for any other index. */
+ * 9 gf_zoom_params, 11 gf_queue_plane, 12 gf_checksum_plane; 0 for any other index (10 is unassigned). */
 GF_API size_t gf_abi_struct_size(int which);
 
 /* ---- lens plugin surface: DistortionModel::from_name / id  distortion_models/mod.rs:79-90 -- */
@@ -582,6 +582,8 @@ GF_API int gf_get_frame_transform_at(const gf_stab_config* stab, const gf_comput
  * gf_cuda_queue_wait first; gf_cuda_queue_wait blocks until the OLDEST frame is done and returns frames in submission order.  HOST buffers must be page-locked and stay valid until the
  * frame has been waited for.  `cp` is copied shallowly: the arrays it points to (tracks are uploaded at creation; fovs, offsets, focal lengths,
  * camera_stab, keyframe tracks, lens_per_frame are read per frame on the host) must stay valid until gf_cuda_queue_destroy.  The optional checksum is sum(word[i] * (2 i + 1)) mod 2^64 over the output buffer's 32-bit words.
+ * Decoder frames of 1-4 planes (NV12, P010, planar YUV, GBRAPF32, ...) take gf_cuda_queue_create_planes / gf_cuda_queue_submit_planes
+ * below: still one producer launch and one slot per frame, the planes' warps and one checksum over all of them on the slot's stream.
  * ---------------------------------------------------------------------------------------- */
 typedef struct gf_cuda_queue gf_cuda_queue;
 typedef struct gf_queue_config {
@@ -601,6 +603,51 @@ GF_API int      gf_cuda_queue_drain(gf_cuda_queue* q);                          
 GF_API uint64_t gf_cuda_queue_launches(gf_cuda_queue* q);                                          /* warp + producer (+ checksum) kernels launched */
 GF_API void     gf_cuda_queue_destroy(gf_cuda_queue* q);
 GF_API const char* gf_cuda_queue_last_error(gf_cuda_queue* q);
+
+/* ---- Multi-plane frames through the queue: what create_planes_proc! (rendering/mod.rs:483-548) builds per decoded frame ----------
+ * The reference renders a decoder frame (NV12, P010, YUV4xxP, GBRAPF32, ...) as 1-4 planes, each with its own Stabilization sized with
+ * the ORIGINAL frame size (:514) and the same ComputeParams, so at_timestamp yields one matrix table per frame for every plane; only the
+ * per-buffer half of KernelParams differs (sizes, strides, source / output rects, pixel limits, plane_index, background).  A planes queue
+ * therefore runs, per frame, on the slot's stream and without a host synchronisation:
+ *     ONE producer launch (table + verdict, sized from the frame)  ->  [H2D of every plane]  ->  the warp of every plane group
+ *     ->  [ONE checksum launch over all planes]  ->  [D2H of every plane]
+ * Planes of the same pixel type and size fraction form a group; each group goes through gf_cuda_undistort_planes_dev_flagged, whose
+ * planner renders planes with equal KernelParams (all but plane_index and background: U and V of planar YUV, the R32f planes of
+ * GBRAPF32) as one coordinate pass plus one sampling pass per plane, and any other plane as a warp of its own.  Planes of different
+ * geometry (Y and UV) never share coordinates.  Each plane's KernelParams are gf_get_frame_transform_at of its buffers with the
+ * queue's gf_stab_config (pixel_type and background replaced by the plane's), then pixel_value_limit = max_pixel_value = max_value,
+ * plane_index = i and, with fill_with_background, GF_FLAG_FILL_WITH_BACKGROUND (rendering/mod.rs:531-541).
+ * Colour decisions stay with the caller: `background` is already in the plane's components (PixelType::from_rgb_color with the
+ * plane's YUV index list and the range of the output), FIX_COLOR_RANGE goes in gf_stab_config.base_flags. */
+typedef struct gf_queue_plane {
+    int32_t pixel_type;                       /* GF_PIX_* */
+    int32_t w_div, h_div;                     /* plane size = ceil(W / w_div) x ceil(H / h_div) of the frame; 1 or 2 */
+    float   max_value;                        /* written to pixel_value_limit and max_pixel_value (255, 1023, 4095, 16383, 65535) */
+    float   background[4];                    /* in this plane's components, 0..1 like gf_stab_config.background */
+} gf_queue_plane;
+/* n_planes 1..4; in_protos / out_protos: n_planes buffer descriptions whose sizes, strides and kind every frame must repeat.  HOST
+ * frames are staged through per-slot device copies of every plane (sized from the prototypes).  Fails with GF_ERR_BAD_PARAMS before
+ * any CUDA call, naming the plane in gf_cuda_last_error(NULL), for: n_planes outside 1..4, w_div / h_div not 1 or 2, a UV8 / UV16 plane
+ * whose buffer width is not ceil(W / w_div) (output: ceil(output W / w_div)), HOST and DEVICE prototypes mixed, an output prototype
+ * whose buffer holds fewer than height rows of stride bytes, and a (pixel type, lens, digital lens, interpolation) that
+ * gf_combo_supported rejects.  gf_cuda_queue_submit on such a queue fails; gf_cuda_queue_wait / drain / launches are shared. */
+GF_API int      gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_config* cfg, const gf_compute_params* cp, size_t n_planes,
+                                            const gf_queue_plane* planes, const gf_buffer_desc* in_protos, const gf_buffer_desc* out_protos);
+/* One frame of a planes queue: in / out are arrays of n_planes (the queue's count) with the prototypes' sizes, strides and kind, all
+ * HOST or all DEVICE.  A mismatch is GF_ERR_BAD_PARAMS before anything is enqueued, with the plane named in gf_cuda_queue_last_error.
+ * A slot holds one frame; gf_cuda_queue_wait returns its frame checksum (below) when cfg.checksum is set. */
+GF_API int      gf_cuda_queue_submit_planes(gf_cuda_queue* q, size_t frame, double timestamp_ms, size_t n_planes, const gf_buffer_desc* in,
+                                            const gf_buffer_desc* out, const float* mesh, size_t mesh_len, int fill_with_background);
+
+/* Multi-plane checksum.  A descriptor names `rows` rows of `row_bytes` bytes, row r starting at ptr + r * stride (no alignment asked of
+ * ptr, stride or row_bytes).  The summed byte string is every descriptor's rows, in order, concatenated; it is read as little-endian
+ * 32-bit words word[i] (a final group of fewer than 4 bytes is left out) and the checksum is sum(word[i] * (2 i + 1)) mod 2^64, i running
+ * over the whole string.  One descriptor {ptr, stride, stride, rows} is gf_cuda_checksum_dev(ptr, rows * stride).  A planes queue sums
+ * {out[i].ptr, stride, stride, height} of every output plane (padding bytes included, as the one-plane checksum does), so a one-plane
+ * layout gives the checksum of a gf_cuda_queue_create queue on the same buffer.  One kernel launch for all descriptors (n 1..4),
+ * accumulated into *out_dev (zeroed first) on `cu_stream`. */
+typedef struct gf_checksum_plane { const void* ptr; size_t row_bytes, stride, rows; } gf_checksum_plane;
+GF_API int      gf_cuda_checksum_planes_dev(const gf_checksum_plane* planes, size_t n, uint64_t* out_dev, void* cu_stream);
 
 /* Bind the calling thread to the CPUs of the NUMA node the GPU hangs off (/sys/bus/pci/devices/<bdf>/local_cpulist), so that
  * page-locked staging allocated afterwards — by this library or by the caller — is node-local and the copy threads do not cross
