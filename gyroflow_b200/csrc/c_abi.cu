@@ -74,8 +74,7 @@ struct gf_cuda_ctx {
     int overlays = 0;
     GrowBuf<uint8_t, true> h_drawing;
     GrowBuf<uint8_t> d_drawing, src_ovl;
-    // HOST multi-plane frames (gf_cuda_undistort_planes): one device staging pair per plane
-    std::vector<GrowBuf<uint8_t>> plane_src, plane_dst;
+    PlaneStaging plane_staging;          // HOST multi-plane frames (gf_cuda_undistort_planes)
     GrowBuf<uint2> coords;               // two-pass path: the frame's coordinate map(s)
     Stream stream;
     size_t max_rows = 0;
@@ -299,7 +298,6 @@ struct FrameJob {
     size_t more_planes = 0;                        // planes after the first that share its geometry (checked by the caller)
     bool coord_only = false;                       // ST maps: the coordinate pass only, into ctx->coords
     const uint32_t* table_flags_dev = nullptr;     // device tables' verdict word (nullptr: not validated, guarded path)
-    uint64_t* checksum_dev = nullptr;              // render queue: accumulate the output's checksum here
     const uint8_t* drawing = nullptr; size_t drawing_len = 0;   // preview overlays (after gf_cuda_set_overlays)
     bool overlays(const gf_cuda_ctx* ctx) const { return ctx->overlays && more_planes == 0 && !coord_only; }
 };
@@ -412,12 +410,7 @@ struct FrameRun {
             CK(err, e_h2d);
             A.src = ctx->src_stage.ptr;
         }
-        // Does the kernel write every pixel of [0,w) x [0,h)?  (output_rect == whole buffer == output size: the bounds test of
-        // cpu_undistort.rs:551 then passes everywhere.)  If so only those bytes travel back; otherwise the untouched pixels
-        // must keep their previous content, like on the CPU path, so the buffer is uploaded first.
-        full_cover = p->output_rect[0] == 0 && p->output_rect[1] == 0 && p->output_rect[2] == out->width && p->output_rect[3] == out->height &&
-                     out->width == p->output_width && out->height == p->output_height && (p->flags & 4) == 0 &&
-                     (size_t)out->height * (size_t)p->output_stride <= out->len + (size_t)(p->output_stride - out->width * ctx->combo.bpp());
+        full_cover = warp_covers_output(*p, *out, ctx->combo.bpp());
         if (out->kind == GF_BUF_HOST) {
             if (!full_cover) CK(err, cudaMemcpyAsync(ctx->dst_stage.ptr, out->ptr, out->len, cudaMemcpyHostToDevice, st));
             A.dst = ctx->dst_stage.ptr;
@@ -486,7 +479,7 @@ struct FrameRun {
         return GF_OK;
     }
 
-    // Pass 2 (one sampling launch per plane), output-stage overlays, checksum, copy back, synchronisation.
+    // Pass 2 (one sampling launch per plane), output-stage overlays, copy back, synchronisation.
     int finish() {
         if (plan.two_pass && !job.coord_only) {
             for (size_t i = 0; i <= job.more_planes; ++i) {
@@ -506,9 +499,6 @@ struct FrameRun {
             if (gf_internal_draw_overlays((void*)st, A.dst, out->len, out->width, out->height, p->output_stride, p, L.channels, L.scalar, 0,
                                           drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (output stage) failed");
         }
-        // render queue: per-frame output checksum, before the result leaves the device
-        if (job.checksum_dev && gf_cuda_checksum_dev(A.dst, std::min<size_t>(out->len, (size_t)out->height * (size_t)p->output_stride), job.checksum_dev, (void*)st) != GF_OK)
-            return fail(err, GF_ERR_CUDA, "checksum kernel failed");
         if (out->kind == GF_BUF_HOST) {                                                                              // opencl.rs:413
             nvtxRangePushA("gf_d2h_frame");
             cudaError_t e_d2h;
@@ -576,12 +566,64 @@ int run_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, cons
 
 } // namespace
 
-int gf_internal_run_frame(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out, const gf_kernel_params* params,
-                          const float* matrices_dev, size_t matrix_rows, const float* mesh_dev, size_t mesh_len,
-                          const uint32_t* table_flags_dev, void* cu_stream, uint64_t* checksum_dev) {
-    FrameJob job{in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
-    job.tables_on_device = true; job.sync_host = false; job.table_flags_dev = table_flags_dev; job.checksum_dev = checksum_dev;
-    return run_warp(ctx, job);
+bool gf::warp_covers_output(const gf_kernel_params& p, const gf_buffer_desc& out, int bpp) {
+    return p.output_rect[0] == 0 && p.output_rect[1] == 0 && p.output_rect[2] == out.width && p.output_rect[3] == out.height &&
+           out.width == p.output_width && out.height == p.output_height && (p.flags & GF_FLAG_FILL_WITH_BACKGROUND) == 0 &&
+           (size_t)out.height * (size_t)p.output_stride <= out.len + (size_t)(p.output_stride - out.width * bpp);
+}
+
+cudaError_t PlaneStaging::reserve(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, cudaStream_t st) {
+    if (in_.size() < n) { in_.resize(n); out_.resize(n); }
+    for (size_t i = 0; i < n; ++i) {
+        cudaError_t e = in[i].kind == GF_BUF_HOST ? in_[i].reserve(in[i].len, st) : cudaSuccess;
+        if (e == cudaSuccess && out[i].kind == GF_BUF_HOST) e = out_[i].reserve(out[i].len, st);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+int PlaneStaging::check(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, std::string* err) const {
+    for (size_t i = 0; i < n; ++i) {
+        for (const gf_buffer_desc* b : {&in[i], &out[i]})
+            if ((b->kind != GF_BUF_HOST && b->kind != GF_BUF_DEVICE) || !b->ptr)
+                return fail(err, GF_ERR_BAD_PARAMS, "plane " + std::to_string(i) + ": unsupported buffer source");
+        const size_t cap_in = i < in_.size() ? in_[i].len : 0, cap_out = i < out_.size() ? out_[i].len : 0;
+        if ((in[i].kind == GF_BUF_HOST && in[i].len > cap_in) || (out[i].kind == GF_BUF_HOST && out[i].len > cap_out))
+            return fail(err, GF_ERR_BUFFER_TOO_SMALL, "plane " + std::to_string(i) + ": HOST buffer longer than its staging");
+    }
+    return GF_OK;
+}
+
+int PlaneStaging::upload(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, const gf_kernel_params* p, bool checksum, cudaStream_t st,
+                         std::string* err, gf_buffer_desc* din, gf_buffer_desc* dout) {
+    for (size_t i = 0; i < n; ++i) {
+        din[i] = in[i]; dout[i] = out[i];
+        if (in[i].kind == GF_BUF_HOST) {
+            CK(err, cudaMemcpyAsync(in_[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
+            din[i].kind = GF_BUF_DEVICE; din[i].ptr = in_[i].ptr;
+        }
+        if (out[i].kind == GF_BUF_HOST) {
+            const int bpp = p[i].bytes_per_pixel;
+            const bool padded = (size_t)p[i].output_stride != (size_t)out[i].width * (size_t)bpp;
+            if (!warp_covers_output(p[i], out[i], bpp) || (checksum && padded))
+                CK(err, cudaMemcpyAsync(out_[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));
+            dout[i].kind = GF_BUF_DEVICE; dout[i].ptr = out_[i].ptr;
+        }
+    }
+    return GF_OK;
+}
+
+int PlaneStaging::download(size_t n, const gf_buffer_desc* out, const gf_kernel_params* p, cudaStream_t st, std::string* err) const {
+    for (size_t i = 0; i < n; ++i) {
+        if (out[i].kind != GF_BUF_HOST) continue;
+        const size_t stride = (size_t)p[i].output_stride;
+        if (warp_covers_output(p[i], out[i], p[i].bytes_per_pixel))
+            CK(err, cudaMemcpy2DAsync(out[i].ptr, stride, out_[i].ptr, stride, (size_t)out[i].width * (size_t)p[i].bytes_per_pixel, (size_t)out[i].height,
+                                      cudaMemcpyDeviceToHost, st));
+        else
+            CK(err, cudaMemcpyAsync(out[i].ptr, out_[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
+    }
+    return GF_OK;
 }
 
 // Packed-kernel launches use programmatic stream serialization: the grid may be scheduled while the previous kernel on the stream
@@ -924,21 +966,15 @@ GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_
     }
     CK(err, cudaSetDevice(ctx->device));
     cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
-    { int rc = order_after_last_call(ctx, st); if (rc != GF_OK) return rc; }   // the staging copies below reuse the context's buffers
-    if (ctx->plane_src.size() < n_planes) { ctx->plane_src.resize(n_planes); ctx->plane_dst.resize(n_planes); }
-    std::vector<gf_buffer_desc> din(in, in + n_planes), dout(out, out + n_planes);
-    for (size_t i = 0; i < n_planes; ++i) {
-        CK(err, ctx->plane_src[i].reserve(in[i].len, st));
-        CK(err, ctx->plane_dst[i].reserve(out[i].len, st));
-        CK(err, cudaMemcpyAsync(ctx->plane_src[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
-        CK(err, cudaMemcpyAsync(ctx->plane_dst[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));   // untouched pixels keep their content, like on the CPU path
-        din[i].kind = GF_BUF_DEVICE; din[i].ptr = ctx->plane_src[i].ptr;
-        dout[i].kind = GF_BUF_DEVICE; dout[i].ptr = ctx->plane_dst[i].ptr;
-    }
+    int rc = order_after_last_call(ctx, st);             // the staging copies below reuse the context's buffers
+    if (rc != GF_OK) return rc;
+    CK(err, ctx->plane_staging.reserve(n_planes, in, out, st));
+    std::vector<gf_buffer_desc> din(n_planes), dout(n_planes);
+    if ((rc = ctx->plane_staging.upload(n_planes, in, out, params, false, st, err, din.data(), dout.data())) != GF_OK) return rc;
     FrameJob job{din.data(), dout.data(), params, matrices, matrix_rows, mesh, mesh_len, (void*)st};
     job.sync_host = false;
-    { int rc = run_planes(ctx, n_planes, din.data(), dout.data(), params, job); if (rc != GF_OK) return rc; }
-    for (size_t i = 0; i < n_planes; ++i) CK(err, cudaMemcpyAsync(out[i].ptr, ctx->plane_dst[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
+    if ((rc = run_planes(ctx, n_planes, din.data(), dout.data(), params, job)) != GF_OK) return rc;
+    if ((rc = ctx->plane_staging.download(n_planes, out, params, st, err)) != GF_OK) return rc;
     CK(err, cudaStreamSynchronize(st));
     return GF_OK;
 }

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <memory>
 #include <string>
+#include <vector>
 #include "../../include/gyroflow_cuda.h"
 #include "frame_geometry.cuh"
 
@@ -136,6 +137,26 @@ private:
     int sm_count = 1;
 };
 
+// ---- HOST image buffers (c_abi.cu) ----
+// The warp of `p` writes every pixel of `out` (output_rect = buffer = output size, no fill-with-background: the bounds test of
+// cpu_undistort.rs:551 passes everywhere), and the buffer lacks at most the last row's padding.  Otherwise the pixels the warp leaves
+// alone keep their previous content, like on the CPU path, so a staged output is uploaded first.
+bool warp_covers_output(const gf_kernel_params& p, const gf_buffer_desc& out, int bpp);
+// Device copies of a frame's HOST planes (render-queue slots, gf_cuda_undistort_planes); a DEVICE buffer is used in place.
+class PlaneStaging {
+public:
+    cudaError_t reserve(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, cudaStream_t st);   // growing waits for `st`
+    // GF_ERR_BAD_PARAMS for a buffer of neither kind or without a pointer, GF_ERR_BUFFER_TOO_SMALL for a HOST one beyond the capacity
+    int check(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, std::string* err) const;
+    // din / dout: what the warp of p[i] reads and writes.  The output is uploaded unless the warp writes every byte of it that is read
+    // afterwards (covered, and no stride padding when `checksum` reads the device rows); a covered one comes back as its pixel rows.
+    int upload(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, const gf_kernel_params* p, bool checksum, cudaStream_t st,
+               std::string* err, gf_buffer_desc* din, gf_buffer_desc* dout);
+    int download(size_t n, const gf_buffer_desc* out, const gf_kernel_params* p, cudaStream_t st, std::string* err) const;
+private:
+    std::vector<GrowBuf<uint8_t>> in_, out_;
+};
+
 // What generate_stmaps does to the user's ComputeParams before either map (stmap.rs:24-35, :44-46): rotation suppressed, fovs cleared,
 // no readout time unless per_frame, fov_scale 1 and the output size the frame size.
 inline gf_compute_params stmap_params(const gf_compute_params& user, int per_frame) {
@@ -149,13 +170,6 @@ inline gf_compute_params stmap_params(const gf_compute_params& user, int per_fra
 inline bool stmap_size_ok(int w, int h) { return w >= 4 && h >= 4 && w <= 32768 && h <= 32768; }
 
 } // namespace gf
-
-// One frame through the warp with a DEVICE matrix table + verdict word, never synchronising: HOST image buffers (page-locked) are
-// copied on `cu_stream` before / after the kernel.  `checksum_dev` (nullable): the output buffer's checksum is accumulated into it
-// on the same stream, between the kernel and the device-to-host copy.  Used by the render queue.
-int gf_internal_run_frame(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out, const gf_kernel_params* params,
-                          const float* matrices_dev, size_t matrix_rows, const float* mesh_dev, size_t mesh_len,
-                          const uint32_t* table_flags_dev, void* cu_stream, uint64_t* checksum_dev);
 
 // Preview overlays (overlay.cu): draw_pixel + draw_safe_area of opencl_undistort.cl:109-154 as a pass over a DEVICE buffer.
 // count / scalar: channels and scalar kind (0 u8, 1 u16, 2 f32, 3 f16) of the pixel type.

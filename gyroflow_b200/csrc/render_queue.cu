@@ -6,16 +6,16 @@
 // independent units (at_timestamp depends on immutable ComputeParams + the timestamp, frame_transform.rs:165), so this queue keeps
 // `depth` of them in flight on one GPU and lets a box shard `i -> GPU (i mod G)` across processes with no data-path collective.
 //
-// One slot = one stream + one warp context (its own device staging when the buffers are HOST) + a device matrix table with its
-// trust verdict word.  Per submitted frame, all enqueued on the slot's stream, nothing synchronous:
-//     producer kernel (gf_cuda_frame_transform_dev_flagged: table + verdict)  ->  [mesh H2D]  ->  [frame H2D]  ->  warp kernel
-//     ->  [checksum kernel]  ->  [frame D2H]  ->  event
+// Every queue renders frames of a plane layout: 1-4 planes (a decoder frame, create_planes_proc!, rendering/mod.rs:483-651), or the
+// one plane of a gf_cuda_queue_create queue.  Every plane's Stabilization has the frame's size and ComputeParams, so one producer launch
+// serves all planes; per plane only the per-buffer half of KernelParams differs.  Planes of one pixel type and size fraction form a
+// group, which has one warp context in each slot.
+// One slot = one stream + a warp context per group + device staging of the HOST planes + a device matrix table with its trust verdict
+// word.  Per submitted frame, all enqueued on the slot's stream, nothing synchronous:
+//     producer kernel (gf_cuda_frame_transform_dev_flagged: table + verdict)  ->  [mesh H2D]  ->  [H2D of the HOST planes]
+//     ->  one gf_cuda_undistort_planes_dev_flagged per group  ->  [one checksum launch over all planes]  ->  [D2H of the HOST planes]  ->  event
 // Slots are used round-robin; submit() waits for a slot's previous frame only when it comes round again, wait() hands finished
 // frames back in submission order (output order restored by frame index on the host, as §8e asks).
-// A planes queue (gf_cuda_queue_create_planes) renders decoder frames of 1-4 planes (create_planes_proc!, rendering/mod.rs:483-651):
-// every plane's Stabilization has the frame's size and ComputeParams, so one producer launch serves all planes; per plane only the
-// per-buffer half of KernelParams differs.  Per frame: producer -> [H2D of every plane into the slot's staging] -> one planes call per
-// group (planes of one pixel type and size fraction, one context each) -> [one checksum launch over all planes] -> [D2H of every plane].
 #include <cuda_runtime.h>
 #include <nvtx3/nvToolsExt.h>
 #include <sched.h>
@@ -25,6 +25,7 @@
 #include <string>
 #include <vector>
 #include <deque>
+#include <algorithm>
 #include "../../include/gyroflow_cuda.h"
 #include "c_abi_internal.h"
 
@@ -33,7 +34,6 @@ using namespace gf;
 namespace {
 
 struct QSlot {
-    std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx;
     Stream stream;
     Event done;
     GrowBuf<float> d_mat;
@@ -42,22 +42,12 @@ struct QSlot {
     GrowBuf<uint64_t> d_sum; GrowBuf<uint64_t, true> h_sum;  // checksum (device word, pinned host copy)
     bool busy = false;
     size_t frame = 0;
-    // planes queue only: one warp context per plane group, device copies of every plane when the frames are HOST
-    std::vector<std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>>> group_ctx;
-    std::vector<GrowBuf<uint8_t>> plane_in, plane_out;
+    std::vector<std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>>> group_ctx;   // one warp context per plane group
+    PlaneStaging staging;                                    // device copies of the HOST planes, sized from the prototypes
 };
 
-// sum(word[i] * (2 i + 1)) mod 2^64: order-independent, so blocks may add their partial sums in any order
-__global__ void checksum_kernel(const uint32_t* __restrict__ w, size_t n, unsigned long long* __restrict__ out) {
-    unsigned long long s = 0;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        s += (unsigned long long)w[i] * (2ull * (unsigned long long)i + 1ull);
-    #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31u) == 0u && s) atomicAdd(out, s);
-}
-
-// The same sum over the rows of up to four descriptors read as one byte string (gf_cuda_checksum_planes_dev).  A block takes whole rows;
+// sum(word[i] * (2 i + 1)) mod 2^64 over the rows of up to four descriptors read as one byte string (gf_cuda_checksum_planes_dev):
+// order-independent, so blocks may add their partial sums in any order.  A block takes whole rows;
 // its threads take the string's 32-bit words that the row touches.  A word cut by a row boundary gets its bytes from both rows, each
 // row adding its own bytes times the word's weight, which sums to the whole word's term.
 struct ChecksumRows {
@@ -94,12 +84,14 @@ __global__ void checksum_rows_kernel(const ChecksumRows P, unsigned long long* _
     if ((threadIdx.x & 31u) == 0u && s) atomicAdd(out, s);
 }
 
-// A planes queue's layout: the planes, their prototypes and per-plane stab configs, and the groups that share a context.
+// One plane of the queue's layout.
 struct QPlane {
     gf_queue_plane spec;
-    gf_buffer_desc in_proto, out_proto;
-    gf_stab_config stab;                  // the queue's, with the plane's pixel type and background
-    int group;
+    // gf_cuda_queue_create's plane: keep the pixel limits gf_get_frame_transform_at derives (FLT_MAX / 1 for float types, which
+    // spec.max_value cannot express) instead of writing spec.max_value to them
+    bool derived_limits;
+    gf_stab_config stab;                  // the queue's, with the plane's pixel type and background (set by create_queue)
+    int group;                            // index into gf_cuda_queue::groups (-1 until create_queue)
 };
 
 } // namespace
@@ -114,9 +106,9 @@ struct gf_cuda_queue {
     size_t max_rows = 0;
     unsigned long long launches = 0;
     std::string last_error;
-    std::vector<QPlane> planes;           // empty: a gf_cuda_queue_create queue
+    std::vector<QPlane> planes;           // the layout: 1-4 planes
+    std::vector<gf_buffer_desc> in_protos, out_protos;   // per plane
     std::vector<std::vector<size_t>> groups;   // plane indices of each group, in plane order
-    bool host_frames = false;
 };
 
 namespace {
@@ -165,6 +157,127 @@ int enqueue_checksum_rows(const gf_checksum_plane* d, size_t n, uint64_t* out_de
 int ceil_div(int a, int b) { return (a + b - 1) / b; }
 bool same_shape(const gf_buffer_desc& a, const gf_buffer_desc& b) {
     return a.width == b.width && a.height == b.height && a.stride == b.stride && a.kind == b.kind;
+}
+
+using QueuePtr = std::unique_ptr<gf_cuda_queue, Deleter<gf_cuda_queue_destroy>>;
+
+// Both creates, once the layout (planes, prototypes) is in `q`: the planes' stab configs and groups, gyro upload, the slots with one
+// context per group (created for the group's first plane) and the HOST staging.
+int create_queue(QueuePtr q, gf_cuda_queue** out) {
+    const gf_queue_config& cfg = q->cfg;
+    for (size_t i = 0; i < q->planes.size(); ++i) {
+        QPlane& qp = q->planes[i];
+        qp.stab = cfg.stab; qp.stab.pixel_type = qp.spec.pixel_type;
+        memcpy(qp.stab.background, qp.spec.background, sizeof(qp.stab.background));
+        for (size_t k = 0; k < q->groups.size() && qp.group < 0; ++k) {
+            const gf_queue_plane& o = q->planes[q->groups[k][0]].spec;
+            if (o.pixel_type == qp.spec.pixel_type && o.w_div == qp.spec.w_div && o.h_div == qp.spec.h_div) qp.group = (int)k;
+        }
+        if (qp.group < 0) { qp.group = (int)q->groups.size(); q->groups.emplace_back(); }
+        q->groups[(size_t)qp.group].push_back(i);
+    }
+    CK(nullptr, cudaSetDevice(cfg.device));
+    if (cfg.pin_numa) (void)gf_cuda_bind_thread_to_device(cfg.device);      // before any page-locked staging is allocated
+    gf_cuda_gyro* gyro = nullptr;
+    int rc = gf_cuda_gyro_upload(&gyro, cfg.device, &q->cp);
+    if (rc != GF_OK) return rc;
+    q->gyro.reset(gyro);
+    q->max_rows = (size_t)(q->cp.width > q->cp.height ? q->cp.width : q->cp.height);
+    q->slots.resize((size_t)cfg.depth);
+    for (QSlot& s : q->slots) {
+        if ((rc = init_slot(s, q->max_rows)) != GF_OK) return rc;
+        for (const std::vector<size_t>& grp : q->groups) {
+            const QPlane& qp = q->planes[grp[0]];
+            gf_buffer_desc bi = q->in_protos[grp[0]], bo = q->out_protos[grp[0]];
+            if (bi.kind == GF_BUF_HOST) bi.kind = GF_BUF_DEVICE;      // the context sees the slot's device copies of HOST planes
+            if (bo.kind == GF_BUF_HOST) bo.kind = GF_BUF_DEVICE;
+            gf_kernel_params kp; memset(&kp, 0, sizeof(kp));          // a template good enough for gf_cuda_create's validation
+            kp.matrix_count = 1;
+            rc = gf_get_frame_transform_at(&qp.stab, &q->cp, &bi, &bo, nullptr, 0, 0.0, 0, 1.0, &kp);
+            if (rc != GF_OK) return fail(nullptr, rc, "plane " + std::to_string(grp[0]) + ": gf_get_frame_transform_at failed");
+            gf_cuda_ctx* ctx = nullptr;
+            rc = gf_cuda_create(&ctx, cfg.device, &kp, qp.spec.pixel_type, cfg.distortion_model, cfg.digital_lens, &bi, &bo, 0);
+            if (rc != GF_OK) return rc;
+            s.group_ctx.emplace_back(ctx);
+        }
+        CK(nullptr, s.staging.reserve(q->planes.size(), q->in_protos.data(), q->out_protos.data(), s.stream.get()));
+    }
+    *out = q.release();
+    return GF_OK;
+}
+
+// Both submits, after their own argument checks: slot, producer, mesh, every plane's KernelParams, HOST staging, one planes call per
+// group, checksum, download, event, FIFO.
+int submit_frame(gf_cuda_queue* q, size_t frame, double timestamp_ms, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out,
+                 const float* mesh, size_t mesh_len, int fill_with_background) {
+    std::string* const err = &q->last_error;
+    if (n_planes != q->planes.size()) return fail(err, GF_ERR_BAD_PARAMS, "n_planes differs from the queue's layout (" + std::to_string(q->planes.size()) + ")");
+    if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
+    CK(err, cudaSetDevice(q->cfg.device));
+    QSlot& s = q->slots[(size_t)q->next];
+    if (s.busy) return fail(err, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
+    int rc = s.staging.check(n_planes, in, out, err);
+    if (rc != GF_OK) return rc;
+    const cudaStream_t st = s.stream.get();
+    nvtxRangePushA("gf_queue_submit");
+    struct PopRange { ~PopRange() { nvtxRangePop(); } } pop_range;
+    // one table + verdict for every plane: each plane's Stabilization is sized with the frame (rendering/mod.rs:514)
+    gf_kernel_params kp0; size_t rows = 0; double fov = 1.0, minimal_fov = 1.0;
+    rc = gf_cuda_frame_transform_dev_flagged(q->gyro.get(), &q->cp, timestamp_ms, frame, &kp0, s.d_mat.ptr, q->max_rows, s.d_flags.ptr,
+                                             &rows, &fov, &minimal_fov, (void*)st);
+    if (rc != GF_OK) return fail(err, rc, "gf_cuda_frame_transform_dev_flagged failed");
+    q->launches++;
+    const float* mesh_dev = nullptr;
+    if (mesh && mesh_len) {
+        memcpy(s.h_mesh.ptr, mesh, mesh_len * sizeof(float));
+        CK(err, cudaMemcpyAsync(s.d_mesh.ptr, s.h_mesh.ptr, mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
+        mesh_dev = s.d_mesh.ptr;
+    }
+    // the per-buffer half, per plane, as rendering/mod.rs:531-541 completes it before process_pixels
+    gf_kernel_params kp[4];
+    gf_buffer_desc din[4], dout[4];
+    for (size_t i = 0; i < n_planes; ++i) {
+        const QPlane& qp = q->planes[i];
+        kp[i] = kp0;
+        rc = gf_get_frame_transform_at(&qp.stab, &q->cp, &in[i], &out[i], mesh, mesh_len, timestamp_ms, frame, minimal_fov, &kp[i]);
+        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(i) + ": gf_get_frame_transform_at failed");
+        if (!qp.derived_limits) kp[i].pixel_value_limit = kp[i].max_pixel_value = qp.spec.max_value;
+        kp[i].plane_index = (int32_t)i;
+        if (fill_with_background) kp[i].flags |= GF_FLAG_FILL_WITH_BACKGROUND;
+    }
+    // from here on, copies from the caller's HOST buffers may be queued: a failure waits for them before it returns
+    struct WaitOnFailure { cudaStream_t st; bool ok; ~WaitOnFailure() { if (!ok) { (void)cudaStreamSynchronize(st); (void)cudaGetLastError(); } } } wait_on_failure{st, false};
+    if ((rc = s.staging.upload(n_planes, in, out, kp, q->cfg.checksum != 0, st, err, din, dout)) != GF_OK) return rc;
+    // each group through the planes path: its planner fuses the planes whose KernelParams agree, the rest get a warp each
+    for (size_t g = 0; g < q->groups.size(); ++g) {
+        const std::vector<size_t>& grp = q->groups[g];
+        gf_buffer_desc gi[4], go[4]; gf_kernel_params gp[4];
+        for (size_t j = 0; j < grp.size(); ++j) { gi[j] = din[grp[j]]; go[j] = dout[grp[j]]; gp[j] = kp[grp[j]]; }
+        gf_cuda_ctx* const ctx = s.group_ctx[g].get();
+        const unsigned long long l0 = gf_cuda_launch_count(ctx);
+        rc = gf_cuda_undistort_planes_dev_flagged(ctx, grp.size(), gi, go, gp, s.d_mat.ptr, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags.ptr, (void*)st);
+        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(grp[0]) + ": " + gf_cuda_last_error(ctx));
+        q->launches += gf_cuda_launch_count(ctx) - l0;
+    }
+    if (q->cfg.checksum) {           // every plane's first min(len, height * stride) bytes: whole rows, then the rest of a short last row
+        gf_checksum_plane d[8]; size_t nd = 0;
+        for (size_t i = 0; i < n_planes; ++i) {
+            const size_t stride = (size_t)dout[i].stride, nr = std::min((size_t)dout[i].height, dout[i].len / stride);
+            const size_t tail = std::min(dout[i].len, (size_t)dout[i].height * stride) - nr * stride;
+            d[nd++] = { dout[i].ptr, stride, stride, nr };
+            if (tail) d[nd++] = { static_cast<const uint8_t*>(dout[i].ptr) + nr * stride, tail, tail, 1 };
+        }
+        if ((rc = enqueue_checksum_rows(d, nd, s.d_sum.ptr, st, err)) != GF_OK) return rc;
+        q->launches++;
+        CK(err, cudaMemcpyAsync(s.h_sum.ptr, s.d_sum.ptr, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    }
+    if ((rc = s.staging.download(n_planes, out, kp, st, err)) != GF_OK) return rc;
+    CK(err, cudaEventRecord(s.done.get(), st));
+    wait_on_failure.ok = true;
+    s.busy = true; s.frame = frame;
+    q->fifo.push_back(q->next);
+    q->next = (q->next + 1) % (int)q->slots.size();
+    return GF_OK;
 }
 } // namespace
 
@@ -219,14 +332,12 @@ GF_API int gf_cuda_host_unregister(void* ptr) {
     return GF_OK;
 }
 
+// One whole-row descriptor of 64 KiB rows and one for the rest: the rows kernel gives each block whole rows.
 GF_API int gf_cuda_checksum_dev(const void* ptr_dev, size_t len, uint64_t* out_dev, void* cu_stream) {
     if (!ptr_dev || !out_dev) return GF_ERR_BAD_PARAMS;
-    cudaStream_t st = (cudaStream_t)cu_stream;
-    CK(nullptr, cudaMemsetAsync(out_dev, 0, sizeof(uint64_t), st));
-    const size_t n = len / 4;
-    if (n) checksum_kernel<<<132 * 4, 256, 0, st>>>(reinterpret_cast<const uint32_t*>(ptr_dev), n, reinterpret_cast<unsigned long long*>(out_dev));
-    CK(nullptr, cudaGetLastError());
-    return GF_OK;
+    const size_t row = (size_t)1 << 16, rows = len >> 16, tail = len & (row - 1);
+    const gf_checksum_plane d[2] = { { ptr_dev, row, row, rows }, { static_cast<const uint8_t*>(ptr_dev) + rows * row, tail, tail, 1 } };
+    return enqueue_checksum_rows(d, tail ? 2 : 1, out_dev, (cudaStream_t)cu_stream, nullptr);
 }
 
 GF_API int gf_cuda_queue_create(gf_cuda_queue** out, const gf_queue_config* cfg, const gf_compute_params* cp,
@@ -234,30 +345,13 @@ GF_API int gf_cuda_queue_create(gf_cuda_queue** out, const gf_queue_config* cfg,
     if (!out || !cfg || !cp || !in_proto || !out_proto) return GF_ERR_BAD_PARAMS;
     *out = nullptr;
     if (cfg->depth < 1 || cfg->depth > 16) return GF_ERR_BAD_PARAMS;
-    std::unique_ptr<gf_cuda_queue, Deleter<gf_cuda_queue_destroy>> q(new gf_cuda_queue());
+    QueuePtr q(new gf_cuda_queue());
     q->cfg = *cfg; q->cp = *cp;
-    CK(nullptr, cudaSetDevice(cfg->device));
-    if (cfg->pin_numa) (void)gf_cuda_bind_thread_to_device(cfg->device);      // before any page-locked staging is allocated
-    gf_cuda_gyro* gyro = nullptr;
-    int rc = gf_cuda_gyro_upload(&gyro, cfg->device, cp);
-    if (rc != GF_OK) return rc;
-    q->gyro.reset(gyro);
-    // a template KernelParams good enough for gf_cuda_create's validation (sizes, strides, interpolation, pixel size)
-    gf_kernel_params kp; memset(&kp, 0, sizeof(kp));
-    kp.matrix_count = 1;
-    rc = gf_get_frame_transform_at(&cfg->stab, cp, in_proto, out_proto, nullptr, 0, 0.0, 0, 1.0, &kp);
-    if (rc != GF_OK) return rc;
-    q->max_rows = (size_t)(cp->width > cp->height ? cp->width : cp->height);
-    q->slots.resize((size_t)cfg->depth);
-    for (QSlot& s : q->slots) {
-        gf_cuda_ctx* ctx = nullptr;
-        rc = gf_cuda_create(&ctx, cfg->device, &kp, cfg->stab.pixel_type, cfg->distortion_model, cfg->digital_lens, in_proto, out_proto, 0);
-        if (rc != GF_OK) return rc;
-        s.ctx.reset(ctx);
-        if ((rc = init_slot(s, q->max_rows)) != GF_OK) return rc;
-    }
-    *out = q.release();
-    return GF_OK;
+    gf_queue_plane spec{cfg->stab.pixel_type, 1, 1, 0.0f, {}};     // the config's pixel type and background, full size
+    memcpy(spec.background, cfg->stab.background, sizeof(spec.background));
+    q->planes.push_back(QPlane{spec, true, {}, -1});
+    q->in_protos.push_back(*in_proto); q->out_protos.push_back(*out_proto);
+    return create_queue(std::move(q), out);
 }
 
 GF_API int gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_config* cfg, const gf_compute_params* cp, size_t n_planes,
@@ -266,9 +360,8 @@ GF_API int gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_confi
     *out = nullptr;
     if (n_planes < 1 || n_planes > 4) return fail(nullptr, GF_ERR_BAD_PARAMS, "n_planes must be 1..4");
     if (cfg->depth < 1 || cfg->depth > 16) return fail(nullptr, GF_ERR_BAD_PARAMS, "depth must be 1..16");
-    std::unique_ptr<gf_cuda_queue, Deleter<gf_cuda_queue_destroy>> q(new gf_cuda_queue());
+    QueuePtr q(new gf_cuda_queue());
     q->cfg = *cfg; q->cp = *cp;
-    q->host_frames = in_protos[0].kind == GF_BUF_HOST;
     // everything checkable on the host first: nothing touches the device before the layout is known to be good
     for (size_t i = 0; i < n_planes; ++i) {
         const gf_queue_plane& pl = planes[i];
@@ -284,178 +377,31 @@ GF_API int gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_confi
             return fail(nullptr, GF_ERR_BAD_PARAMS, name + "a UV plane is ceil(W / w_div) pixels wide");
         if (bo.stride < 1 || bo.height < 1 || bo.len < (size_t)bo.height * (size_t)bo.stride)
             return fail(nullptr, GF_ERR_BAD_PARAMS, name + "the output buffer holds fewer than height rows of stride bytes");
-        QPlane qp;
-        qp.spec = pl; qp.in_proto = bi; qp.out_proto = bo;
-        qp.stab = cfg->stab; qp.stab.pixel_type = pl.pixel_type;
-        for (int c = 0; c < 4; ++c) qp.stab.background[c] = pl.background[c];
-        qp.group = -1;
-        for (size_t k = 0; k < q->groups.size() && qp.group < 0; ++k) {
-            const gf_queue_plane& o = q->planes[q->groups[k][0]].spec;
-            if (o.pixel_type == pl.pixel_type && o.w_div == pl.w_div && o.h_div == pl.h_div) qp.group = (int)k;
-        }
-        if (qp.group < 0) { qp.group = (int)q->groups.size(); q->groups.emplace_back(); }
-        q->groups[(size_t)qp.group].push_back(i);
-        q->planes.push_back(qp);
+        q->planes.push_back(QPlane{pl, false, {}, -1});
     }
-    CK(nullptr, cudaSetDevice(cfg->device));
-    if (cfg->pin_numa) (void)gf_cuda_bind_thread_to_device(cfg->device);
-    gf_cuda_gyro* gyro = nullptr;
-    int rc = gf_cuda_gyro_upload(&gyro, cfg->device, cp);
-    if (rc != GF_OK) return rc;
-    q->gyro.reset(gyro);
-    q->max_rows = (size_t)(cp->width > cp->height ? cp->width : cp->height);
-    q->slots.resize((size_t)cfg->depth);
-    for (QSlot& s : q->slots) {
-        if ((rc = init_slot(s, q->max_rows)) != GF_OK) return rc;
-        for (const std::vector<size_t>& grp : q->groups) {            // one context per group, created for its first plane's buffers
-            const QPlane& qp = q->planes[grp[0]];
-            gf_buffer_desc bi = qp.in_proto, bo = qp.out_proto;
-            bi.kind = bo.kind = GF_BUF_DEVICE;                         // HOST frames are staged by the queue, the context sees device copies
-            gf_kernel_params kp; memset(&kp, 0, sizeof(kp));
-            kp.matrix_count = 1;
-            rc = gf_get_frame_transform_at(&qp.stab, cp, &bi, &bo, nullptr, 0, 0.0, 0, 1.0, &kp);
-            if (rc != GF_OK) return fail(nullptr, rc, "plane " + std::to_string(grp[0]) + ": gf_get_frame_transform_at failed");
-            gf_cuda_ctx* ctx = nullptr;
-            rc = gf_cuda_create(&ctx, cfg->device, &kp, qp.spec.pixel_type, cfg->distortion_model, cfg->digital_lens, &bi, &bo, 0);
-            if (rc != GF_OK) return rc;
-            s.group_ctx.emplace_back(ctx);
-        }
-        if (q->host_frames) {
-            s.plane_in.resize(n_planes); s.plane_out.resize(n_planes);
-            for (size_t i = 0; i < n_planes; ++i) {
-                CK(nullptr, s.plane_in[i].reserve(q->planes[i].in_proto.len, s.stream.get()));
-                CK(nullptr, s.plane_out[i].reserve(q->planes[i].out_proto.len, s.stream.get()));
-            }
-        }
-    }
-    *out = q.release();
-    return GF_OK;
+    q->in_protos.assign(in_protos, in_protos + n_planes); q->out_protos.assign(out_protos, out_protos + n_planes);
+    return create_queue(std::move(q), out);
 }
 
 GF_API int gf_cuda_queue_submit(gf_cuda_queue* q, size_t frame, double timestamp_ms, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                 const float* mesh, size_t mesh_len) {
     if (!q || !in || !out) return fail(q ? &q->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    std::string* const err = &q->last_error;
-    if (!q->planes.empty()) return fail(err, GF_ERR_BAD_PARAMS, "a planes queue takes gf_cuda_queue_submit_planes");
-    if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
-    CK(err, cudaSetDevice(q->cfg.device));
-    QSlot& s = q->slots[(size_t)q->next];
-    if (s.busy) return fail(err, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
-    const cudaStream_t st = s.stream.get();
-    nvtxRangePushA("gf_queue_submit");
-    // FrameTransform::at_timestamp on the device: rows x 14 table + its trust verdict, then the per-buffer half of KernelParams
-    gf_kernel_params kp; size_t rows = 0; double fov = 1.0, minimal_fov = 1.0;
-    int rc = gf_cuda_frame_transform_dev_flagged(q->gyro.get(), &q->cp, timestamp_ms, frame, &kp, s.d_mat.ptr, q->max_rows, s.d_flags.ptr,
-                                                 &rows, &fov, &minimal_fov, (void*)st);
-    if (rc != GF_OK) { nvtxRangePop(); return fail(err, rc, "gf_cuda_frame_transform_dev_flagged failed"); }
-    q->launches++;
-    rc = gf_get_frame_transform_at(&q->cfg.stab, &q->cp, in, out, mesh, mesh_len, timestamp_ms, frame, minimal_fov, &kp);
-    if (rc != GF_OK) { nvtxRangePop(); return fail(err, rc, "gf_get_frame_transform_at failed"); }
-    const float* mesh_dev = nullptr;
-    if (mesh && mesh_len) {
-        memcpy(s.h_mesh.ptr, mesh, mesh_len * sizeof(float));
-        cudaError_t e = cudaMemcpyAsync(s.d_mesh.ptr, s.h_mesh.ptr, mesh_len * sizeof(float), cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { nvtxRangePop(); return cuda_error(e, "mesh upload", err); }
-        mesh_dev = s.d_mesh.ptr;
-    }
-    const unsigned long long l0 = gf_cuda_launch_count(s.ctx.get());
-    rc = gf_internal_run_frame(s.ctx.get(), in, out, &kp, s.d_mat.ptr, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags.ptr, (void*)st,
-                               q->cfg.checksum ? s.d_sum.ptr : nullptr);
-    if (rc != GF_OK) { q->last_error = gf_cuda_last_error(s.ctx.get()); nvtxRangePop(); return rc; }
-    q->launches += gf_cuda_launch_count(s.ctx.get()) - l0 + (q->cfg.checksum ? 1 : 0);
-    if (q->cfg.checksum) {
-        cudaError_t e = cudaMemcpyAsync(s.h_sum.ptr, s.d_sum.ptr, sizeof(uint64_t), cudaMemcpyDeviceToHost, st);
-        if (e != cudaSuccess) { nvtxRangePop(); return cuda_error(e, "checksum download", err); }
-    }
-    cudaError_t e = cudaEventRecord(s.done.get(), st);
-    nvtxRangePop();
-    if (e != cudaSuccess) return cuda_error(e, "cudaEventRecord", err);
-    s.busy = true; s.frame = frame;
-    q->fifo.push_back(q->next);
-    q->next = (q->next + 1) % (int)q->slots.size();
-    return GF_OK;
+    return submit_frame(q, frame, timestamp_ms, 1, in, out, mesh, mesh_len, 0);
 }
 
 GF_API int gf_cuda_queue_submit_planes(gf_cuda_queue* q, size_t frame, double timestamp_ms, size_t n_planes, const gf_buffer_desc* in,
                                        const gf_buffer_desc* out, const float* mesh, size_t mesh_len, int fill_with_background) {
     if (!q || !in || !out) return fail(q ? &q->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
     std::string* const err = &q->last_error;
-    if (q->planes.empty()) return fail(err, GF_ERR_BAD_PARAMS, "a one-plane queue takes gf_cuda_queue_submit");
-    if (n_planes != q->planes.size()) return fail(err, GF_ERR_BAD_PARAMS, "n_planes differs from the queue's layout (" + std::to_string(q->planes.size()) + ")");
-    if (mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
-    for (size_t i = 0; i < n_planes; ++i) {
-        const QPlane& qp = q->planes[i];
+    for (size_t i = 0; i < std::min(n_planes, q->planes.size()); ++i) {      // a count other than the layout's: submit_frame refuses it
         const std::string name = "plane " + std::to_string(i) + ": ";
         if (in[i].kind != in[0].kind || out[i].kind != in[0].kind) return fail(err, GF_ERR_BAD_PARAMS, name + "HOST and DEVICE buffers mixed in one frame");
-        if (!same_shape(in[i], qp.in_proto) || !same_shape(out[i], qp.out_proto) || !in[i].ptr || !out[i].ptr)
+        if (!same_shape(in[i], q->in_protos[i]) || !same_shape(out[i], q->out_protos[i]) || !in[i].ptr || !out[i].ptr)
             return fail(err, GF_ERR_BAD_PARAMS, name + "buffer size, stride or kind differs from the prototype's");
         if (out[i].len < (size_t)out[i].height * (size_t)out[i].stride)
             return fail(err, GF_ERR_BAD_PARAMS, name + "the output buffer holds fewer than height rows of stride bytes");
-        if (q->host_frames && (in[i].len > qp.in_proto.len || out[i].len > qp.out_proto.len))
-            return fail(err, GF_ERR_BUFFER_TOO_SMALL, name + "HOST buffer longer than the prototype's (the staging size)");
     }
-    CK(err, cudaSetDevice(q->cfg.device));
-    QSlot& s = q->slots[(size_t)q->next];
-    if (s.busy) return fail(err, GF_ERR_BAD_PARAMS, "queue full: gf_cuda_queue_wait for the oldest frame first");
-    const cudaStream_t st = s.stream.get();
-    nvtxRangePushA("gf_queue_submit_planes");
-    struct PopRange { ~PopRange() { nvtxRangePop(); } } pop_range;
-    // one table + verdict for every plane: each plane's Stabilization is sized with the frame (rendering/mod.rs:514)
-    gf_kernel_params kp0; size_t rows = 0; double fov = 1.0, minimal_fov = 1.0;
-    int rc = gf_cuda_frame_transform_dev_flagged(q->gyro.get(), &q->cp, timestamp_ms, frame, &kp0, s.d_mat.ptr, q->max_rows, s.d_flags.ptr,
-                                                 &rows, &fov, &minimal_fov, (void*)st);
-    if (rc != GF_OK) return fail(err, rc, "gf_cuda_frame_transform_dev_flagged failed");
-    q->launches++;
-    const float* mesh_dev = nullptr;
-    if (mesh && mesh_len) {
-        memcpy(s.h_mesh.ptr, mesh, mesh_len * sizeof(float));
-        CK(err, cudaMemcpyAsync(s.d_mesh.ptr, s.h_mesh.ptr, mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
-        mesh_dev = s.d_mesh.ptr;
-    }
-    // the per-buffer half, per plane, as rendering/mod.rs:531-541 completes it before process_pixels
-    gf_kernel_params kp[4];
-    gf_buffer_desc din[4], dout[4];
-    for (size_t i = 0; i < n_planes; ++i) {
-        const QPlane& qp = q->planes[i];
-        kp[i] = kp0;
-        rc = gf_get_frame_transform_at(&qp.stab, &q->cp, &in[i], &out[i], mesh, mesh_len, timestamp_ms, frame, minimal_fov, &kp[i]);
-        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(i) + ": gf_get_frame_transform_at failed");
-        kp[i].pixel_value_limit = kp[i].max_pixel_value = qp.spec.max_value;
-        kp[i].plane_index = (int32_t)i;
-        if (fill_with_background) kp[i].flags |= GF_FLAG_FILL_WITH_BACKGROUND;
-        din[i] = in[i]; dout[i] = out[i];
-        if (q->host_frames) {                  // the output too: pixels the warp leaves alone keep their content, like on the CPU path
-            CK(err, cudaMemcpyAsync(s.plane_in[i].ptr, in[i].ptr, in[i].len, cudaMemcpyHostToDevice, st));
-            CK(err, cudaMemcpyAsync(s.plane_out[i].ptr, out[i].ptr, out[i].len, cudaMemcpyHostToDevice, st));
-            din[i].kind = dout[i].kind = GF_BUF_DEVICE;
-            din[i].ptr = s.plane_in[i].ptr; dout[i].ptr = s.plane_out[i].ptr;
-        }
-    }
-    // each group through the planes path: its planner fuses the planes whose KernelParams agree, the rest get a warp each
-    for (size_t g = 0; g < q->groups.size(); ++g) {
-        const std::vector<size_t>& grp = q->groups[g];
-        gf_buffer_desc gi[4], go[4]; gf_kernel_params gp[4];
-        for (size_t j = 0; j < grp.size(); ++j) { gi[j] = din[grp[j]]; go[j] = dout[grp[j]]; gp[j] = kp[grp[j]]; }
-        gf_cuda_ctx* const ctx = s.group_ctx[g].get();
-        const unsigned long long l0 = gf_cuda_launch_count(ctx);
-        rc = gf_cuda_undistort_planes_dev_flagged(ctx, grp.size(), gi, go, gp, s.d_mat.ptr, rows, mesh_dev, mesh_dev ? mesh_len : 0, s.d_flags.ptr, (void*)st);
-        if (rc != GF_OK) return fail(err, rc, "plane " + std::to_string(grp[0]) + ": " + gf_cuda_last_error(ctx));
-        q->launches += gf_cuda_launch_count(ctx) - l0;
-    }
-    if (q->cfg.checksum) {
-        gf_checksum_plane d[4];
-        for (size_t i = 0; i < n_planes; ++i) d[i] = { dout[i].ptr, (size_t)dout[i].stride, (size_t)dout[i].stride, (size_t)dout[i].height };
-        if ((rc = enqueue_checksum_rows(d, n_planes, s.d_sum.ptr, st, err)) != GF_OK) return rc;
-        q->launches++;
-        CK(err, cudaMemcpyAsync(s.h_sum.ptr, s.d_sum.ptr, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-    }
-    if (q->host_frames)
-        for (size_t i = 0; i < n_planes; ++i) CK(err, cudaMemcpyAsync(out[i].ptr, s.plane_out[i].ptr, out[i].len, cudaMemcpyDeviceToHost, st));
-    CK(err, cudaEventRecord(s.done.get(), st));
-    s.busy = true; s.frame = frame;
-    q->fifo.push_back(q->next);
-    q->next = (q->next + 1) % (int)q->slots.size();
-    return GF_OK;
+    return submit_frame(q, frame, timestamp_ms, n_planes, in, out, mesh, mesh_len, fill_with_background);
 }
 
 GF_API int gf_cuda_checksum_planes_dev(const gf_checksum_plane* planes, size_t n, uint64_t* out_dev, void* cu_stream) {

@@ -576,14 +576,21 @@ GF_API int gf_get_frame_transform_at(const gf_stab_config* stab, const gf_comput
  * Frame-sharded render queue (SURVEY §8e; the shape of rendering/mod.rs:451,531-542,657-661 with rendering/render_queue.rs:550-612
  * turned inside out: instead of whole jobs in parallel, the frames of one job run `depth` deep on one GPU, and `i -> GPU i mod G`
  * across the processes of a box).  One queue = one device: `depth` slots, each with its own stream, device table + verdict word,
- * and (HOST buffers) device staging.  Per submitted frame, all on the slot's stream, nothing synchronous:
+ * and device staging of the HOST buffers.  Per submitted frame, all on the slot's stream, nothing synchronous:
  *     gf_cuda_frame_transform_dev_flagged (table + verdict on the device)  ->  [H2D]  ->  warp  ->  [checksum]  ->  [D2H]
+ * A HOST output is uploaded before the warp unless the warp writes every byte of it that is read afterwards; a warp that covers the
+ * buffer sends back only its pixel rows, so stride padding keeps the host's bytes.
  * gf_cuda_queue_submit never blocks: with `depth` frames already in flight it fails with GF_ERR_BAD_PARAMS ("queue full") — call
  * gf_cuda_queue_wait first; gf_cuda_queue_wait blocks until the OLDEST frame is done and returns frames in submission order.  HOST buffers must be page-locked and stay valid until the
  * frame has been waited for.  `cp` is copied shallowly: the arrays it points to (tracks are uploaded at creation; fovs, offsets, focal lengths,
- * camera_stab, keyframe tracks, lens_per_frame are read per frame on the host) must stay valid until gf_cuda_queue_destroy.  The optional checksum is sum(word[i] * (2 i + 1)) mod 2^64 over the output buffer's 32-bit words.
+ * camera_stab, keyframe tracks, lens_per_frame are read per frame on the host) must stay valid until gf_cuda_queue_destroy.  The optional checksum is sum(word[i] * (2 i + 1)) mod 2^64 over the output buffer's 32-bit words:
+ * its first min(len, height * stride) bytes, padding included.  For a HOST output that is the host buffer's own padding, uploaded with the
+ * frame, so the checksum equals the one computed on the host buffer gf_cuda_queue_wait hands back.
  * Decoder frames of 1-4 planes (NV12, P010, planar YUV, GBRAPF32, ...) take gf_cuda_queue_create_planes / gf_cuda_queue_submit_planes
  * below: still one producer launch and one slot per frame, the planes' warps and one checksum over all of them on the slot's stream.
+ * A gf_cuda_queue_create queue is a layout of one plane (the config's pixel type and background, full size, the pixel limits
+ * gf_get_frame_transform_at derives), so gf_cuda_queue_submit_planes with n_planes = 1 takes its frames too when its two prototypes
+ * are of one kind (a frame of HOST and DEVICE buffers is gf_cuda_queue_submit's alone).
  * ---------------------------------------------------------------------------------------- */
 typedef struct gf_cuda_queue gf_cuda_queue;
 typedef struct gf_queue_config {
@@ -626,15 +633,17 @@ typedef struct gf_queue_plane {
     float   background[4];                    /* in this plane's components, 0..1 like gf_stab_config.background */
 } gf_queue_plane;
 /* n_planes 1..4; in_protos / out_protos: n_planes buffer descriptions whose sizes, strides and kind every frame must repeat.  HOST
- * frames are staged through per-slot device copies of every plane (sized from the prototypes).  Fails with GF_ERR_BAD_PARAMS before
+ * buffers are staged through per-slot device copies (sized from the prototypes).  Fails with GF_ERR_BAD_PARAMS before
  * any CUDA call, naming the plane in gf_cuda_last_error(NULL), for: n_planes outside 1..4, w_div / h_div not 1 or 2, a UV8 / UV16 plane
  * whose buffer width is not ceil(W / w_div) (output: ceil(output W / w_div)), HOST and DEVICE prototypes mixed, an output prototype
  * whose buffer holds fewer than height rows of stride bytes, and a (pixel type, lens, digital lens, interpolation) that
- * gf_combo_supported rejects.  gf_cuda_queue_submit on such a queue fails; gf_cuda_queue_wait / drain / launches are shared. */
+ * gf_combo_supported rejects.  gf_cuda_queue_submit takes the frames of a one-plane layout and fails on any other (GF_ERR_BAD_PARAMS);
+ * gf_cuda_queue_wait / drain / launches are shared. */
 GF_API int      gf_cuda_queue_create_planes(gf_cuda_queue** out, const gf_queue_config* cfg, const gf_compute_params* cp, size_t n_planes,
                                             const gf_queue_plane* planes, const gf_buffer_desc* in_protos, const gf_buffer_desc* out_protos);
-/* One frame of a planes queue: in / out are arrays of n_planes (the queue's count) with the prototypes' sizes, strides and kind, all
- * HOST or all DEVICE.  A mismatch is GF_ERR_BAD_PARAMS before anything is enqueued, with the plane named in gf_cuda_queue_last_error.
+/* One frame of a queue of either create: in / out are arrays of n_planes (the queue's count) with the prototypes' sizes, strides and
+ * kind, all HOST or all DEVICE.  A mismatch is GF_ERR_BAD_PARAMS before anything is enqueued, with the plane named in
+ * gf_cuda_queue_last_error; a HOST buffer longer than its prototype is GF_ERR_BUFFER_TOO_SMALL.
  * A slot holds one frame; gf_cuda_queue_wait returns its frame checksum (below) when cfg.checksum is set. */
 GF_API int      gf_cuda_queue_submit_planes(gf_cuda_queue* q, size_t frame, double timestamp_ms, size_t n_planes, const gf_buffer_desc* in,
                                             const gf_buffer_desc* out, const float* mesh, size_t mesh_len, int fill_with_background);
@@ -642,9 +651,9 @@ GF_API int      gf_cuda_queue_submit_planes(gf_cuda_queue* q, size_t frame, doub
 /* Multi-plane checksum.  A descriptor names `rows` rows of `row_bytes` bytes, row r starting at ptr + r * stride (no alignment asked of
  * ptr, stride or row_bytes).  The summed byte string is every descriptor's rows, in order, concatenated; it is read as little-endian
  * 32-bit words word[i] (a final group of fewer than 4 bytes is left out) and the checksum is sum(word[i] * (2 i + 1)) mod 2^64, i running
- * over the whole string.  One descriptor {ptr, stride, stride, rows} is gf_cuda_checksum_dev(ptr, rows * stride).  A planes queue sums
- * {out[i].ptr, stride, stride, height} of every output plane (padding bytes included, as the one-plane checksum does), so a one-plane
- * layout gives the checksum of a gf_cuda_queue_create queue on the same buffer.  One kernel launch for all descriptors (n 1..4),
+ * over the whole string.  One descriptor {ptr, stride, stride, rows} is gf_cuda_checksum_dev(ptr, rows * stride).  The queue sums
+ * {out[i].ptr, stride, stride, min(height, len / stride)} of every output plane (padding bytes included), plus the rest of a short last
+ * row when a gf_cuda_queue_create output holds less than height * stride bytes.  One kernel launch for all descriptors (n 1..4),
  * accumulated into *out_dev (zeroed first) on `cu_stream`. */
 typedef struct gf_checksum_plane { const void* ptr; size_t row_bytes, stride, rows; } gf_checksum_plane;
 GF_API int      gf_cuda_checksum_planes_dev(const gf_checksum_plane* planes, size_t n, uint64_t* out_dev, void* cu_stream);

@@ -7,6 +7,7 @@ against the host producer (gf_frame_transform_at_timestamp: IBIS / OIS columns b
 tests/test_device_producer.py checks the host producer against the numpy restatement, so a wrong device table cannot pass as its
 own reference.  The 2-rank test renders frames `rank::2` of one job on two processes and gathers the per-frame checksums in frame order — over NCCL when the box has two GPUs,
 over gloo with both ranks on GPU 0 otherwise (the data path has no collective either way)."""
+import ctypes as C
 import os
 import socket
 
@@ -23,22 +24,23 @@ W, H = 640, 360
 FPS = 60.0
 
 
-def _job(pix="RGBA8", lens="opencv_fisheye", digital=None, w=W, h=H, **cpkw):
-    p = synth.base_kernel_params(w, h, pixel_type=pix, lens=lens, digital_lens=digital)
+def _job(pix="RGBA8", lens="opencv_fisheye", digital=None, w=W, h=H, out_stride=None, **cpkw):
+    p = synth.base_kernel_params(w, h, pixel_type=pix, lens=lens, digital_lens=digital, out_stride=out_stride)
     org, sm = cases.gyro()
     cp = g.ComputeParams(p, org, sm, **cpkw)
     return p, cp, g.stab_config(p, pix, digital_lens=digital)
 
 
-def _expected(p, cp, st, dg, mats_dev, ts, frame, src, pix, lens, digital, bufs, mesh=None):
-    """The frame as the reference would render it from the table the device producer writes for (ts, frame)."""
+def _expected(p, cp, st, dg, mats_dev, ts, frame, src, pix, lens, digital, bufs, mesh=None, fill=0):
+    """The frame as the reference would render it from the table the device producer writes for (ts, frame), into an output buffer
+    whose bytes are all `fill` before."""
     kp, rows = dg.frame_transform(ts, mats_dev.data_ptr(), max(p.width, p.height), frame=frame)     # stream = 0: synchronous
     table = mats_dev.cpu().numpy()[:rows].copy()
     kp_h, table_h, _, _ = cp.at_timestamp(ts, frame)              # the host producer: same KernelParams, the same table to the bars
     assert bytes(kp) == bytes(kp_h)                               # of tests/test_device_producer.py
     producer_cases.compare_tables(table, table_h)
     g.get_frame_transform_at(st, cp, bufs, kp, mesh=mesh, frame=frame)
-    want = np.zeros((p.output_height, p.output_stride), np.uint8)
+    want = np.full((p.output_height, p.output_stride), fill, np.uint8)
     assert oracle_lib.undistort_image(src, want, kp, pix, lens, digital, table, mesh) == 0
     return want
 
@@ -119,6 +121,33 @@ def test_queue_host_buffers_pipelined(pix, lens, digital, extra):
     dg.close()
 
 
+@pytest.mark.parametrize("rect", [None, (24, 10, W - 40, H - 30)])
+def test_queue_host_output_rows_with_padding(rect):
+    """HOST output rows with 64 bytes of padding, every byte pre-filled with 0xA5: the bytes equal the oracle's render into the same
+    pre-fill, the padding keeps its 0xA5, and the checksum the queue returns is that of the host buffer it hands back.  Without a rect the
+    warp covers the buffer, so only the pixel rows come back; with one it does not, so the buffer is uploaded before the warp."""
+    import torch
+    pix, lens, n = "RGBA8", "opencv_fisheye", 6
+    p, cp, st = _job(out_stride=W * 4 + 64)
+    src = torch.from_numpy(synth.synthetic_frame(W, H, pix, stride=p.stride)).pin_memory()
+    outs = [torch.full((H, p.output_stride), 0xA5, dtype=torch.uint8).pin_memory() for _ in range(n)]
+    bufs = [g.Buffers(g.BufferDescription((W, H, p.stride), src.numpy()), g.BufferDescription((W, H, p.output_stride), o.numpy(), rect=rect))
+            for o in outs]
+    q = g.RenderQueue(cp, st, lens, None, bufs[0].input, bufs[0].output, depth=3, checksum=True)
+    ts_of = lambda f: 500.0 + f * (1000.0 / FPS)
+    sums = q.render(range(n), ts_of, lambda f: bufs[f])
+    q.close()
+    dg = g.DeviceGyro(cp)
+    mats = torch.zeros((max(W, H), 14), dtype=torch.float32, device="cuda")
+    for f in range(n):
+        got = outs[f].numpy()
+        want = _expected(p, cp, st, dg, mats, ts_of(f), f, src.numpy(), pix, lens, None, bufs[f], fill=0xA5)
+        assert np.array_equal(got, want), "frame %d" % f
+        assert (got[:, W * 4:] == 0xA5).all(), "frame %d" % f
+        assert sums[f] == render_queue.checksum_host(got), "frame %d" % f
+    dg.close()
+
+
 def test_thousand_frame_job_cfg5_shape():
     """BASELINE config 5's shape at a reduced frame size: 1000 frames with distinct timestamps through one queue, 6 in flight, results in
     frame order; every 40th frame against the oracle (bytes through the checksum), and no two neighbouring frames alike."""
@@ -152,6 +181,9 @@ def test_queue_full_and_errors():
     src = torch.zeros((H, p.stride), dtype=torch.uint8, device="cuda"); dst = torch.zeros((H, p.output_stride), dtype=torch.uint8, device="cuda")
     b = g.Buffers(g.BufferDescription((W, H, p.stride), src.data_ptr(), length=src.numel()), g.BufferDescription((W, H, p.output_stride), dst.data_ptr(), length=dst.numel()))
     q = g.RenderQueue(cp, st, "opencv_fisheye", None, b.input, b.output, depth=2)
+    for bad in (g.BufferDescription((W, H, p.stride), None), g.BufferDescription((W, H, p.stride), 0, length=src.numel())):
+        rc = q._lib.gf_cuda_queue_submit(q._h, 0, 100.0, C.byref(bad.to_c()), C.byref(b.output.to_c()), None, 0)
+        assert rc == -1                                        # no buffer / a null pointer: GF_ERR_BAD_PARAMS, not a failed copy
     q.submit(0, 100.0, b); q.submit(1, 120.0, b)
     with pytest.raises(g.GyroflowCoreError):
         q.submit(2, 140.0, b)                                  # queue full: wait() first
