@@ -25,6 +25,12 @@ class GyroflowCoreError(RuntimeError):
         self.kind = abi.ERRORS.get(code, "Unknown")
 
 
+def check_call(rc, what):
+    """Raise a failed call's code with `what` and the calling thread's last error message (gf_cuda_last_error(NULL))."""
+    if rc != 0:
+        raise GyroflowCoreError(rc, what + ": " + (abi.load_library().gf_cuda_last_error(None) or b"").decode())
+
+
 @dataclass
 class BufferDescription:
     """size = (width, height, stride_bytes); data is a C-contiguous uint8 numpy array (BufferSource::Cpu) or an
@@ -348,8 +354,7 @@ class ComputeParams:
         kp = abi.KernelParams(); rows = C.c_size_t(); fov = C.c_double(); mfov = C.c_double()
         rc = lib.gf_frame_transform_at_timestamp(C.byref(self.c), timestamp_ms, frame, C.byref(kp), m.ctypes.data, rows_max,
                                                  C.byref(rows), C.byref(fov), C.byref(mfov))
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_frame_transform_at_timestamp")
+        check_call(rc, "gf_frame_transform_at_timestamp")
         return kp, m[: rows.value].copy(), fov.value, mfov.value
 
 
@@ -383,8 +388,7 @@ def zoom_fovs(zp: ZoomParams, timestamps_ms, fov_values):
     assert ts.size == v.size
     fovs, minimal = np.zeros_like(v), np.zeros_like(v)
     rc = abi.load_library().gf_zoom_fovs(C.byref(zp.c), ts.ctypes.data, v.ctypes.data, v.size, fovs.ctypes.data, minimal.ctypes.data)
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_zoom_fovs")
+    check_call(rc, "gf_zoom_fovs")
     return fovs, minimal
 
 
@@ -396,8 +400,7 @@ class DeviceGyro:
         self.cp = cp
         h = C.c_void_p()
         rc = self._lib.gf_cuda_gyro_upload(C.byref(h), device, C.byref(cp.c))
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_gyro_upload")
+        check_call(rc, "gf_cuda_gyro_upload")
         self._h = h
 
     def frame_transform(self, timestamp_ms, matrices_dev: int, max_rows: int, frame=0, stream=0, table_flags_dev: int = 0, with_fov=False):
@@ -407,8 +410,7 @@ class DeviceGyro:
         kp = abi.KernelParams(); rows = C.c_size_t(); fov = C.c_double(); mfov = C.c_double()
         rc = self._lib.gf_cuda_frame_transform_dev_flagged(self._h, C.byref(self.cp.c), timestamp_ms, frame, C.byref(kp), matrices_dev, max_rows,
                                                            table_flags_dev or None, C.byref(rows), C.byref(fov), C.byref(mfov), stream or None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_frame_transform_dev")
+        check_call(rc, "gf_cuda_frame_transform_dev")
         return (kp, rows.value, fov.value, mfov.value) if with_fov else (kp, rows.value)
 
     def find_fovs(self, distortion_model: str, digital_lens, timestamps_ms, margin=2.0, stream=0):
@@ -417,8 +419,7 @@ class DeviceGyro:
         out = np.zeros(ts.size, np.float64)
         rc = self._lib.gf_cuda_find_fovs(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
                                          ts.ctypes.data, ts.size, margin, out.ctypes.data, stream or None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_find_fovs")
+        check_call(rc, "gf_cuda_find_fovs")
         return out
 
     def calculate_fovs(self, distortion_model: str, digital_lens, zp: ZoomParams, timestamps_ms, stream=0):
@@ -428,8 +429,7 @@ class DeviceGyro:
         fovs, minimal = np.zeros(ts.size, np.float64), np.zeros(ts.size, np.float64)
         rc = self._lib.gf_cuda_calculate_fovs(self._h, C.byref(self.cp.c), C.byref(zp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
                                               ts.ctypes.data, ts.size, fovs.ctypes.data, minimal.ctypes.data, stream or None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_calculate_fovs")
+        check_call(rc, "gf_cuda_calculate_fovs")
         return fovs, minimal
 
     def undistort_points(self, distortion_model: str, digital_lens, points_xy, timestamp_ms, frame=0, use_fovs=False, lens_correction_amount=1.0):
@@ -438,8 +438,7 @@ class DeviceGyro:
         out = np.zeros_like(pts)
         rc = self._lib.gf_cuda_undistort_points(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
                                                 timestamp_ms, frame, int(use_fovs), lens_correction_amount, pts.ctypes.data, pts.shape[0], out.ctypes.data, None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_undistort_points")
+        check_call(rc, "gf_cuda_undistort_points")
         return out
 
     def generate_stmap(self, distortion_model: str, digital_lens, timestamp_ms, frame=0, per_frame=True):
@@ -448,15 +447,13 @@ class DeviceGyro:
         m, d = abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0
         nw, nh = C.c_int32(), C.c_int32()
         rc = self._lib.gf_cuda_generate_stmap(self._h, C.byref(self.cp.c), m, d, int(per_frame), frame, timestamp_ms, C.byref(nw), C.byref(nh), None, 0, None, 0, None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_generate_stmap (size query)")
+        check_call(rc, "gf_cuda_generate_stmap (size query)")
         w, h = self.cp.c.width, self.cp.c.height
         dist = torch.empty((h, w, 3), dtype=torch.float32, device="cuda")
         und = torch.empty((nh.value, nw.value, 3), dtype=torch.float32, device="cuda")
         rc = self._lib.gf_cuda_generate_stmap(self._h, C.byref(self.cp.c), m, d, int(per_frame), frame, timestamp_ms, C.byref(nw), C.byref(nh),
                                               dist.data_ptr(), dist.numel(), und.data_ptr(), und.numel(), None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, "gf_cuda_generate_stmap")
+        check_call(rc, "gf_cuda_generate_stmap")
         torch.cuda.synchronize()
         return dist.cpu().numpy(), und.cpu().numpy()
 
@@ -473,8 +470,7 @@ class DeviceGyro:
         nw, nh = np.zeros(ts.size, np.int32), np.zeros(ts.size, np.int32)
         rc = self._lib.gf_cuda_stmap_sizes(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
                                            int(per_frame), fr.ctypes.data, ts.ctypes.data, ts.size, nw.ctypes.data, nh.ctypes.data, stream or None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, (self._lib.gf_cuda_last_error(None) or b"").decode())
+        check_call(rc, "gf_cuda_stmap_sizes")
         return nw, nh
 
     def generate_stmaps(self, distortion_model: str, digital_lens, timestamps_ms, frames=None, per_frame=True, stream=None):
@@ -501,8 +497,7 @@ class DeviceGyro:
         up = (C.c_void_p * n)(*[t.data_ptr() for t in bufs])
         rc = self._lib.gf_cuda_generate_stmaps_dev(self._h, C.byref(self.cp.c), m, d, int(per_frame), fr.ctypes.data, ts.ctypes.data, n,
                                                    nw.ctypes.data, nh.ctypes.data, dp, up, w * h * 3, cap, st or None)
-        if rc != 0:
-            raise GyroflowCoreError(rc, (self._lib.gf_cuda_last_error(None) or b"").decode())
+        check_call(rc, "gf_cuda_generate_stmaps_dev")
         undists = [b[: 3 * int(nw[i]) * int(nh[i])].view(int(nh[i]), int(nw[i]), 3) for i, b in enumerate(bufs)]
         return dists, undists
 
@@ -521,16 +516,14 @@ def zoom_dynamic(fov_minimal, window_s, fps, method=1):
     a = np.ascontiguousarray(fov_minimal, dtype=np.float64)
     out = np.zeros_like(a)
     rc = lib.gf_zoom_dynamic_compute(a.ctypes.data, a.size, window_s, fps, method, out.ctypes.data)
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_zoom_dynamic_compute")
+    check_call(rc, "gf_zoom_dynamic_compute")
     return out
 
 
 def scan_tables_dev(matrices_dev: int, matrix_rows: int, table_flags_dev: int, stream: int = 0):
     """Asynchronous: one small kernel on `stream` writes the table's trust verdict (0 = tame, IBIS-free) to the device word."""
     rc = abi.load_library().gf_cuda_scan_tables_dev(matrices_dev, matrix_rows, table_flags_dev, stream or None)
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_cuda_scan_tables_dev")
+    check_call(rc, "gf_cuda_scan_tables_dev")
 
 
 def bind_thread_to_device(device: int) -> int:
@@ -541,14 +534,12 @@ def bind_thread_to_device(device: int) -> int:
 def host_register(arr: np.ndarray):
     """Page-lock a host array in place (gf_cuda_host_register); pair with host_unregister before the array is freed."""
     rc = abi.load_library().gf_cuda_host_register(arr.ctypes.data, arr.nbytes)
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_cuda_host_register")
+    check_call(rc, "gf_cuda_host_register")
 
 
 def host_unregister(arr: np.ndarray):
     rc = abi.load_library().gf_cuda_host_unregister(arr.ctypes.data)
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_cuda_host_unregister")
+    check_call(rc, "gf_cuda_host_unregister")
 
 
 def stab_config(params: abi.KernelParams, pixel_type: str, digital_lens=None, base_flags=0, background=(0.0, 0.0, 0.0, 0.0),
@@ -573,6 +564,5 @@ def get_frame_transform_at(stab: abi.StabConfig, cp: ComputeParams, buffers: Buf
     m = None if mesh is None else np.ascontiguousarray(mesh, dtype=np.float32)
     rc = abi.load_library().gf_get_frame_transform_at(C.byref(stab), C.byref(cp.c), C.byref(i), C.byref(o), m.ctypes.data if m is not None and m.size else None,
                                                       m.size if m is not None else 0, float(timestamp_ms), frame, minimal_fov, C.byref(kernel_params))
-    if rc != 0:
-        raise GyroflowCoreError(rc, "gf_get_frame_transform_at")
+    check_call(rc, "gf_get_frame_transform_at")
     return kernel_params

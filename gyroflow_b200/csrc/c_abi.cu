@@ -804,20 +804,8 @@ __global__ void stmap_rgb_kernel(const uint2* __restrict__ coords, int w, int h,
 
 namespace {
 
-// The coordinate-mode warp context of the undistort map (LUMA8, bilinear, pass 1 only) for maps of up to max_w x max_h, with a
-// table slot of max(max_w, max_h) rows.  `any_dev`: a device pointer for the buffer description validation wants (coordinate mode
-// never dereferences it).
-int create_stmap_ctx(int device, int lens, int digital, int max_w, int max_h, void* any_dev, gf_cuda_ctx** out) {
-    gf_kernel_params kq; memset(&kq, 0, sizeof(kq));
-    kq.width = kq.output_width = kq.stride = kq.output_stride = max_w; kq.height = kq.output_height = max_h;
-    kq.matrix_count = 1; kq.interpolation = GF_INTERP_BILINEAR; kq.bytes_per_pixel = 1; kq.pix_element_count = 1;
-    gf_buffer_desc d; memset(&d, 0, sizeof(d));
-    d.width = max_w; d.height = max_h; d.stride = max_w; d.kind = GF_BUF_DEVICE; d.ptr = any_dev; d.len = (size_t)max_w * (size_t)max_h;
-    return gf_cuda_create(out, device, &kq, GF_PIX_LUMA8, lens, digital, &d, &d, 0);
-}
-
 // Both maps of one frame, enqueued on `st` without waiting — stmap.rs:73-116.  `cp`: stmap_params of the user's ComputeParams.  `ctx`:
-// a context of create_stmap_ctx at least new_w x new_h; it is set to this frame's size.
+// the gyro's ST-map context, at least new_w x new_h; it is set to this frame's size.
 int enqueue_stmap_frame(gf_cuda_ctx* ctx, gf_cuda_gyro* g, gf_compute_params cp, int distortion_model, int digital_lens, size_t frame,
                         double timestamp_ms, int new_w, int new_h, float* dist_rgb_dev, float* undist_rgb_dev, cudaStream_t st) {
     const int width = cp.width, height = cp.height;
@@ -828,7 +816,7 @@ int enqueue_stmap_frame(gf_cuda_ctx* ctx, gf_cuda_gyro* g, gf_compute_params cp,
     std::vector<float> mats(max_rows * GF_MATRIX_STRIDE);
     size_t rows = 0;
     int rc = gf_frame_transform_at_timestamp(&cp, timestamp_ms, frame, &kp, mats.data(), max_rows, &rows, nullptr, nullptr);   // :79
-    if (rc != GF_OK) return fail(nullptr, rc, "gf_frame_transform_at_timestamp failed");
+    if (rc != GF_OK) return rc;
     kp.width = new_w; kp.height = new_h; kp.output_width = new_w; kp.output_height = new_h;   // :80-84
     kp.flags = (digital_lens != GF_LENS_NONE ? GF_FLAG_HAS_DIGITAL_LENS : 0) | (cp.readout_horizontal ? GF_FLAG_HORIZONTAL_RS : 0);
     // The closure of :88-109 is undistort_coord's row selection + rotate_and_distort and nothing else: run the warp kernel in
@@ -856,60 +844,17 @@ int enqueue_stmap_frame(gf_cuda_ctx* ctx, gf_cuda_gyro* g, gf_compute_params cp,
     return gf_cuda_stmap_distort_dev(g, &cp, distortion_model, digital_lens, timestamp_ms, frame, dist_rgb_dev, st);
 }
 
-} // namespace
-
-extern "C" {
-
-GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
-                                  int per_frame, size_t frame, double timestamp_ms, int32_t* out_new_width, int32_t* out_new_height,
-                                  float* dist_rgb_dev, size_t dist_capacity_floats, float* undist_rgb_dev, size_t undist_capacity_floats,
-                                  void* cu_stream) {
-    if (!g || !cp_user || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    int rc = gf_cuda_stmap_sizes(g, cp_user, distortion_model, digital_lens, per_frame, &frame, &timestamp_ms, 1, out_new_width, out_new_height, cu_stream);
-    if (rc != GF_OK) return rc;
-    if (!dist_rgb_dev || !undist_rgb_dev) return GF_OK;                                      // size query
-    const int new_w = *out_new_width, new_h = *out_new_height;
-    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
-    if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < (size_t)new_w * new_h * 3)
-        return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "ST map output buffers too small");
-    gf_cuda_ctx* raw = nullptr;
-    if ((rc = create_stmap_ctx(g->device, distortion_model, digital_lens, new_w, new_h, undist_rgb_dev, &raw)) != GF_OK) return rc;
-    const std::unique_ptr<gf_cuda_ctx, Deleter<gf_cuda_destroy>> ctx(raw);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
-    if ((rc = enqueue_stmap_frame(ctx.get(), g, cp, distortion_model, digital_lens, frame, timestamp_ms, new_w, new_h, dist_rgb_dev, undist_rgb_dev, st)) != GF_OK)
-        return rc;
-    CK(nullptr, cudaStreamSynchronize(st));
-    return GF_OK;
-}
-
-GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens, int per_frame,
-                                       const size_t* frames, const double* timestamps_ms, size_t n,
-                                       const int32_t* new_w, const int32_t* new_h, float* const* dist_rgb_dev, float* const* undist_rgb_dev,
-                                       size_t dist_capacity_floats, size_t undist_capacity_floats, void* cu_stream) {
-    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    if (n == 0) return GF_OK;
-    if (!frames || !timestamps_ms || !new_w || !new_h || !dist_rgb_dev || !undist_rgb_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
-    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall");
-    Combo combo;
-    if (!make_combo(GF_PIX_LUMA8, distortion_model, digital_lens, GF_INTERP_BILINEAR, &combo) || !combo.kernels[KV_GENERAL] ||
-        !point_path_supported(distortion_model, digital_lens))
-        return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "no ST-map kernels for this (lens, digital lens) pair");
-    // every argument is checked before the first launch
+// An ST-map job of n frames whose arguments have been checked: both maps of every frame, enqueued on `st` in the gyro's coordinate-mode
+// warp context.
+int stmap_job(gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, int digital_lens, const size_t* frames,
+              const double* timestamps_ms, size_t n, const int32_t* new_w, const int32_t* new_h, float* const* dist_rgb_dev,
+              float* const* undist_rgb_dev, cudaStream_t st) {
     int max_w = 0, max_h = 0;
     size_t max_px = 0;
     for (size_t i = 0; i < n; ++i) {
-        const std::string at = " at entry " + std::to_string(i);
-        if (!dist_rgb_dev[i] || !undist_rgb_dev[i]) return fail(nullptr, GF_ERR_BAD_PARAMS, "null map buffer" + at);
-        if (!stmap_size_ok(new_w[i], new_h[i])) return fail(nullptr, GF_ERR_SIZE_MISMATCH, "ST map: undistorted frame size out of range" + at);
-        if (new_w[i] > 16384) return fail(nullptr, GF_ERR_BAD_PARAMS, "ST map: undistorted width beyond the warp's 16384" + at);
-        const size_t px = (size_t)new_w[i] * (size_t)new_h[i];
-        if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < px * 3)
-            return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "ST map output buffers too small" + at);
-        max_w = std::max(max_w, new_w[i]); max_h = std::max(max_h, new_h[i]); max_px = std::max(max_px, px);
+        max_w = std::max(max_w, new_w[i]); max_h = std::max(max_h, new_h[i]); max_px = std::max(max_px, (size_t)new_w[i] * (size_t)new_h[i]);
     }
     CK(nullptr, cudaSetDevice(g->device));
-    const cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
     if (!g->stmap_done) CK(nullptr, create_event(g->stmap_done));
     // The context is the previous job's: this stream waits for that job on the device.  A context too small or of another lens pair is
     // replaced, which waits for the previous job on the host.
@@ -918,8 +863,15 @@ GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params*
         g->stmap_ctx->max_rows < (size_t)std::max(max_w, max_h)) {
         CK(nullptr, cudaEventSynchronize(g->stmap_done.get()));
         g->stmap_ctx.reset();
+        // LUMA8, bilinear, pass 1 only, for maps of up to max_w x max_h: a table slot of max(max_w, max_h) rows.  The buffer description
+        // is for gf_cuda_create's validation, which wants a device pointer (coordinate mode never dereferences it).
+        gf_kernel_params kq; memset(&kq, 0, sizeof(kq));
+        kq.width = kq.output_width = kq.stride = kq.output_stride = max_w; kq.height = kq.output_height = max_h;
+        kq.matrix_count = 1; kq.interpolation = GF_INTERP_BILINEAR; kq.bytes_per_pixel = 1; kq.pix_element_count = 1;
+        gf_buffer_desc d; memset(&d, 0, sizeof(d));
+        d.width = max_w; d.height = max_h; d.stride = max_w; d.kind = GF_BUF_DEVICE; d.ptr = undist_rgb_dev[0]; d.len = (size_t)max_w * (size_t)max_h;
         gf_cuda_ctx* raw = nullptr;
-        const int rc = create_stmap_ctx(g->device, distortion_model, digital_lens, max_w, max_h, undist_rgb_dev[0], &raw);
+        const int rc = gf_cuda_create(&raw, g->device, &kq, GF_PIX_LUMA8, distortion_model, digital_lens, &d, &d, 0);
         if (rc != GF_OK) return rc;
         g->stmap_ctx.reset(raw);
     }
@@ -931,6 +883,56 @@ GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params*
                                  dist_rgb_dev[i], undist_rgb_dev[i], st);
     CK(nullptr, cudaEventRecord(g->stmap_done.get(), st));    // also after a failure: whatever was enqueued still uses the context
     return rc;
+}
+
+} // namespace
+
+extern "C" {
+
+GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
+                                  int per_frame, size_t frame, double timestamp_ms, int32_t* out_new_width, int32_t* out_new_height,
+                                  float* dist_rgb_dev, size_t dist_capacity_floats, float* undist_rgb_dev, size_t undist_capacity_floats,
+                                  void* cu_stream) {
+    if (!g || !cp_user || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmap: null argument");
+    int rc = gf_cuda_stmap_sizes(g, cp_user, distortion_model, digital_lens, per_frame, &frame, &timestamp_ms, 1, out_new_width, out_new_height, cu_stream);
+    if (rc != GF_OK) return rc;
+    if (!dist_rgb_dev || !undist_rgb_dev) return GF_OK;                                      // size query
+    const int new_w = *out_new_width, new_h = *out_new_height;
+    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
+    if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < (size_t)new_w * new_h * 3)
+        return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "gf_cuda_generate_stmap: ST map output buffers too small");
+    if (new_w > 16384) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmap: undistorted width beyond the warp's 16384");
+    if (!gf_combo_supported(GF_PIX_LUMA8, distortion_model, digital_lens, GF_INTERP_BILINEAR))           // the warp renders the undistort map
+        return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_generate_stmap: no warp kernel for this (lens, digital lens) pair");
+    const cudaStream_t st = g->stream_of(cu_stream);
+    if ((rc = stmap_job(g, cp, distortion_model, digital_lens, &frame, &timestamp_ms, 1, out_new_width, out_new_height, &dist_rgb_dev, &undist_rgb_dev, st)) != GF_OK)
+        return rc;
+    CK(nullptr, cudaStreamSynchronize(st));
+    return GF_OK;
+}
+
+GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens, int per_frame,
+                                       const size_t* frames, const double* timestamps_ms, size_t n,
+                                       const int32_t* new_w, const int32_t* new_h, float* const* dist_rgb_dev, float* const* undist_rgb_dev,
+                                       size_t dist_capacity_floats, size_t undist_capacity_floats, void* cu_stream) {
+    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmaps_dev: null argument");
+    if (n == 0) return GF_OK;
+    if (!frames || !timestamps_ms || !new_w || !new_h || !dist_rgb_dev || !undist_rgb_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmaps_dev: null argument");
+    const gf_compute_params cp = stmap_params(*cp_user, per_frame);
+    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "gf_cuda_generate_stmaps_dev: SizeTooSmall");
+    if (!gf_combo_supported(GF_PIX_LUMA8, distortion_model, digital_lens, GF_INTERP_BILINEAR) || !point_path_supported(distortion_model, digital_lens))
+        return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_generate_stmaps_dev: no ST-map kernels for this (lens, digital lens) pair");
+    // every argument is checked before the first launch
+    for (size_t i = 0; i < n; ++i) {
+        const std::string at = " at entry " + std::to_string(i);
+        if (!dist_rgb_dev[i] || !undist_rgb_dev[i]) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmaps_dev: null map buffer" + at);
+        if (!stmap_size_ok(new_w[i], new_h[i])) return fail(nullptr, GF_ERR_SIZE_MISMATCH, "gf_cuda_generate_stmaps_dev: undistorted frame size out of range" + at);
+        if (new_w[i] > 16384) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_generate_stmaps_dev: undistorted width beyond the warp's 16384" + at);
+        if (dist_capacity_floats < (size_t)cp.width * cp.height * 3 || undist_capacity_floats < (size_t)new_w[i] * (size_t)new_h[i] * 3)
+            return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "gf_cuda_generate_stmaps_dev: ST map output buffers too small" + at);
+    }
+    return stmap_job(g, cp, distortion_model, digital_lens, frames, timestamps_ms, n, new_w, new_h, dist_rgb_dev, undist_rgb_dev,
+                     g->stream_of(cu_stream));
 }
 
 GF_API int gf_cuda_undistort_planes_dev(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out,

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cfloat>
 #include "../../include/gyroflow_cuda.h"
+#include "c_abi_internal.h"
 
 namespace {
 
@@ -40,9 +41,9 @@ void get_rect(const gf_buffer_desc* d, int32_t (&r)[4]) {                      /
 
 extern "C" GF_API int gf_get_frame_transform_at(const gf_stab_config* st, const gf_compute_params* cp, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                                 const float* mesh, size_t mesh_len, double timestamp_ms, size_t frame, double minimal_fov, gf_kernel_params* kp) {
-    if (!st || !cp || !in || !out || !kp) return GF_ERR_BAD_PARAMS;
+    if (!st || !cp || !in || !out || !kp) return gf::fail(nullptr, GF_ERR_BAD_PARAMS, "gf_get_frame_transform_at: null argument");
     int count = 0, sbytes = 0; float maxv = 0.0f; bool has_max = false;
-    if (!pixel_info(st->pixel_type, &count, &sbytes, &maxv, &has_max)) return GF_ERR_BAD_PARAMS;
+    if (!pixel_info(st->pixel_type, &count, &sbytes, &maxv, &has_max)) return gf::fail(nullptr, GF_ERR_BAD_PARAMS, "gf_get_frame_transform_at: unknown pixel type");
 
     kp->pixel_value_limit = has_max ? maxv : FLT_MAX;                           // :258 T::default_max_value().unwrap_or(f32::MAX)
     kp->max_pixel_value   = has_max ? maxv : 1.0f;                              // :259

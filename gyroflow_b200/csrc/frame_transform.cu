@@ -305,7 +305,7 @@ GF_API int gf_keyframe_value_at(const gf_keyframe_track* track, double timestamp
 GF_API int gf_frame_transform_at_timestamp(const gf_compute_params* cp, double timestamp_ms, size_t frame,
                                            gf_kernel_params* out_params, float* out_matrices, size_t max_rows,
                                            size_t* out_rows, double* out_fov, double* out_minimal_fov) {
-    if (!cp || !out_matrices) return GF_ERR_BAD_PARAMS;
+    if (!cp || !out_matrices) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_frame_transform_at_timestamp: null argument");
     RowCtx C;
     StabSplines sp; memset(&sp, 0, sizeof(sp));
     if (cp->camera_stab && frame < cp->n_camera_stab) {
@@ -314,7 +314,7 @@ GF_API int gf_frame_transform_at_timestamp(const gf_compute_params* cp, double t
     }
     const size_t rows = prepare(cp, timestamp_ms, frame, &sp, C, out_params, out_fov, out_minimal_fov);
     if (out_rows) *out_rows = rows;
-    if (rows > max_rows) return GF_ERR_BUFFER_TOO_SMALL;
+    if (rows > max_rows) return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "gf_frame_transform_at_timestamp: max_rows below the frame's matrix rows");
     for (size_t y = 0; y < rows; ++y) frame_row(C, y, out_matrices + y * GF_MATRIX_STRIDE);       // rayon par_iter in the reference (:249)
     return GF_OK;
 }
@@ -327,7 +327,7 @@ GF_API uint32_t gf_table_flags_host(const float* matrices, size_t rows) {
 }
 
 GF_API int gf_cuda_gyro_upload(gf_cuda_gyro** out, int device, const gf_compute_params* cp) {
-    if (!out || !cp || !cp->org.ts_us || !cp->org.quats) return GF_ERR_BAD_PARAMS;
+    if (!out || !cp || !cp->org.ts_us || !cp->org.quats) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_gyro_upload: null argument");
     *out = nullptr;
     CK(nullptr, cudaSetDevice(device));
     std::unique_ptr<gf_cuda_gyro, Deleter<gf_cuda_gyro_free>> g(new gf_cuda_gyro());
@@ -392,7 +392,7 @@ GF_API void gf_cuda_gyro_free(gf_cuda_gyro* g) {
 GF_API int gf_cuda_frame_transform_dev_flagged(gf_cuda_gyro* g, const gf_compute_params* cp, double timestamp_ms, size_t frame,
                                                gf_kernel_params* out_params, float* matrices_dev, size_t max_rows, uint32_t* table_flags_dev,
                                                size_t* out_rows, double* out_fov, double* out_minimal_fov, void* cu_stream) {
-    if (!g || !cp || !matrices_dev) return GF_ERR_BAD_PARAMS;
+    if (!g || !cp || !matrices_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_frame_transform_dev_flagged: null argument");
     CK(nullptr, cudaSetDevice(g->device));
     RowCtx C;
     // the two per-frame lookups (org(ts), smoothed(ts)) stay on the host: O(log n) each; the per-row ones run on the device
@@ -400,10 +400,10 @@ GF_API int gf_cuda_frame_transform_dev_flagged(gf_cuda_gyro* g, const gf_compute
     const bool has_stab = g->frame_splines(frame, sp);
     const size_t rows = prepare(cp, timestamp_ms, frame, has_stab ? &sp : nullptr, C, out_params, out_fov, out_minimal_fov);
     if (out_rows) *out_rows = rows;
-    if (rows > max_rows) return GF_ERR_BUFFER_TOO_SMALL;
+    if (rows > max_rows) return fail(nullptr, GF_ERR_BUFFER_TOO_SMALL, "gf_cuda_frame_transform_dev_flagged: max_rows below the frame's matrix rows");
     C.org = g->org_track();
     C.offsets = g->sync_offsets(cp->gyro_offset_ms);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    const cudaStream_t st = g->stream_of(cu_stream);
     unsigned* scratch = g->d_scratch.ptr + 2u * (g->next_scratch++ % gf_cuda_gyro::kScratchPairs);     // self-cleaning: the last block re-arms it
     frame_rows_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(C, rows, matrices_dev, table_flags_dev, scratch);
     CK(nullptr, cudaGetLastError());

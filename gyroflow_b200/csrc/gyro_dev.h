@@ -22,10 +22,13 @@ struct gf_cuda_gyro {
     static constexpr unsigned kScratchPairs = 64;
     gf::GrowBuf<unsigned> d_scratch; unsigned next_scratch = 0;
     gf::Stream stream;
-    // ST-map jobs (gf_cuda_generate_stmaps_dev): the coordinate-mode warp context they share, and the end of the last job on its stream
+    // ST-map jobs (gf_cuda_generate_stmaps_dev, and gf_cuda_generate_stmap as a job of one frame): the coordinate-mode warp context they
+    // share, kept from job to job, and the end of the last job on its stream
     std::unique_ptr<gf_cuda_ctx, gf::Deleter<gf_cuda_destroy>> stmap_ctx;
     gf::Event stmap_done;
 
+    // the stream of a call: the caller's `cu_stream`, or this object's own when it is NULL
+    cudaStream_t stream_of(void* cu_stream) const { return cu_stream ? (cudaStream_t)cu_stream : stream.get(); }
     gf::Track org_track() const { return gf::Track{ d_org_ts.ptr, d_org_q.ptr, n_org }; }
     // the uploaded multi-point sync offsets; `scalar_ms` (gyro_offset_ms) applies when there are none
     gf::SyncOffsets sync_offsets(double scalar_ms) const { return gf::SyncOffsets{ d_off_ts.ptr, d_off_ms.ptr, n_offsets, scalar_ms }; }

@@ -232,17 +232,17 @@ __global__ void __launch_bounds__(128) points_kernel(const ZoomArgs A, const Zoo
     if (pts) { out[2 * i] = ox; out[2 * i + 1] = oy; }
     else     { out[3 * i] = ox / (float)grid_w; out[3 * i + 1] = 1.0f - (oy / (float)grid_h); out[3 * i + 2] = 0.0f; }
 }
-// One frame of gf_cuda_stmap_sizes: what gf_cuda_undistort_points derives for it.  The lens may change per frame (lens_per_frame), so
-// the call-wide values are per frame here.
-struct StmapFrame { ZoomArgs A; ZoomFrame F; };
+// What gf_cuda_undistort_points derives for one frame (point_frame).  The lens may change per frame (lens_per_frame), so in a call over
+// several frames (gf_cuda_stmap_sizes) the call-wide values are per frame.
+struct PointFrame { ZoomArgs A; ZoomFrame F; };
 
 // The undistorted size of one frame per CTA — stmap.rs:58-77: the 120 points_around_rect(w, h, 31, 31) edge points with margin 0
 // (fov_iterative.rs:154-175) through undistort_points, their bounding box folded in order from 0 with f32::min / max (NaN is
 // ignored, :62-71), then `ceil(max - min) as usize` for each extent.
 template <int LENS, int DIGITAL>
-__global__ void __launch_bounds__(128) stmap_size_kernel(const StmapFrame* __restrict__ frames, float w, float h, int2* __restrict__ out) {
+__global__ void __launch_bounds__(128) stmap_size_kernel(const PointFrame* __restrict__ frames, float w, float h, int2* __restrict__ out) {
     __shared__ float und[2 * RECT_POINTS];
-    const StmapFrame& S = frames[blockIdx.x];
+    const PointFrame& S = frames[blockIdx.x];
     const int tid = threadIdx.x;
     if (tid < RECT_POINTS) {
         float x, y; rect_point(w, h, 0.0f, tid, x, y);
@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(128) stmap_size_kernel(const StmapFrame* __res
 struct ZoomKernels {
     void (*find_fov)(const ZoomArgs, const ZoomFrame*, double*);
     void (*points)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
-    void (*stmap_size)(const StmapFrame*, float, float, int2*);
+    void (*stmap_size)(const PointFrame*, float, float, int2*);
 };
 template <int LENS, int DIGITAL> ZoomKernels kernels_of() { return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL> }; }
 template <int LENS> ZoomKernels pick_digital(int digital) {
@@ -353,15 +353,20 @@ static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& 
     f.out_fx = A.kp.f[0] / A.fov / f.factor; f.out_fy = A.kp.f[1] / A.fov / f.factor;
     return f;
 }
-// get_lens_data_at_timestamp of this frame (frame_transform.rs:360) for ONE timestamp: the per-frame lens in a private copy of `cp`
-static gf_compute_params resolve_point_lens(const gf_compute_params& cp, size_t frame) {
-    gf_compute_params r = cp;
-    if (cp.lens_per_frame && frame < cp.n_lens_per_frame) {
-        const gf_lens_data& L = cp.lens_per_frame[frame];
-        memcpy(r.camera_matrix, L.camera_matrix, sizeof(r.camera_matrix)); memcpy(r.distortion_coeffs, L.distortion_coeffs, sizeof(r.distortion_coeffs));
-        r.radial_distortion_limit = L.radial_distortion_limit;
+// One frame of undistort_points at `timestamp_ms`: its lens, fov (get_fov with `use_fovs`), call-wide values and uniforms.  The lens is
+// get_lens_data_at_timestamp of this frame (frame_transform.rs:360) for ONE timestamp: the per-frame lens in a private copy of `cp_user`.
+static PointFrame point_frame(const gf_cuda_gyro* g, const gf_compute_params& cp_user, int distortion_model, size_t frame, double timestamp_ms,
+                              bool use_fovs, double lens_correction_amount) {
+    gf_compute_params cp = cp_user;
+    if (cp_user.lens_per_frame && frame < cp_user.n_lens_per_frame) {
+        const gf_lens_data& L = cp_user.lens_per_frame[frame];
+        memcpy(cp.camera_matrix, L.camera_matrix, sizeof(cp.camera_matrix)); memcpy(cp.distortion_coeffs, L.distortion_coeffs, sizeof(cp.distortion_coeffs));
+        cp.radial_distortion_limit = L.radial_distortion_limit;
     }
-    return r;
+    PointFrame p;
+    setup_points_args(g, cp, distortion_model, points_fov(&cp, frame, use_fovs, timestamp_ms), p.A);
+    p.F = frame_uniforms(g, cp, p.A, timestamp_ms, frame, lens_correction_amount, false);
+    return p;
 }
 
 bool gf::point_path_supported(int lens, int digital) { return pick_kernels(lens, digital).points != nullptr; }
@@ -421,10 +426,10 @@ extern "C" {
 // zooming/mod.rs:41-49) are applied here.
 GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
                              const double* timestamps_ms, size_t n, float fov_algorithm_margin, double* out_fov_minimal, void* cu_stream) {
-    if (!g || !cp_user || !timestamps_ms || !out_fov_minimal) return GF_ERR_BAD_PARAMS;
+    if (!g || !cp_user || !timestamps_ms || !out_fov_minimal) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_find_fovs: null argument");
     if (n == 0) return GF_OK;
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.find_fov) return GF_ERR_UNSUPPORTED_COMBO;
+    if (!k.find_fov) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_find_fovs: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
     gf_compute_params cp = *cp_user;
     const int org_ow = cp.output_width, org_oh = cp.output_height;
@@ -440,7 +445,7 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
     // per-frame uniforms on the host: two O(log n) lookups per frame
     std::vector<ZoomFrame> hf(n);
     for (size_t i = 0; i < n; ++i) hf[i] = frame_uniforms(g, cp, A, timestamps_ms[i], i, cp.lens_correction_amount, true);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    const cudaStream_t st = g->stream_of(cu_stream);
     GrowBuf<ZoomFrame> d_frames; GrowBuf<double> d_out;
     CK(nullptr, d_frames.reserve(n, st));
     CK(nullptr, d_out.reserve(n, st));
@@ -456,23 +461,18 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
 GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
                                     double timestamp_ms, size_t frame, int use_fovs, double lens_correction_amount,
                                     const float* points_xy, size_t n, float* out_xy, void* cu_stream) {
-    if (!g || !cp_user || !points_xy || !out_xy) return GF_ERR_BAD_PARAMS;
+    if (!g || !cp_user || !points_xy || !out_xy) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_points: null argument");
     if (n == 0) return GF_OK;
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
+    if (!k.points) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_undistort_points: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
-    ZoomArgs A;
-    const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
-    const gf_compute_params* cp = &rcp;
-    const double fov = points_fov(cp, frame, use_fovs != 0, timestamp_ms);
-    setup_points_args(g, *cp, distortion_model, fov, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, lens_correction_amount, false);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
+    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, use_fovs != 0, lens_correction_amount);
+    const cudaStream_t st = g->stream_of(cu_stream);
     GrowBuf<float2> d_in; GrowBuf<float> d_out;
     CK(nullptr, d_in.reserve(n, st));
     CK(nullptr, d_out.reserve(n * 2, st));
     CK(nullptr, cudaMemcpyAsync(d_in.ptr, points_xy, n * sizeof(float2), cudaMemcpyHostToDevice, st));
-    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, d_in.ptr, n, 0, 0, d_out.ptr);
+    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(p.A, p.F, d_in.ptr, n, 0, 0, d_out.ptr);
     CK(nullptr, cudaGetLastError());
     CK(nullptr, cudaMemcpyAsync(out_xy, d_out.ptr, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
     CK(nullptr, cudaStreamSynchronize(st));
@@ -483,20 +483,15 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
 // device memory as RGB f32 (x / width, 1 - y / height, 0).  Asynchronous on the stream.
 GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
                                      double timestamp_ms, size_t frame, float* out_rgb_dev, void* cu_stream) {
-    if (!g || !cp_user || !out_rgb_dev) return GF_ERR_BAD_PARAMS;
+    if (!g || !cp_user || !out_rgb_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_distort_dev: null argument");
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.points) return GF_ERR_UNSUPPORTED_COMBO;
-    const gf_compute_params rcp = resolve_point_lens(*cp_user, frame);
-    const gf_compute_params* cp = &rcp;
-    if (cp->width < 1 || cp->height < 1) return GF_ERR_BAD_PARAMS;
+    if (!k.points) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_distort_dev: no point-path kernel for this (lens, digital lens) pair");
+    const int w = cp_user->width, h = cp_user->height;
+    if (w < 1 || h < 1) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_distort_dev: frame size < 1");
     CK(nullptr, cudaSetDevice(g->device));
-    ZoomArgs A;
-    const double fov = points_fov(cp, frame, true, timestamp_ms);
-    setup_points_args(g, *cp, distortion_model, fov, A);
-    const ZoomFrame F = frame_uniforms(g, *cp, A, timestamp_ms, frame, 1.0, false);
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
-    const size_t n = (size_t)cp->width * (size_t)cp->height;
-    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(A, F, nullptr, n, cp->width, cp->height, out_rgb_dev);
+    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, true, 1.0);
+    const size_t n = (size_t)w * (size_t)h;
+    k.points<<<(unsigned)((n + 127) / 128), 128, 0, g->stream_of(cu_stream)>>>(p.A, p.F, nullptr, n, w, h, out_rgb_dev);
     CK(nullptr, cudaGetLastError());
     return GF_OK;
 }
@@ -506,26 +501,22 @@ GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* c
 GF_API int gf_cuda_stmap_sizes(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens, int per_frame,
                                const size_t* frames, const double* timestamps_ms, size_t n,
                                int32_t* out_new_width, int32_t* out_new_height, void* cu_stream) {
-    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
+    if (!g || !cp_user) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_sizes: null argument");
     if (n == 0) return GF_OK;
-    if (!frames || !timestamps_ms || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    if (n > 0x7fffffffu) return fail(nullptr, GF_ERR_BAD_PARAMS, "too many frames");
+    if (!frames || !timestamps_ms || !out_new_width || !out_new_height) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_sizes: null argument");
+    if (n > 0x7fffffffu) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_sizes: too many frames");
     const gf_compute_params cp = stmap_params(*cp_user, per_frame);
-    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "SizeTooSmall");
+    if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "gf_cuda_stmap_sizes: SizeTooSmall");
     const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.stmap_size) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "no point-path kernel for this (lens, digital lens) pair");
+    if (!k.stmap_size) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_sizes: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
-    std::vector<StmapFrame> hf(n);
-    for (size_t i = 0; i < n; ++i) {
-        const gf_compute_params rcp = resolve_point_lens(cp, frames[i]);
-        setup_points_args(g, rcp, distortion_model, points_fov(&rcp, frames[i], false, timestamps_ms[i]), hf[i].A);
-        hf[i].F = frame_uniforms(g, rcp, hf[i].A, timestamps_ms[i], frames[i], 1.0, false);
-    }
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : g->stream.get();
-    GrowBuf<StmapFrame> d_frames; GrowBuf<int2> d_out;
+    std::vector<PointFrame> hf(n);
+    for (size_t i = 0; i < n; ++i) hf[i] = point_frame(g, cp, distortion_model, frames[i], timestamps_ms[i], false, 1.0);
+    const cudaStream_t st = g->stream_of(cu_stream);
+    GrowBuf<PointFrame> d_frames; GrowBuf<int2> d_out;
     CK(nullptr, d_frames.reserve(n, st));
     CK(nullptr, d_out.reserve(n, st));
-    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(StmapFrame), cudaMemcpyHostToDevice, st));
+    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(PointFrame), cudaMemcpyHostToDevice, st));
     k.stmap_size<<<(unsigned)n, 128, 0, st>>>(d_frames.ptr, (float)cp.width, (float)cp.height, d_out.ptr);
     CK(nullptr, cudaGetLastError());
     std::vector<int2> sizes(n);
@@ -537,26 +528,27 @@ GF_API int gf_cuda_stmap_sizes(gf_cuda_gyro* g, const gf_compute_params* cp_user
         if (bad == n && !stmap_size_ok(sizes[i].x, sizes[i].y)) bad = i;
     }
     if (bad < n)
-        return fail(nullptr, GF_ERR_SIZE_MISMATCH, "ST map: undistorted frame size out of range: " + std::to_string(sizes[bad].x) + "x" +
+        return fail(nullptr, GF_ERR_SIZE_MISMATCH, "gf_cuda_stmap_sizes: undistorted frame size out of range: " + std::to_string(sizes[bad].x) + "x" +
                     std::to_string(sizes[bad].y) + " at entry " + std::to_string(bad) + " (frame " + std::to_string(frames[bad]) + ")");
     return GF_OK;
 }
 
 // zoom_dynamic::compute, static-window branch (zoom_dynamic.rs:56-76): sequential 1-D filters, stays on the host like in the reference
 GF_API int gf_zoom_dynamic_compute(const double* fov_minimal, size_t n, double window_s, double fps, int method, double* out) {
-    if (!fov_minimal || !out) return GF_ERR_BAD_PARAMS;
+    if (!fov_minimal || !out) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_dynamic_compute: null argument");
     if (n == 0) return GF_OK;
     std::vector<double> v(fov_minimal, fov_minimal + n);
-    if (!zoom_static_window(v, window_s, fps, method)) return GF_ERR_BAD_PARAMS;
+    if (!zoom_static_window(v, window_s, fps, method)) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_dynamic_compute: zoom window longer than 1e8 frames");
     memcpy(out, v.data(), n * sizeof(double));
     return GF_OK;
 }
 
 GF_API int gf_zoom_fovs(const gf_zoom_params* zp, const double* timestamps_ms, const double* fov_values, size_t n,
                         double* out_fovs, double* out_minimal_fovs) {
-    if (!zp) return GF_ERR_BAD_PARAMS;
+    if (!zp) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_fovs: null argument");
     if (n == 0) return GF_OK;                                        // calculate_fovs returns empty vectors (zooming/mod.rs:36-38)
-    if (!timestamps_ms || !fov_values || !out_fovs || !out_minimal_fovs || (zp->n_trim_ranges && !zp->trim_ranges)) return GF_ERR_BAD_PARAMS;
+    if (!timestamps_ms || !fov_values || !out_fovs || !out_minimal_fovs || (zp->n_trim_ranges && !zp->trim_ranges))
+        return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_fovs: null argument");
     std::vector<double> v(fov_values, fov_values + n);
     // Trim ranges (fov_iterative.rs:59-69) come before the mode branch, so the minimal FOVs of a trimmed clip carry the max-FOV fill.
     if (zp->n_trim_ranges > 0) {
@@ -597,10 +589,10 @@ GF_API int gf_zoom_fovs(const gf_zoom_params* zp, const double* timestamps_ms, c
         } else {
             // get_frames_per_window reads the global adaptive_zoom_window, not the frame's window (zoom_dynamic.rs:31): every frame has the
             // static window, so min_rolling_dynamic / convolve_dynamic (:129-163) are the static min_rolling / convolve.
-            if (!zoom_static_window(v, window, fps, 0)) return GF_ERR_BAD_PARAMS;
+            if (!zoom_static_window(v, window, fps, 0)) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_fovs: zoom window longer than 1e8 frames");
         }
     } else if (!zoom_static_window(v, window, fps, zp->adaptive_zoom_method)) {                    // static window (zoom_dynamic.rs:56-76)
-        return GF_ERR_BAD_PARAMS;
+        return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_zoom_fovs: zoom window longer than 1e8 frames");
     }
     memcpy(out_fovs, v.data(), n * sizeof(double));
     memcpy(out_minimal_fovs, minimal.data(), n * sizeof(double));
@@ -609,7 +601,7 @@ GF_API int gf_zoom_fovs(const gf_zoom_params* zp, const double* timestamps_ms, c
 
 GF_API int gf_cuda_calculate_fovs(gf_cuda_gyro* g, const gf_compute_params* cp, const gf_zoom_params* zp, int distortion_model, int digital_lens,
                                   const double* timestamps_ms, size_t n, double* out_fovs, double* out_minimal_fovs, void* cu_stream) {
-    if (!g || !cp || !zp || !timestamps_ms || !out_fovs || !out_minimal_fovs) return GF_ERR_BAD_PARAMS;
+    if (!g || !cp || !zp || !timestamps_ms || !out_fovs || !out_minimal_fovs) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_calculate_fovs: null argument");
     if (n == 0) return GF_OK;
     std::vector<double> fov_values(n);
     const int rc = gf_cuda_find_fovs(g, cp, distortion_model, digital_lens, timestamps_ms, n, zp->fov_algorithm_margin, fov_values.data(), cu_stream);

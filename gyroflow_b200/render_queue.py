@@ -14,7 +14,7 @@ from typing import Tuple
 import numpy as np
 
 from . import abi
-from .backend import GyroflowCoreError
+from .backend import GyroflowCoreError, check_call
 
 
 class RenderQueue:
@@ -49,8 +49,7 @@ class RenderQueue:
             outs = (abi.BufferDesc * n)(*[b.to_c() for b in out_proto])
             rc = self._lib.gf_cuda_queue_create_planes(C.byref(h), C.byref(cfg), C.byref(compute_params.c), n, specs, ins, outs)
             what = "gf_cuda_queue_create_planes"
-        if rc != 0:
-            raise GyroflowCoreError(rc, what + ": " + (self._lib.gf_cuda_last_error(None) or b"").decode())
+        check_call(rc, what)
         self._h = h
 
     @classmethod

@@ -488,7 +488,8 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
  *   undist : new_width x new_height (the bounding box of the undistorted frame edge, :58-77), rotate_and_distort of every pixel (:86-109)
  * Call once with NULL buffers to get new_width / new_height, then with buffers of width*height*3 and new_width*new_height*3 floats.
  * `cp` is the user's ComputeParams; the adjustments of :24-35 (suppress_rotation, fovs cleared, per_frame == 0 -> no readout time)
- * are applied inside.  Synchronous. */
+ * are applied inside.  Synchronous.  gf_cuda_generate_stmap renders the maps as a job of one frame of gf_cuda_generate_stmaps_dev below:
+ * it uses the warp context the gyro object keeps for ST-map jobs, and leaves it there for the next call. */
 GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens,
                                      double timestamp_ms, size_t frame, float* out_rgb_dev, void* cu_stream);
 GF_API int gf_cuda_generate_stmap(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens,

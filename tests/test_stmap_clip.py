@@ -94,7 +94,9 @@ def clip_sizes(dg, lens, digital, per_frame, frames=CLIP_FRAMES, ts=CLIP_TS):
 @pytest.mark.parametrize("lens,digital", POINT_PAIRS, ids=["%s+%s" % (l, d) for l, d in POINT_PAIRS])
 def test_clip_matches_single_frame_and_oracle(lens, digital):
     """Every option row on a STMAP_SIZE frame: the clip's sizes are the single-frame call's, both maps of every frame are byte-identical
-    to the single-frame call's, and one frame per row is byte-identical to the oracle."""
+    to the single-frame call's, and one frame per row is byte-identical to the oracle.  The single-frame calls share the gyro's warp
+    context with the clip: the smallest frame's call before the clip starts it at that frame's size, the clip reuses or replaces it, and
+    each call after the clip reuses the clip's context set to its frame's size."""
     sw, sh = STMAP_SIZE
     bad, compared = [], 0
     for name, per_frame, kw in ROWS:
@@ -116,14 +118,17 @@ def test_clip_matches_single_frame_and_oracle(lens, digital):
                     dg.generate_stmaps(lens, digital, CLIP_TS, CLIP_FRAMES, per_frame)
                 assert e.value.code == GF_ERR_UNSUPPORTED_COMBO
                 continue
+            small = int(np.argmin(nw.astype(np.int64) * nh))
+            before = dg.generate_stmap(lens, digital, CLIP_TS[small], CLIP_FRAMES[small], per_frame)
             dists, undists = dg.generate_stmaps(lens, digital, CLIP_TS, CLIP_FRAMES, per_frame)
             dists = [t.cpu().numpy() for t in dists]; undists = [t.cpu().numpy() for t in undists]
-            for i, (frame, ts) in enumerate(zip(CLIP_FRAMES, CLIP_TS)):
-                want_dist, want_und = dg.generate_stmap(lens, digital, ts, frame, per_frame)
+            singles = [(small, "before the clip", before)]
+            singles += [(i, "after the clip", dg.generate_stmap(lens, digital, ts, frame, per_frame)) for i, (frame, ts) in enumerate(zip(CLIP_FRAMES, CLIP_TS))]
+            for i, when, (want_dist, want_und) in singles:
                 for what, got, want in (("redistort", dists[i], want_dist), ("undistort", undists[i], want_und)):
                     compared += 1
                     if not same_bits(got, want).all():
-                        bad.append("%s frame %d %s map vs single frame: %s" % (name, frame, what, first_diff(got, want)))
+                        bad.append("%s frame %d %s map vs single frame %s: %s" % (name, CLIP_FRAMES[i], what, when, first_diff(got, want)))
             frame, ts = CLIP_FRAMES[ORACLE_ENTRY], CLIP_TS[ORACLE_ENTRY]
             onw, onh, o_dist, o_und = oracle_stmap(oracle_cp(name, kw, lens, digital, sw, sh, frame), lens, digital, ts, frame, per_frame)
             if o_dist is None or (onw, onh) != (nw[ORACLE_ENTRY], nh[ORACLE_ENTRY]):
@@ -201,6 +206,42 @@ def test_two_jobs_back_to_back_on_one_gyro():
                 assert same_bits(undists[i].cpu().numpy(), want_und).all(), (lens, i)
     finally:
         dg.close()
+
+
+@pytest.mark.gpu
+def test_single_frame_between_jobs_of_another_lens_pair():
+    """A one-frame sony call between two fisheye clip jobs on one gyro, nothing synchronised in between: the one-frame call replaces the
+    gyro's warp context while the first job may still use it, and the second job replaces it again.  Every map is byte-identical to the
+    same call's on a gyro of its own."""
+    import torch
+    sw, sh = STMAP_SIZE
+    fisheye = make_cp(w=sw, h=sh, camera_stab=_zoom_stab(5, sh))
+    sony = make_cp(w=sw, h=sh, lens="sony", camera_stab=_zoom_stab(5, sh))       # the same gyro data, the sony lens profile
+    calls = [(fisheye, lambda dg: dg.generate_stmaps("opencv_fisheye", None, CLIP_TS, CLIP_FRAMES, True)),
+             (sony, lambda dg: [[m] for m in dg.generate_stmap("sony", None, CLIP_TS[2], CLIP_FRAMES[2], True)]),
+             (fisheye, lambda dg: dg.generate_stmaps("opencv_fisheye", None, CLIP_TS[::-1], CLIP_FRAMES, False))]
+    shared = g.DeviceGyro(fisheye)
+    try:
+        got = []
+        for cp, call in calls:
+            shared.cp = cp
+            got.append(call(shared))
+        torch.cuda.synchronize()
+        for k, (cp, call) in enumerate(calls):
+            own = g.DeviceGyro(cp)
+            try:
+                want = call(own)
+                torch.cuda.synchronize()
+            finally:
+                own.close()
+            for maps_got, maps_want in zip(got[k], want):
+                assert len(maps_got) == len(maps_want)
+                for i, (a, b) in enumerate(zip(maps_got, maps_want)):
+                    a = a.cpu().numpy() if isinstance(a, torch.Tensor) else a
+                    b = b.cpu().numpy() if isinstance(b, torch.Tensor) else b
+                    assert same_bits(a, b).all(), (k, i, first_diff(a, b))
+    finally:
+        shared.close()
 
 
 # ---- errors -----------------------------------------------------------------------------------------------------------------------
