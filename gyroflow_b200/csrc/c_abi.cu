@@ -74,13 +74,15 @@ struct gf_cuda_ctx {
     int overlays = 0;
     GrowBuf<uint8_t, true> h_drawing;
     GrowBuf<uint8_t> d_drawing, src_ovl;
-    PlaneStaging plane_staging;          // HOST multi-plane frames (gf_cuda_undistort_planes)
+    PlaneStaging plane_staging;          // device copies of HOST planes, one plane's worth from gf_cuda_create on
+    // The longest HOST input / output (0: none) a single-plane call takes: the lengths of gf_cuda_create's buffers, like the reference's
+    // fixed OpenCL buffers.  gf_cuda_undistort_planes grows the staging instead, which leaves these limits alone.
+    size_t host_in_len = 0, host_out_len = 0;
     GrowBuf<uint2> coords;               // two-pass path: the frame's coordinate map(s)
     Stream stream;
     size_t max_rows = 0;
     Slot slots[kSlots];
     int next_slot = 0;
-    GrowBuf<uint8_t> src_stage, dst_stage;   // staging when buffers are HOST
     unsigned long long launches = 0;
     std::string last_error;
 };
@@ -287,22 +289,22 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     }
 }
 
-// One frame through the warp: `FrameJob job{in, out, p, matrices, rows, mesh, mesh_len, stream}`, then the options a call needs.
+// One call through the warp: `FrameJob job{n, in, out, p, matrices, rows, mesh, mesh_len, stream}`, then the options a call needs.
 struct FrameJob {
-    const gf_buffer_desc* in; const gf_buffer_desc* out; const gf_kernel_params* p;   // arrays of 1 + more_planes planes
+    size_t n; const gf_buffer_desc* in; const gf_buffer_desc* out; const gf_kernel_params* p;   // arrays of the frame's n planes
     const float* matrices; size_t matrix_rows;
     const float* mesh; size_t mesh_len;
     void* stream;                                  // nullptr: the context's stream
     bool tables_on_device = false;                 // matrices / mesh are device pointers (else host memory, staged through a slot)
     bool sync_host = true;                         // with a HOST image buffer: wait for the frame before returning
-    size_t more_planes = 0;                        // planes after the first that share its geometry (checked by the caller)
+    int kind = -1; const char* kind_error = nullptr;   // the kind every buffer must have (-1: either), and the refusal's message
+    bool grow_staging = false;                     // HOST planes of any length (the staging grows), not only up to gf_cuda_create's
     bool coord_only = false;                       // ST maps: the coordinate pass only, into ctx->coords
     const uint32_t* table_flags_dev = nullptr;     // device tables' verdict word (nullptr: not validated, guarded path)
     const uint8_t* drawing = nullptr; size_t drawing_len = 0;   // preview overlays (after gf_cuda_set_overlays)
-    bool overlays(const gf_cuda_ctx* ctx) const { return ctx->overlays && more_planes == 0 && !coord_only; }
 };
 
-// How a frame is rendered: the one planner behind run_warp and gf_cuda_plan.
+// How a frame is rendered: the one planner behind run_frame and gf_cuda_plan.
 struct Plan {
     bool two_pass;                  // coordinates into a map (pass 1), then one sampling launch per plane (pass 2)
     int n_maps;                     // coordinate maps of pass 1: 1, or 3 for EWA (pixel + two Jacobian probes)
@@ -310,14 +312,14 @@ struct Plan {
     bool filter;                    // the packed kernel runs the filtered rolling-shutter pre-pass if the lens has a radial table
 };
 // A holds the frame's filled uniforms; table_flags is what the HOST knows of the matrix table (0 = tame and IBIS-free, non-zero =
-// anything else, including device tables not scanned on the host).  Of the job only its shape is read.
-Plan plan_frame(const Combo& c, const WarpArgs& A, uint32_t table_flags, const FrameJob& s) {
+// anything else, including device tables not scanned on the host).  n_planes: the planes that share this coordinate pass.
+Plan plan_frame(const Combo& c, const WarpArgs& A, uint32_t table_flags, bool tables_on_device, size_t n_planes, bool coord_only) {
     Plan pl;
     // Two-pass mode: used for multi-plane frames, for every resampler other than bilinear (so that the 16/64-tap and EWA code lives in
     // 11 sampling kernels instead of every lens instantiation) and for ST maps (pass 1 only).  EWA needs three coordinate maps.
     const int interp = A.p.interpolation;
-    pl.two_pass = s.more_planes > 0 || s.coord_only || interp != GF_INTERP_BILINEAR;
-    pl.n_maps = (interp > 8 && !s.coord_only) ? 3 : 1;
+    pl.two_pass = n_planes > 1 || coord_only || interp != GF_INTERP_BILINEAR;
+    pl.n_maps = (interp > 8 && !coord_only) ? 3 : 1;
     // lean instantiation iff it is in service (GF_DISABLE_LEAN), no general-only feature is on, vector access is legal, and the
     // digital-lens flag matches the template
     const bool lean_ok = c.kernels[KV_LEAN] && (A.feat & F_GENERAL_ONLY) == 0 && (A.feat & F_LEAN_REQUIRED) == F_LEAN_REQUIRED &&
@@ -330,7 +332,7 @@ Plan plan_frame(const Combo& c, const WarpArgs& A, uint32_t table_flags, const F
     // filtered pre-pass: rolling shutter on, geometry that fits the queue's entries; host tables known to be wild / IBIS take the
     // guarded path, which has no tail launch
     pl.filter = packed_ok && filter_pair(c.lens, c.digital) && (A.feat & F_RS) && !c.no_filter && A.out_cols <= WarpArgs::X2Filter::kMaxCols &&
-                A.out_rows <= WarpArgs::X2Filter::kMaxRows && (s.tables_on_device || table_flags == 0);
+                A.out_rows <= WarpArgs::X2Filter::kMaxRows && (tables_on_device || table_flags == 0);
     return pl;
 }
 
@@ -354,25 +356,29 @@ bool planes_share_geometry(const gf_kernel_params* p, const gf_buffer_desc* in, 
 
 const dim3 kBlock(GF_BLOCK_X, GF_BLOCK_Y);
 
-// One frame through the warp: the steps of run_warp and what they hand on to each other.
+// One call through the warp: the steps of run_frame and what they hand on to each other.
 struct FrameRun {
     gf_cuda_ctx* const ctx; const FrameJob& job;
     std::string* const err = &ctx->last_error;
-    const gf_buffer_desc* const in = job.in; const gf_buffer_desc* const out = job.out; const gf_kernel_params* const p = job.p;
+    const gf_kernel_params* const p = job.p;
     const cudaStream_t st = job.stream ? (cudaStream_t)job.stream : ctx->stream.get();
-    WarpArgs A;
-    Slot* slot = nullptr;                   // the table slot of this frame, if it uses one (host tables, or a mesh to widen)
-    uint32_t table_flags = TBL_WILD;        // host-known verdict: device tables are not trusted until validated
-    bool full_cover = false;                // the kernel writes every output byte that travels back
+    const bool fused = job.n > 1 && ctx->fn_shade && planes_share_geometry(p, job.in, job.out, job.n);   // one coordinate pass
+    const bool overlays = ctx->overlays && !fused && !job.coord_only;   // preview overlays, on every plane rendered on its own
+    const bool host = std::any_of(job.in, job.in + job.n, [](const gf_buffer_desc& b) { return b.kind == GF_BUF_HOST; }) ||
+                      std::any_of(job.out, job.out + job.n, [](const gf_buffer_desc& b) { return b.kind == GF_BUF_HOST; });
+    std::vector<gf_buffer_desc> in{job.in, job.in + job.n}, out{job.out, job.out + job.n};   // what the kernels read and write
+    bool src_private = false;               // in[0] is the context's staged copy of a HOST input
+    WarpArgs T;                             // the call's tables, which every plane's arguments start from
+    Slot* slot = nullptr;                   // the table slot of this call, if it uses one (host tables, or a mesh to widen)
+    size_t table_rows = 0;                  // host tables: the rows copied and scanned, the most any plane reads
+    uint32_t table_flags = TBL_WILD;        // host-known verdict of those rows: device tables are not trusted until validated
     const uint8_t* drawing_dev = nullptr;
-    Plan plan;
-    const FilterPrepass::Table* radial = nullptr;   // the lens's radial table when the frame runs the filtered pre-pass
-    dim3 grid;                              // of the scalar kernels and the sampling pass (blocks of kBlock)
 
-    // Tables and mesh: host tables are copied through a slot and scanned on the host; a mesh is widened to f64 on the device.
-    // HOST image buffers: the input to its staging buffer, and the output too unless the kernel overwrites all of it.
+    // Tables and mesh, once per call: host tables are copied through a slot and scanned on the host; a mesh is widened to f64 on the
+    // device.  HOST planes: their device copies, which the planes are rendered from.
     int stage() {
-        const size_t mat_bytes = (size_t)p->matrix_count * GF_MATRIX_STRIDE * sizeof(float);
+        if (job.grow_staging) CK(err, ctx->plane_staging.reserve(job.n, job.in, job.out, st));
+        memset(&T, 0, sizeof(T));
         if (!job.tables_on_device || job.mesh_len > 0) {      // device tables still need a slot for the widened mesh
             slot = &ctx->slots[ctx->next_slot];
             ctx->next_slot = (ctx->next_slot + 1) % kSlots;
@@ -380,47 +386,42 @@ struct FrameRun {
         }
         if (job.tables_on_device) {
             // the verdict travels with the data: a device word written on this stream (or ordered before it) by whoever produced the table
-            A.table_flags = job.table_flags_dev ? job.table_flags_dev : ctx->const_flags.ptr + 1;
-            A.matrices = job.matrices;
-            A.mesh = job.mesh_len ? job.mesh : nullptr;
+            T.table_flags = job.table_flags_dev ? job.table_flags_dev : ctx->const_flags.ptr + 1;
+            T.matrices = job.matrices;
+            T.mesh = job.mesh_len ? job.mesh : nullptr;
         } else {
+            for (size_t i = 0; i < job.n; ++i) table_rows = std::max(table_rows, (size_t)p[i].matrix_count);
+            const size_t mat_bytes = table_rows * GF_MATRIX_STRIDE * sizeof(float);
             memcpy(slot->h_mat.ptr, job.matrices, mat_bytes);
-            table_flags = gf_table_flags_host(slot->h_mat.ptr, (size_t)p->matrix_count);
-            A.table_flags = ctx->const_flags.ptr + (table_flags ? 1 : 0);
+            table_flags = gf_table_flags_host(slot->h_mat.ptr, table_rows);
             CK(err, cudaMemcpyAsync(slot->d_mat.ptr, slot->h_mat.ptr, mat_bytes, cudaMemcpyHostToDevice, st));
-            A.matrices = slot->d_mat.ptr;
+            T.matrices = slot->d_mat.ptr;
             if (job.mesh_len) {
                 memcpy(slot->h_mesh.ptr, job.mesh, job.mesh_len * sizeof(float));
                 CK(err, cudaMemcpyAsync(slot->d_mesh.ptr, slot->h_mesh.ptr, job.mesh_len * sizeof(float), cudaMemcpyHostToDevice, st));
-                A.mesh = slot->d_mesh.ptr;
+                T.mesh = slot->d_mesh.ptr;
             }
         }
-        A.mesh_len = (int)job.mesh_len;
+        T.mesh_len = (int)job.mesh_len;
         if (job.mesh_len) {                                    // cpu_undistort.rs:539 — `mesh_data.iter().map(|x| *x as f64)`, once per frame
             double* const m64 = slot->d_mesh64.ptr;
-            widen_mesh_kernel<<<(unsigned)((job.mesh_len + 255) / 256), 256, 0, st>>>(A.mesh, m64, (int)job.mesh_len, (float)p->width, (float)p->height);
+            widen_mesh_kernel<<<(unsigned)((job.mesh_len + 255) / 256), 256, 0, st>>>(T.mesh, m64, (int)job.mesh_len, (float)p->width, (float)p->height);
             CK(err, cudaGetLastError());
-            A.mesh64 = m64; A.mesh_aux = reinterpret_cast<const MeshAux*>(m64 + GF_MESH_MAX_LEN);
+            T.mesh64 = m64; T.mesh_aux = reinterpret_cast<const MeshAux*>(m64 + GF_MESH_MAX_LEN);
         }
-        A.src = (const uint8_t*)in->ptr; A.dst = (uint8_t*)out->ptr; A.src_len = in->len; A.dst_len = out->len;
-        if (in->kind == GF_BUF_HOST) {                         // opencl.rs:359 `self.src.write(buffer)`
+        if (host) {                                            // opencl.rs:359 `self.src.write(buffer)`
             nvtxRangePushA("gf_h2d_frame");
-            cudaError_t e_h2d = cudaMemcpyAsync(ctx->src_stage.ptr, in->ptr, in->len, cudaMemcpyHostToDevice, st);
+            const int rc = ctx->plane_staging.upload(job.n, job.in, job.out, p, false, st, err, in.data(), out.data());
             nvtxRangePop();
-            CK(err, e_h2d);
-            A.src = ctx->src_stage.ptr;
-        }
-        full_cover = warp_covers_output(*p, *out, ctx->combo.bpp());
-        if (out->kind == GF_BUF_HOST) {
-            if (!full_cover) CK(err, cudaMemcpyAsync(ctx->dst_stage.ptr, out->ptr, out->len, cudaMemcpyHostToDevice, st));
-            A.dst = ctx->dst_stage.ptr;
+            if (rc != GF_OK) return rc;
+            src_private = job.in[0].kind == GF_BUF_HOST;
         }
         return GF_OK;
     }
 
     // Preview overlays, input stage: drawing entries with stage bit 0 are drawn onto the device copy of the input.
     int draw_input_overlays() {
-        if (!job.overlays(ctx)) return GF_OK;
+        if (!overlays || job.n != 1) return GF_OK;
         bool any_input_stage = false;
         if ((p->flags & GF_FLAG_DRAWING_ENABLED) && job.drawing && job.drawing_len) {
             CK(err, ctx->h_drawing.reserve(job.drawing_len, st));   // (a growing reserve waits for the stream itself)
@@ -431,34 +432,44 @@ struct FrameRun {
             drawing_dev = ctx->d_drawing.ptr;
         }
         if (!any_input_stage) return GF_OK;
-        if (in->kind == GF_BUF_DEVICE) {                       // never draw into the caller's buffer: private copy
-            CK(err, ctx->src_ovl.reserve(in->len, st));
-            CK(err, cudaMemcpyAsync(ctx->src_ovl.ptr, in->ptr, in->len, cudaMemcpyDeviceToDevice, st));
-            A.src = ctx->src_ovl.ptr;
+        if (!src_private) {                                    // never draw into the caller's buffer: private copy
+            CK(err, ctx->src_ovl.reserve(in[0].len, st));
+            CK(err, cudaMemcpyAsync(ctx->src_ovl.ptr, in[0].ptr, in[0].len, cudaMemcpyDeviceToDevice, st));
+            in[0].ptr = ctx->src_ovl.ptr;
         }
         const LayoutInfo& L = kLayouts[ctx->combo.layout];
-        if (gf_internal_draw_overlays((void*)st, const_cast<uint8_t*>(A.src), in->len, in->width, in->height, p->stride, p, L.channels, L.scalar, 1,
+        if (gf_internal_draw_overlays((void*)st, (uint8_t*)in[0].ptr, in[0].len, in[0].width, in[0].height, p->stride, p, L.channels, L.scalar, 1,
                                       drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (input stage) failed");
         return GF_OK;
     }
 
-    // Uniforms, launch geometry, plan, and the coordinate map of the two-pass path.
-    int plan_launch() {
+    // The planes: one coordinate pass for all of them when they share a geometry, otherwise each plane on its own.
+    int render() {
+        if (fused) return render_planes(0, job.n);
+        for (size_t i = 0; i < job.n; ++i) { const int rc = render_planes(i, 1); if (rc != GF_OK) return rc; }
+        return GF_OK;
+    }
+
+    // Planes [first, first + count) of one geometry: uniforms, launch geometry and plan of the first, pass 1 (or the whole frame), then
+    // pass 2, one sampling launch per plane.
+    int render_planes(size_t first, size_t count) {
+        WarpArgs A = T;
+        A.p = p[first];
+        A.src = (const uint8_t*)in[first].ptr; A.dst = (uint8_t*)out[first].ptr; A.src_len = in[first].len; A.dst_len = out[first].len;
+        // a plane that reads fewer rows than the call staged has the verdict of its own rows
+        const uint32_t flags = (size_t)A.p.matrix_count < table_rows ? gf_table_flags_host(slot->h_mat.ptr, (size_t)A.p.matrix_count) : table_flags;
+        if (!job.tables_on_device) A.table_flags = ctx->const_flags.ptr + (flags ? 1 : 0);
         fill_uniforms(A, ctx->combo);
-        grid = dim3((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);
+        const dim3 grid((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);
         if (grid.x == 0 || grid.y == 0 || grid.y > 65535) return fail(err, GF_ERR_BAD_PARAMS, "output buffer geometry out of range");
-        plan = plan_frame(ctx->combo, A, table_flags, job);
+        const Plan plan = plan_frame(ctx->combo, A, flags, job.tables_on_device, count, job.coord_only);
+        const FilterPrepass::Table* radial = nullptr;   // the lens's radial table when the frame runs the filtered pre-pass
         if (plan.filter) { const int rc = ctx->filter.table(A.p.k, st, err, &radial); if (rc != GF_OK) return rc; }
         if (plan.two_pass) {
             if (!ctx->fn_shade && !job.coord_only) return fail(err, GF_ERR_UNSUPPORTED_COMBO, "no sampling kernel for this pixel layout");
             CK(err, ctx->coords.reserve((size_t)A.out_cols * (size_t)A.out_rows * (size_t)plan.n_maps, st));
             A.coord_out = ctx->coords.ptr;
         }
-        return GF_OK;
-    }
-
-    // Pass 1, or the whole frame: the planned kernel.
-    int launch() {
         const KernelFn fn = ctx->combo.kernels[plan.kernel];
         if (plan.kernel == KV_PACKED || plan.kernel == KV_PACKED_COORDS) {
             // 32 x 4 threads (4 x 8 output rows... 32 x 8 pixels) per block measured 2 % faster than 32 x 8 threads (finer tail)
@@ -476,39 +487,34 @@ struct FrameRun {
         }
         CK(err, cudaGetLastError());
         ctx->launches++;
+        if (!plan.two_pass || job.coord_only) return GF_OK;
+        for (size_t i = first; i < first + count; ++i) {
+            WarpArgs B = A;
+            B.p = p[i];
+            B.coord_out = nullptr; B.coord_in = ctx->coords.ptr; B.coord_maps = plan.n_maps; B.coord_shift = 0;
+            B.src = (const uint8_t*)in[i].ptr; B.dst = (uint8_t*)out[i].ptr; B.src_len = in[i].len; B.dst_len = out[i].len;
+            fill_uniforms(B, ctx->combo);
+            ctx->fn_shade<<<grid, kBlock, 0, st>>>(B);
+            CK(err, cudaGetLastError());
+            ctx->launches++;
+        }
         return GF_OK;
     }
 
-    // Pass 2 (one sampling launch per plane), output-stage overlays, copy back, synchronisation.
+    // Output-stage overlays, copy back, synchronisation.
     int finish() {
-        if (plan.two_pass && !job.coord_only) {
-            for (size_t i = 0; i <= job.more_planes; ++i) {
-                WarpArgs B = A;
-                B.p = p[i];
-                B.coord_out = nullptr; B.coord_in = ctx->coords.ptr; B.coord_maps = plan.n_maps; B.coord_shift = 0;
-                if (job.more_planes > 0) { B.src = (const uint8_t*)in[i].ptr; B.dst = (uint8_t*)out[i].ptr; B.src_len = in[i].len; B.dst_len = out[i].len; }
-                fill_uniforms(B, ctx->combo);
-                ctx->fn_shade<<<grid, kBlock, 0, st>>>(B);
-                CK(err, cudaGetLastError());
-                ctx->launches++;
-            }
-        }
         if (slot) CK(err, cudaEventRecord(slot->done.get(), st));
-        if (job.overlays(ctx)) {                               // output stage: stage-1 drawing entries + safe area, on the final pixels
+        for (size_t i = 0; overlays && i < job.n; ++i) {      // output stage: stage-1 drawing entries + safe area, on the final pixels
             const LayoutInfo& L = kLayouts[ctx->combo.layout];
-            if (gf_internal_draw_overlays((void*)st, A.dst, out->len, out->width, out->height, p->output_stride, p, L.channels, L.scalar, 0,
-                                          drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (output stage) failed");
+            if (gf_internal_draw_overlays((void*)st, (uint8_t*)out[i].ptr, out[i].len, out[i].width, out[i].height, p[i].output_stride, &p[i], L.channels,
+                                          L.scalar, 0, drawing_dev, job.drawing_len) != GF_OK) return fail(err, GF_ERR_CUDA, "overlay kernel (output stage) failed");
         }
-        if (out->kind == GF_BUF_HOST) {                                                                              // opencl.rs:413
-            nvtxRangePushA("gf_d2h_frame");
-            cudaError_t e_d2h;
-            if (full_cover) e_d2h = cudaMemcpy2DAsync(out->ptr, (size_t)p->output_stride, ctx->dst_stage.ptr, (size_t)p->output_stride,
-                                                      (size_t)out->width * (size_t)ctx->combo.bpp(), (size_t)out->height, cudaMemcpyDeviceToHost, st);
-            else            e_d2h = cudaMemcpyAsync(out->ptr, ctx->dst_stage.ptr, out->len, cudaMemcpyDeviceToHost, st);
-            nvtxRangePop();
-            CK(err, e_d2h);
-        }
-        if (job.sync_host && (in->kind == GF_BUF_HOST || out->kind == GF_BUF_HOST)) CK(err, cudaStreamSynchronize(st));
+        if (!host) return GF_OK;
+        nvtxRangePushA("gf_d2h_frame");                                                                              // opencl.rs:413
+        const int rc = ctx->plane_staging.download(job.n, job.out, p, st, err);
+        nvtxRangePop();
+        if (rc != GF_OK) return rc;
+        if (job.sync_host) CK(err, cudaStreamSynchronize(st));
         return GF_OK;
     }
 };
@@ -520,48 +526,53 @@ int order_after_last_call(gf_cuda_ctx* ctx, cudaStream_t st) {
     return GF_OK;
 }
 
-int run_warp(gf_cuda_ctx* ctx, const FrameJob& job) {
+// Every argument check of a call, before anything is enqueued: each plane's buffer kind and validate, then the checks of the call
+// against the context, plane by plane.
+int check_frame(gf_cuda_ctx* ctx, const FrameJob& job) {
+    std::string* const err = &ctx->last_error;
+    for (size_t i = 0; i < job.n; ++i) {
+        if (job.kind >= 0 && (job.in[i].kind != job.kind || job.out[i].kind != job.kind)) return fail(err, GF_ERR_BAD_PARAMS, job.kind_error);
+        const int rc = validate(err, job.p + i, job.in + i, job.out + i, ctx->combo.bpp());
+        if (rc != GF_OK) return rc;
+    }
+    for (size_t i = 0; i < job.n; ++i) {
+        const gf_kernel_params* p = &job.p[i];
+        if (!job.matrices) return fail(err, GF_ERR_NO_DATA, "NoStabilizationData: matrices is null");
+        if (p->width != ctx->width || p->height != ctx->height || p->output_width != ctx->output_width || p->output_height != ctx->output_height)
+            return fail(err, GF_ERR_SIZE_MISMATCH, "SizeMismatch: KernelParams size differs from the size this context was created for");
+        if (p->interpolation != ctx->interpolation)
+            return fail(err, GF_ERR_UNSUPPORTED_COMBO, "interpolation differs from the one this context was created for");
+        if ((size_t)p->matrix_count > job.matrix_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices: matrix_count > rows supplied");
+        if (!job.tables_on_device && job.matrix_rows > ctx->max_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices");
+        if (job.mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
+        if (job.mesh_len > 0 && !job.mesh) return fail(err, GF_ERR_BAD_PARAMS, "mesh is null");
+        if (job.mesh_len > 0 && job.mesh_len < 9) return fail(err, GF_ERR_BAD_PARAMS, "mesh shorter than its 9-value header (the reference would index out of bounds)");
+        if (!job.grow_staging && job.in[i].kind == GF_BUF_HOST && job.in[i].len > ctx->host_in_len)
+            return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input");
+        if (!job.grow_staging && job.out[i].kind == GF_BUF_HOST && job.out[i].len > ctx->host_out_len)
+            return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch output");
+        if (job.tables_on_device && (reinterpret_cast<uintptr_t>(job.matrices) & 7u)) return fail(err, GF_ERR_BAD_PARAMS, "device matrices must be 8-byte aligned");
+    }
+    return GF_OK;
+}
+
+// Every call that renders pixels (and the coordinate pass of ST maps): its checks, then its tables and HOST planes staged once, the
+// planes rendered, copied back, and the call recorded in last_call.
+int run_frame(gf_cuda_ctx* ctx, const FrameJob& job) {
     if (!ctx) return fail(nullptr, GF_ERR_BAD_PARAMS, "ctx is null");
     std::string* const err = &ctx->last_error;
-    const gf_kernel_params* p = job.p;
-    int rc = validate(err, p, job.in, job.out, ctx->combo.bpp());
+    int rc = check_frame(ctx, job);
     if (rc != GF_OK) return rc;
-    if (!job.matrices) return fail(err, GF_ERR_NO_DATA, "NoStabilizationData: matrices is null");
-    if (p->width != ctx->width || p->height != ctx->height || p->output_width != ctx->output_width || p->output_height != ctx->output_height)
-        return fail(err, GF_ERR_SIZE_MISMATCH, "SizeMismatch: KernelParams size differs from the size this context was created for");
-    if (p->interpolation != ctx->interpolation)
-        return fail(err, GF_ERR_UNSUPPORTED_COMBO, "interpolation differs from the one this context was created for");
-    if ((size_t)p->matrix_count > job.matrix_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices: matrix_count > rows supplied");
-    if (!job.tables_on_device && job.matrix_rows > ctx->max_rows) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch matrices");
-    if (job.mesh_len > GF_MESH_MAX_LEN) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch buf_mesh_data");
-    if (job.mesh_len > 0 && !job.mesh) return fail(err, GF_ERR_BAD_PARAMS, "mesh is null");
-    if (job.mesh_len > 0 && job.mesh_len < 9) return fail(err, GF_ERR_BAD_PARAMS, "mesh shorter than its 9-value header (the reference would index out of bounds)");
-    if (job.in->kind == GF_BUF_HOST && job.in->len > ctx->src_stage.len)   return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input");
-    if (job.out->kind == GF_BUF_HOST && job.out->len > ctx->dst_stage.len) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch output");
-    if (job.tables_on_device && (reinterpret_cast<uintptr_t>(job.matrices) & 7u)) return fail(err, GF_ERR_BAD_PARAMS, "device matrices must be 8-byte aligned");
     CK(err, cudaSetDevice(ctx->device));
     FrameRun F{ctx, job};
     if ((rc = order_after_last_call(ctx, F.st)) != GF_OK) return rc;
-    memset(&F.A, 0, sizeof(F.A));
-    F.A.p = *job.p;
-    if ((rc = F.stage()) == GF_OK && (rc = F.draw_input_overlays()) == GF_OK && (rc = F.plan_launch()) == GF_OK) {
+    if ((rc = F.stage()) == GF_OK && (rc = F.draw_input_overlays()) == GF_OK) {
         nvtxRangePushA("gf_warp_launch");
-        if ((rc = F.launch()) == GF_OK) rc = F.finish();
+        if ((rc = F.render()) == GF_OK) rc = F.finish();
         nvtxRangePop();
     }
     CK(err, cudaEventRecord(ctx->last_call.get(), F.st));    // also after a failure: whatever was enqueued still uses the context
     return rc;
-}
-
-// The planes of one frame, DEVICE buffers (staged ones included): one coordinate pass for all planes when they share a geometry.
-int run_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out, const gf_kernel_params* params, FrameJob job) {
-    const bool fuse = n_planes > 1 && ctx->fn_shade && planes_share_geometry(params, in, out, n_planes);
-    for (size_t i = 0; i < (fuse ? 1 : n_planes); ++i) {
-        job.in = &in[i]; job.out = &out[i]; job.p = &params[i]; job.more_planes = fuse ? n_planes - 1 : 0;
-        int rc = run_warp(ctx, job);
-        if (rc != GF_OK) return rc;
-    }
-    return GF_OK;
 }
 
 } // namespace
@@ -733,8 +744,9 @@ GF_API int gf_cuda_create(gf_cuda_ctx** out_ctx, int device, const gf_kernel_par
         CK(nullptr, sl.d_mesh64.reserve(GF_MESH_MAX_LEN + (sizeof(MeshAux) + 7) / 8, st));
         CK(nullptr, create_event(sl.done));
     }
-    if (in->kind == GF_BUF_HOST) CK(nullptr, ctx->src_stage.reserve(in->len, st));
-    if (out->kind == GF_BUF_HOST) CK(nullptr, ctx->dst_stage.reserve(out->len, st));
+    ctx->host_in_len = in->kind == GF_BUF_HOST ? in->len : 0;
+    ctx->host_out_len = out->kind == GF_BUF_HOST ? out->len : 0;
+    CK(nullptr, ctx->plane_staging.reserve(1, in, out, st));
     *out_ctx = ctx.release();
     return GF_OK;
 }
@@ -752,9 +764,9 @@ GF_API int gf_cuda_undistort_image(gf_cuda_ctx* ctx, const gf_buffer_desc* in, c
                                    const float* mesh, size_t mesh_len, const uint8_t* drawing, size_t drawing_len, void* cu_stream) {
     // the CPU path (the parity target) draws no overlay (cpu_undistort.rs:234-251,607,617): `drawing` is used only after
     // gf_cuda_set_overlays(ctx, 1) — then like the reference's GPU kernels (opencl_undistort.cl:121-154, overlay.cu)
-    FrameJob job{in, out, params, matrices, matrix_rows, mesh, mesh_len, cu_stream};
+    FrameJob job{1, in, out, params, matrices, matrix_rows, mesh, mesh_len, cu_stream};
     job.drawing = drawing; job.drawing_len = drawing_len;
-    return run_warp(ctx, job);
+    return run_frame(ctx, job);
 }
 
 GF_API int gf_cuda_undistort_image_dev(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out,
@@ -766,9 +778,9 @@ GF_API int gf_cuda_undistort_image_dev(gf_cuda_ctx* ctx, const gf_buffer_desc* i
 GF_API int gf_cuda_undistort_image_dev_flagged(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                                const gf_kernel_params* params, const float* matrices_dev, size_t matrix_rows,
                                                const float* mesh_dev, size_t mesh_len, const uint32_t* table_flags_dev, void* cu_stream) {
-    FrameJob job{in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
+    FrameJob job{1, in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
     job.tables_on_device = true; job.table_flags_dev = table_flags_dev;
-    return run_warp(ctx, job);
+    return run_frame(ctx, job);
 }
 
 GF_API int gf_cuda_scan_tables_dev(const float* matrices_dev, size_t matrix_rows, uint32_t* table_flags_dev, void* cu_stream) {
@@ -781,9 +793,9 @@ GF_API int gf_cuda_scan_tables_dev(const float* matrices_dev, size_t matrix_rows
 GF_API int gf_cuda_undistort_image_async(gf_cuda_ctx* ctx, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                          const gf_kernel_params* params, const float* matrices, size_t matrix_rows,
                                          const float* mesh, size_t mesh_len, void* cu_stream) {
-    FrameJob job{in, out, params, matrices, matrix_rows, mesh, mesh_len, cu_stream};
+    FrameJob job{1, in, out, params, matrices, matrix_rows, mesh, mesh_len, cu_stream};
     job.sync_host = false;
-    return run_warp(ctx, job);
+    return run_frame(ctx, job);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -834,9 +846,9 @@ int enqueue_stmap_frame(gf_cuda_ctx* ctx, gf_cuda_gyro* g, gf_compute_params cp,
     d.width = new_w; d.height = new_h; d.stride = new_w; d.kind = GF_BUF_DEVICE;
     d.ptr = undist_rgb_dev; d.len = (size_t)new_w * (size_t)new_h;                          // never dereferenced in coordinate mode
     ctx->width = ctx->output_width = new_w; ctx->height = ctx->output_height = new_h;
-    FrameJob job{&d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};                    // the table is staged through a slot
+    FrameJob job{1, &d, &d, &kq, mats.data(), rows, nullptr, 0, (void*)st};                 // the table is staged through a slot
     job.coord_only = true;
-    if ((rc = run_warp(ctx, job)) != GF_OK) return rc;
+    if ((rc = run_frame(ctx, job)) != GF_OK) return rc;
     const dim3 block(32, 8), grid(((unsigned)new_w + 31) / 32, ((unsigned)new_h + 7) / 8);
     stmap_rgb_kernel<<<grid, block, 0, st>>>(ctx->coords.ptr, new_w, new_h, new_w, undist_rgb_dev);
     CK(nullptr, cudaGetLastError());
@@ -945,45 +957,29 @@ GF_API int gf_cuda_undistort_planes_dev_flagged(gf_cuda_ctx* ctx, size_t n_plane
                                                 const gf_kernel_params* params, const float* matrices_dev, size_t matrix_rows,
                                                 const float* mesh_dev, size_t mesh_len, const uint32_t* table_flags_dev, void* cu_stream) {
     if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    for (size_t i = 0; i < n_planes; ++i) {
-        if (in[i].kind != GF_BUF_DEVICE || out[i].kind != GF_BUF_DEVICE) return fail(&ctx->last_error, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes_dev takes DEVICE buffers");
-        int rc = validate(&ctx->last_error, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
-    }
-    FrameJob job{in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
+    FrameJob job{n_planes, in, out, params, matrices_dev, matrix_rows, mesh_dev, mesh_len, cu_stream};
+    job.kind = GF_BUF_DEVICE; job.kind_error = "gf_cuda_undistort_planes_dev takes DEVICE buffers";
     job.tables_on_device = true; job.table_flags_dev = table_flags_dev;
-    return run_planes(ctx, n_planes, in, out, params, job);
+    return run_frame(ctx, job);
 }
 
 // The planes of one frame in HOST memory — what the render path hands over for planar software frames (rendering/mod.rs:596-629:
 // every plane a BufferSource::Cpu slice): stage every plane to the device, render them like gf_cuda_undistort_planes_dev (one
-// coordinate pass shared by the planes of one geometry), copy every plane back, synchronise.  Host tables, like gf_cuda_undistort_image.
+// coordinate pass shared by the planes of one geometry), copy every plane back, synchronise.  Host tables, like gf_cuda_undistort_image;
+// unlike it, planes of any length (the context's staging grows to them).
 GF_API int gf_cuda_undistort_planes(gf_cuda_ctx* ctx, size_t n_planes, const gf_buffer_desc* in, const gf_buffer_desc* out,
                                     const gf_kernel_params* params, const float* matrices, size_t matrix_rows,
                                     const float* mesh, size_t mesh_len, void* cu_stream) {
     if (!ctx || !in || !out || !params || n_planes == 0) return fail(ctx ? &ctx->last_error : nullptr, GF_ERR_BAD_PARAMS, "null argument");
-    std::string* const err = &ctx->last_error;
-    for (size_t i = 0; i < n_planes; ++i) {
-        if (in[i].kind != GF_BUF_HOST || out[i].kind != GF_BUF_HOST) return fail(err, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_planes takes HOST buffers (DEVICE: gf_cuda_undistort_planes_dev)");
-        int rc = validate(err, &params[i], &in[i], &out[i], ctx->combo.bpp()); if (rc != GF_OK) return rc;
-    }
-    CK(err, cudaSetDevice(ctx->device));
-    cudaStream_t st = cu_stream ? (cudaStream_t)cu_stream : ctx->stream.get();
-    int rc = order_after_last_call(ctx, st);             // the staging copies below reuse the context's buffers
-    if (rc != GF_OK) return rc;
-    CK(err, ctx->plane_staging.reserve(n_planes, in, out, st));
-    std::vector<gf_buffer_desc> din(n_planes), dout(n_planes);
-    if ((rc = ctx->plane_staging.upload(n_planes, in, out, params, false, st, err, din.data(), dout.data())) != GF_OK) return rc;
-    FrameJob job{din.data(), dout.data(), params, matrices, matrix_rows, mesh, mesh_len, (void*)st};
-    job.sync_host = false;
-    if ((rc = run_planes(ctx, n_planes, din.data(), dout.data(), params, job)) != GF_OK) return rc;
-    if ((rc = ctx->plane_staging.download(n_planes, out, params, st, err)) != GF_OK) return rc;
-    CK(err, cudaStreamSynchronize(st));
-    return GF_OK;
+    FrameJob job{n_planes, in, out, params, matrices, matrix_rows, mesh, mesh_len, cu_stream};
+    job.kind = GF_BUF_HOST; job.kind_error = "gf_cuda_undistort_planes takes HOST buffers (DEVICE: gf_cuda_undistort_planes_dev)";
+    job.grow_staging = true;
+    return run_frame(ctx, job);
 }
 
 // Host-only: which kernel variant would render this frame (no CUDA call, no context).  table_flags: 0 = validated tame tables without
 // IBIS rows, non-zero = anything else.  Returns 0 general, 1 lean, 2 packed, 3 packed + trusted tables, | 0x10 two-pass (plan_frame,
-// the planner run_warp uses), or a negative GF_ERR_*.  A planning aid for integrators and the hook the CPU-only tests use to check
+// the planner run_frame uses), or a negative GF_ERR_*.  A planning aid for integrators and the hook the CPU-only tests use to check
 // the host logic.  gf_cuda_plan_features also writes the frame's feature word (F_* of warp_kernel.cuh) to *feat_out: the bits
 // fill_uniforms computes, plus F_FILTER when the plan runs the filtered pre-pass (FilterPrepass::launch sets that bit at launch time).
 GF_API int gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type, int distortion_model, int digital_lens,
@@ -999,9 +995,7 @@ GF_API int gf_cuda_plan_features(const gf_kernel_params* params, int pixel_type,
     A.p = *params; A.mesh_len = (int)mesh_len;
     A.src = (const uint8_t*)in->ptr; A.dst = (uint8_t*)out->ptr; A.src_len = in->len; A.dst_len = out->len;
     fill_uniforms(A, c);
-    FrameJob job{in, out, params, nullptr, 0, nullptr, mesh_len, nullptr};
-    job.more_planes = n_planes > 1 ? n_planes - 1 : 0;
-    Plan pl = plan_frame(c, A, table_flags, job);
+    Plan pl = plan_frame(c, A, table_flags, false, n_planes, false);
     if (pl.filter) { std::vector<float4> rows(GF_RADIAL_ROWS); pl.filter = radial_table_cap(A.p.k, rows.data()) > 0.0f; }   // as FilterPrepass::table
     // packed: the trusted path runs when the table's verdict word is 0, which the host knows only for tables it scanned
     const int v = pl.kernel == KV_GENERAL ? 0 : (pl.kernel == KV_LEAN ? 1 : (table_flags == 0 ? 3 : 2));

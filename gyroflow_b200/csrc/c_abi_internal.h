@@ -142,7 +142,7 @@ private:
 // cpu_undistort.rs:551 passes everywhere), and the buffer lacks at most the last row's padding.  Otherwise the pixels the warp leaves
 // alone keep their previous content, like on the CPU path, so a staged output is uploaded first.
 bool warp_covers_output(const gf_kernel_params& p, const gf_buffer_desc& out, int bpp);
-// Device copies of a frame's HOST planes (render-queue slots, gf_cuda_undistort_planes); a DEVICE buffer is used in place.
+// Device copies of a frame's HOST planes (render-queue slots, warp contexts); a DEVICE buffer is used in place.
 class PlaneStaging {
 public:
     cudaError_t reserve(size_t n, const gf_buffer_desc* in, const gf_buffer_desc* out, cudaStream_t st);   // growing waits for `st`
