@@ -33,6 +33,8 @@ struct Slot {                                   // one in-flight set of per-fram
 };
 constexpr int kSlots = 4;
 constexpr int kPackedBlockY = 4;                // packed-kernel blocks are GF_BLOCK_X x kPackedBlockY threads
+constexpr unsigned long long kMaxOutRows = 65535ull * GF_BLOCK_Y;   // output rows one launch covers (65535 row blocks, gridDim.y)
+static_assert(2 * kPackedBlockY == GF_BLOCK_Y, "the packed kernel's row blocks cover GF_BLOCK_Y rows, like the scalar kernels'");
 
 // Per pixel layout (LAY_*): bytes per pixel, channels, scalar kind (SC_*), the maximum value pixel_value_limit is compared against
 struct LayoutInfo { int bpp, channels, scalar; float max_value; };
@@ -150,6 +152,11 @@ int validate(std::string* err, const gf_kernel_params* p, const gf_buffer_desc* 
         if (last > in->len) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "Buffer size mismatch input: source_rect exceeds the input buffer");
     }
     if (out->len == 0) return fail(err, GF_ERR_BUFFER_TOO_SMALL, "empty output buffer");
+    // launch geometry: at least one whole pixel per row, and ceil(len / output_stride) rows in blocks of GF_BLOCK_Y rows, at most 65535
+    // blocks (gridDim.y); checked here so that gf_cuda_plan refuses what the rendering call would
+    const unsigned long long out_rows = (out->len + (unsigned long long)p->output_stride - 1) / (unsigned long long)p->output_stride;
+    if (p->output_stride < bpp || out_rows > kMaxOutRows)
+        return fail(err, GF_ERR_BAD_PARAMS, "output buffer geometry out of range (a pixel per row, at most 524280 rows)");
     return GF_OK;
 }
 
@@ -460,8 +467,7 @@ struct FrameRun {
         const uint32_t flags = (size_t)A.p.matrix_count < table_rows ? gf_table_flags_host(slot->h_mat.ptr, (size_t)A.p.matrix_count) : table_flags;
         if (!job.tables_on_device) A.table_flags = ctx->const_flags.ptr + (flags ? 1 : 0);
         fill_uniforms(A, ctx->combo);
-        const dim3 grid((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);
-        if (grid.x == 0 || grid.y == 0 || grid.y > 65535) return fail(err, GF_ERR_BAD_PARAMS, "output buffer geometry out of range");
+        const dim3 grid((A.out_cols + GF_BLOCK_X - 1) / GF_BLOCK_X, (A.out_rows + GF_BLOCK_Y - 1) / GF_BLOCK_Y);   // in range: validate
         const Plan plan = plan_frame(ctx->combo, A, flags, job.tables_on_device, count, job.coord_only);
         const FilterPrepass::Table* radial = nullptr;   // the lens's radial table when the frame runs the filtered pre-pass
         if (plan.filter) { const int rc = ctx->filter.table(A.p.k, st, err, &radial); if (rc != GF_OK) return rc; }

@@ -217,7 +217,9 @@ GF_API int         gf_pixel_bytes(int pixel_type);        /* COUNT * SCALAR_BYTE
 GF_API int         gf_combo_supported(int pixel_type, int distortion_model, int digital_lens, int interpolation);
 
 /* ---- construct: OclWrapper::new opencl.rs:178 / WgpuWrapper::new wgpu.rs:147 ----------------
- * Validates (height >= 4, stride >= 1, width <= 16384 — opencl.rs:179, wgpu.rs:150), selects the
+ * Validates (height >= 4, stride >= 1, width <= 16384 — opencl.rs:179, wgpu.rs:150; and, as every
+ * warp call and gf_cuda_plan do, an output buffer of at most 524280 rows, ceil(len / output_stride):
+ * 65535 launch row blocks of 8 rows — else GF_ERR_BAD_PARAMS), selects the
  * pre-compiled kernel instantiation for (pixel_type, distortion_model, digital_lens, interpolation)
  * and allocates device staging for params / matrices (14*max(W,H) f32) / mesh (839 f32) / drawing,
  * plus src/dst staging when the buffers are HOST.  `digital_lens` = GF_LENS_NONE for Option::None. */
