@@ -160,6 +160,21 @@ class ChecksumPlane(C.Structure):
     _fields_ = [("ptr", C.c_void_p), ("row_bytes", C.c_size_t), ("stride", C.c_size_t), ("rows", C.c_size_t)]
 
 
+class SyncPair(C.Structure):
+    """gf_sync_pair: one matched pair of point lists ((ts, pts1), (next_ts, pts2)) of the visual-features sync (visual_features.rs:33-35)."""
+    _fields_ = [("ts_us", C.c_int64), ("next_ts_us", C.c_int64), ("pts1", C.POINTER(C.c_float)), ("pts2", C.POINTER(C.c_float)), ("n", C.c_size_t)]
+
+
+class SyncRange(C.Structure):
+    """gf_sync_range: one sync range (from_us..to_us) and its selected pairs."""
+    _fields_ = [("from_us", C.c_int64), ("to_us", C.c_int64), ("pairs", C.POINTER(SyncPair)), ("n_pairs", C.c_size_t)]
+
+
+class SyncResult(C.Structure):
+    """gf_sync_result: (timestamp, offset or readout time, cost) of find_offsets."""
+    _fields_ = [("timestamp_ms", C.c_double), ("value_ms", C.c_double), ("cost", C.c_double)]
+
+
 # KernelParamsFlags — stabilization/mod.rs:85-98
 FLAG_FIX_COLOR_RANGE, FLAG_HAS_DIGITAL_LENS, FLAG_FILL_WITH_BACKGROUND, FLAG_DRAWING_ENABLED = 1, 2, 4, 8
 FLAG_HORIZONTAL_RS, FLAG_HAS_SOURCE_RECT, FLAG_HAS_OUTPUT_RECT, FLAG_FRAMEBUFFER_INVERTED = 16, 32, 64, 128
@@ -281,6 +296,11 @@ EXPORTS = [
     ("gf_cuda_checksum_planes_dev", C.c_int, [_P(ChecksumPlane), C.c_size_t, C.c_void_p, C.c_void_p]),
     ("gf_cuda_host_register", C.c_int, [C.c_void_p, C.c_size_t]),
     ("gf_cuda_host_unregister", C.c_int, [C.c_void_p]),
+    ("gf_cuda_sync_costs", C.c_int, [C.c_void_p, _P(ComputeParams), C.c_int, C.c_int, C.c_double, _P(SyncPair), C.c_size_t, C.c_void_p, C.c_void_p,
+                                     C.c_size_t, C.c_int, C.c_void_p, C.c_void_p]),
+    ("gf_cuda_find_sync_offsets", C.c_int, [C.c_void_p, _P(ComputeParams), C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
+                                            _P(SyncRange), C.c_size_t, _P(SyncResult), _P(C.c_size_t), C.c_void_p]),
+    ("gf_cuda_sync_last_timing", C.c_int, [C.c_void_p, _P(C.c_double), _P(C.c_double), _P(C.c_size_t)]),
 ]
 
 _lib = None

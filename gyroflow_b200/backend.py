@@ -392,6 +392,21 @@ def zoom_fovs(zp: ZoomParams, timestamps_ms, fov_values):
     return fovs, minimal
 
 
+def _sync_pairs(pairs, keep: list):
+    """[((ts_us, pts1), (next_ts_us, pts2))] as a gf_sync_pair array; the point arrays go into `keep`."""
+    arr = (abi.SyncPair * max(1, len(pairs)))()
+    fp = C.POINTER(C.c_float)
+    for i, ((ts, p1), (nts, p2)) in enumerate(pairs):
+        a = np.ascontiguousarray(p1, dtype=np.float32).reshape(-1, 2); b = np.ascontiguousarray(p2, dtype=np.float32).reshape(-1, 2)
+        if a.shape != b.shape:
+            raise ValueError("pair %d: %d and %d points" % (i, a.shape[0], b.shape[0]))
+        keep += [a, b]
+        arr[i].ts_us, arr[i].next_ts_us = int(ts), int(nts)
+        arr[i].pts1, arr[i].pts2, arr[i].n = a.ctypes.data_as(fp), b.ctypes.data_as(fp), a.shape[0]
+    keep.append(arr)
+    return arr
+
+
 class DeviceGyro:
     """Quaternion tracks resident in HBM + the per-frame matrix kernel (gf_cuda_frame_transform_dev)."""
 
@@ -500,6 +515,52 @@ class DeviceGyro:
         check_call(rc, "gf_cuda_generate_stmaps_dev")
         undists = [b[: 3 * int(nw[i]) * int(nh[i])].view(int(nh[i]), int(nw[i]), 3) for i, b in enumerate(bufs)]
         return dists, undists
+
+    def sync_costs(self, distortion_model: str, digital_lens, scaled_fps, pairs, offsets_ms=None, readout_ms=None, clear_offsets=True, stream=0):
+        """calculate_distance of find_offsets (visual_features.rs:46-84) for every candidate: the cost at offsets_ms[c] (None: 0) with
+        frame_readout_time readout_ms[c] (None: the ComputeParams' own).  pairs: [((ts_us, pts1), (next_ts_us, pts2))] with (n, 2)
+        float32 point lists.  clear_offsets: evaluate the gyro without its sync offsets, as the offset search does.  Returns float64 costs."""
+        offs = None if offsets_ms is None else np.ascontiguousarray(offsets_ms, dtype=np.float64).reshape(-1)
+        rs = None if readout_ms is None else np.ascontiguousarray(readout_ms, dtype=np.float64).reshape(-1)
+        n = offs.size if offs is not None else (rs.size if rs is not None else 0)
+        if offs is not None and rs is not None and offs.size != rs.size:
+            raise ValueError("offsets_ms and readout_ms differ in length")
+        keep = []
+        arr = _sync_pairs(pairs, keep)
+        out = np.zeros(n, np.float64)
+        rc = self._lib.gf_cuda_sync_costs(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
+                                          scaled_fps, arr, len(pairs), offs.ctypes.data if offs is not None else None,
+                                          rs.ctypes.data if rs is not None else None, n, int(clear_offsets), out.ctypes.data, stream or None)
+        check_call(rc, "gf_cuda_sync_costs")
+        return out
+
+    def find_sync_offsets(self, distortion_model: str, digital_lens, scaled_fps, ranges, initial_offset_ms=0.0, search_size_ms=0.0, for_rs=False, stream=0):
+        """find_offsets (visual_features.rs:9-145) of the "Visual features" method (for_rs=False: offsets initial_offset_ms +- search_size_ms / 2
+        every 1 ms, then every 0.01 ms around the best) or of "Estimate rolling shutter" (for_rs=True: readout times).  ranges:
+        [(from_us, to_us, pairs)] with each range's pairs already selected, as for sync_costs.  Returns [(timestamp_ms, value_ms, cost)]."""
+        keep = []
+        arr = (abi.SyncRange * max(1, len(ranges)))()
+        for i, (a, b, pairs) in enumerate(ranges):
+            arr[i].from_us, arr[i].to_us = int(a), int(b)
+            arr[i].pairs = _sync_pairs(pairs, keep); arr[i].n_pairs = len(pairs)
+        out = (abi.SyncResult * max(1, len(ranges)))()
+        n_out = C.c_size_t()
+        rc = self._lib.gf_cuda_find_sync_offsets(self._h, C.byref(self.cp.c), abi.LENS[distortion_model], abi.LENS[digital_lens] if digital_lens else 0,
+                                                 scaled_fps, initial_offset_ms, search_size_ms, int(for_rs), arr, len(ranges), out, C.byref(n_out),
+                                                 stream or None)
+        check_call(rc, "gf_cuda_find_sync_offsets")
+        return [(out[i].timestamp_ms, out[i].value_ms, out[i].cost) for i in range(n_out.value)]
+
+    def estimate_rolling_shutter(self, distortion_model: str, digital_lens, scaled_fps, ranges, stream=0):
+        """The "Estimate rolling shutter" mode (autosync.rs:240-242): find_sync_offsets with for_rs=True.  Returns
+        [(0.0, frame_readout_time_ms, cost)], one entry per range whose readout-time set is not empty (scaled_fps <= 1000)."""
+        return self.find_sync_offsets(distortion_model, digital_lens, scaled_fps, ranges, for_rs=True, stream=stream)
+
+    def sync_timing(self):
+        """The last sync call's host record time and device time in ms, and its number of record chunks (gf_cuda_sync_last_timing)."""
+        h, d, n = C.c_double(), C.c_double(), C.c_size_t()
+        check_call(self._lib.gf_cuda_sync_last_timing(self._h, C.byref(h), C.byref(d), C.byref(n)), "gf_cuda_sync_last_timing")
+        return dict(host_record_ms=h.value, device_ms=d.value, chunks=n.value)
 
     def close(self):
         if self._h:

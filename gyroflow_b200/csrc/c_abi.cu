@@ -697,7 +697,8 @@ GF_API size_t gf_abi_struct_size(int which) {
     case 3: return sizeof(gf_camera_stab);    case 4: return sizeof(gf_keyframe_track); case 5: return sizeof(gf_stab_config);
     case 6: return sizeof(gf_queue_config);   case 7: return sizeof(gf_lens_data);
     case 8: return sizeof(gf_mesh_f64);       case 9: return sizeof(gf_zoom_params);    case 11: return sizeof(gf_queue_plane);
-    case 12: return sizeof(gf_checksum_plane); default: return 0;
+    case 12: return sizeof(gf_checksum_plane); case 13: return sizeof(gf_sync_pair);    case 14: return sizeof(gf_sync_range);
+    case 15: return sizeof(gf_sync_result);    default: return 0;
     }
 }
 GF_API const char* gf_cuda_backend_name(void) { return "CUDA"; }

@@ -26,6 +26,8 @@ struct gf_cuda_gyro {
     // share, kept from job to job, and the end of the last job on its stream
     std::unique_ptr<gf_cuda_ctx, gf::Deleter<gf_cuda_destroy>> stmap_ctx;
     gf::Event stmap_done;
+    // the last visual-features sync call (gf_cuda_sync_last_timing)
+    double sync_host_ms = 0.0, sync_device_ms = 0.0; size_t sync_chunks = 0;
 
     // the stream of a call: the caller's `cu_stream`, or this object's own when it is NULL
     cudaStream_t stream_of(void* cu_stream) const { return cu_stream ? (cudaStream_t)cu_stream : stream.get(); }

@@ -12,8 +12,11 @@
 // The rotations are f64, and the slerp's acos / sin differ from glibc's in the last f64 bit, so with the rotation on parity with the
 // oracle is to 1e-6.  With suppress_rotation set no libm result reaches the output and the point path is bit-exact.
 #include <cuda_runtime.h>
+#include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstring>
+#include <thread>
 #include <vector>
 #include "lens_models.cuh"
 #include "warp_kernel.cuh"      // the warp's stage functions: lens correction, refraction, mesh
@@ -261,14 +264,107 @@ __global__ void __launch_bounds__(128) stmap_size_kernel(const PointFrame* __res
     out[blockIdx.x] = make_int2(as_size(fw), as_size(fh));
 }
 
+// ---- visual-features sync: calculate_distance (synchronization/find_offset/visual_features.rs:46-84) ----
+constexpr int SYNC_THREADS = 256;
+constexpr unsigned SYNC_SMEM_KEYS = 8192;       // distance keys per pair held in shared memory; larger pairs keep them in global scratch
+constexpr uint32_t SYNC_NO_KEY = 0xFFFFFFFFu;   // a point pair outside the frame; every real key is <= 2^31 (frames of <= 32768 px a side)
+struct SyncPairDev { uint32_t off, n; };        // a pair's first point in the concatenated lists, and its point count
+
+__device__ __forceinline__ uint64_t block_sum_u64(uint64_t v, uint64_t* red) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+    __syncthreads();                            // `red` may still be read from the previous reduction
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    uint64_t s = 0;
+    for (int w = 0; w < SYNC_THREADS / 32; ++w) s += red[w];
+    return s;
+}
+
+// One CTA per (candidate, pair).  recs: 2 PointFrames per CTA (the pair's two timestamps at this candidate), blockIdx.x = candidate *
+// n_pairs + pair.  Every thread undistorts its points, keeps the truncated f32 squared distance of each point pair inside the frame as a
+// 32-bit key, the CTA finds the k-th smallest key T by radix select (one 256-bin histogram per byte) and adds
+// sum(keys < T) + (k - count(keys < T)) * T — the sum of the k smallest — to sums[candidate] with an integer atomic, whose order does not
+// matter.
+template <int LENS, int DIGITAL>
+__global__ void __launch_bounds__(SYNC_THREADS) sync_cost_kernel(const PointFrame* __restrict__ recs, const SyncPairDev* __restrict__ pairs, unsigned n_pairs,
+                                                                 const float2* __restrict__ pts1, const float2* __restrict__ pts2, float w, float h,
+                                                                 uint32_t* __restrict__ scratch, size_t scratch_stride, unsigned long long* __restrict__ sums) {
+    extern __shared__ uint32_t skeys[];
+    __shared__ unsigned hist[256];
+    __shared__ uint64_t red[SYNC_THREADS / 32];
+    __shared__ uint32_t s_prefix, s_rank;
+    const unsigned cand = blockIdx.x / n_pairs;
+    const SyncPairDev pr = pairs[blockIdx.x % n_pairs];
+    if (pr.n == 0) return;
+    uint32_t* keys = pr.n <= SYNC_SMEM_KEYS ? skeys : scratch + (size_t)cand * scratch_stride + pr.off;
+    const PointFrame& S1 = recs[2 * (size_t)blockIdx.x];
+    const PointFrame& S2 = recs[2 * (size_t)blockIdx.x + 1];
+    uint64_t valid = 0;
+    for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
+        const float2 a = pts1[pr.off + i], b = pts2[pr.off + i];
+        float x1, y1, x2, y2;
+        undistort_point_rs<LENS, DIGITAL>(S1.A, S1.F, a.x, a.y, (size_t)i, x1, y1);
+        undistort_point_rs<LENS, DIGITAL>(S2.A, S2.F, b.x, b.y, (size_t)i, x2, y2);
+        uint32_t key = SYNC_NO_KEY;
+        if (x1 > 0.0f && x1 < w && y1 > 0.0f && y1 < h && x2 > 0.0f && x2 < w && y2 > 0.0f && y2 < h) {      // :66-67
+            const float dx = x2 - x1, dy = y2 - y1;
+            key = (uint32_t)(dx * dx + dy * dy);         // `dist as u64` (no contraction: built with -fmad=false)
+            ++valid;
+        }
+        keys[i] = key;
+    }
+    const uint64_t m = block_sum_u64(valid, red);
+    const uint64_t k = (uint64_t)((double)m * 0.9);     // (len as f64 * 0.9) as usize
+    if (k == 0) return;
+    if (threadIdx.x == 0) { s_prefix = 0; s_rank = (uint32_t)k; }
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        for (int b = threadIdx.x; b < 256; b += SYNC_THREADS) hist[b] = 0;
+        __syncthreads();                                 // also publishes s_prefix / s_rank and (first pass) every key
+        const uint32_t prefix = s_prefix, hi = shift == 24 ? 0u : (0xFFFFFFFFu << (shift + 8));
+        for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
+            const uint32_t key = keys[i];
+            if ((key & hi) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x < 32) {                          // one warp: lane l scans bins 8l..8l+7
+            const int l = threadIdx.x;
+            unsigned c[8], own = 0;
+            for (int j = 0; j < 8; ++j) { c[j] = hist[8 * l + j]; own += c[j]; }
+            unsigned incl = own;
+            for (int o = 1; o < 32; o <<= 1) { const unsigned t = __shfl_up_sync(0xffffffffu, incl, o); if (l >= o) incl += t; }
+            const uint32_t rank = s_rank;
+            unsigned before = incl - own;
+            if (before < rank && rank <= incl) {         // exactly one lane holds the bin of the rank-th key
+                int j = 0;
+                while (before + c[j] < rank) before += c[j++];
+                s_rank = rank - before;
+                s_prefix = prefix | ((uint32_t)(8 * l + j) << shift);
+            }
+        }
+        __syncthreads();                                 // the scan has read `hist` before the next pass clears it
+    }
+    const uint32_t T = s_prefix;
+    uint64_t below = 0, n_below = 0;
+    for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
+        const uint32_t key = keys[i];
+        if (key < T) { below += key; ++n_below; }
+    }
+    below = block_sum_u64(below, red);
+    n_below = block_sum_u64(n_below, red);
+    if (threadIdx.x == 0) atomicAdd(&sums[cand], (unsigned long long)(below + (k - n_below) * (uint64_t)T));
+}
+
 // The kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye
 // model, GoPro warp the GoPro model).
 struct ZoomKernels {
     void (*find_fov)(const ZoomArgs, const ZoomFrame*, double*);
     void (*points)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
     void (*stmap_size)(const PointFrame*, float, float, int2*);
+    void (*sync_cost)(const PointFrame*, const SyncPairDev*, unsigned, const float2*, const float2*, float, float, uint32_t*, size_t, unsigned long long*);
 };
-template <int LENS, int DIGITAL> ZoomKernels kernels_of() { return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL> }; }
+template <int LENS, int DIGITAL> ZoomKernels kernels_of() {
+    return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL>, sync_cost_kernel<LENS, DIGITAL> };
+}
 template <int LENS> ZoomKernels pick_digital(int digital) {
     switch (digital) {
     case GF_LENS_NONE:             return kernels_of<LENS, GF_LENS_NONE>();
@@ -279,7 +375,7 @@ template <int LENS> ZoomKernels pick_digital(int digital) {
     case GF_LENS_GOPRO_WARP:       if (LENS == GF_LENS_GOPRO) return kernels_of<LENS, GF_LENS_GOPRO_WARP>();                break;
     default: break;
     }
-    return { nullptr, nullptr, nullptr };
+    return { nullptr, nullptr, nullptr, nullptr };
 }
 ZoomKernels pick_kernels(int lens, int digital) {
     switch (lens) {
@@ -292,7 +388,7 @@ ZoomKernels pick_kernels(int lens, int digital) {
     case GF_LENS_SONY:               return pick_digital<GF_LENS_SONY>(digital);
     case GF_LENS_GENERIC_POLYNOMIAL: return pick_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
     case GF_LENS_GOPRO:              return pick_digital<GF_LENS_GOPRO>(digital);
-    default: return { nullptr, nullptr, nullptr };
+    default: return { nullptr, nullptr, nullptr, nullptr };
     }
 }
 
@@ -370,6 +466,146 @@ static PointFrame point_frame(const gf_cuda_gyro* g, const gf_compute_params& cp
 }
 
 bool gf::point_path_supported(int lens, int digital) { return pick_kernels(lens, digital).points != nullptr; }
+
+// ---- visual-features sync on the host: argument checks, point records in chunks of candidates, the two-stage search ----
+
+// frame_at_timestamp (lib.rs:2069): `(timestamp_ms * (fps / 1000.0)).round() as i32`, then `as usize`, so a negative frame wraps
+static size_t sync_frame(double timestamp_ms, double fps) {
+    const double r = round(timestamp_ms * (fps / 1000.0));
+    const int32_t i = r != r ? 0 : (r <= -2147483648.0 ? INT32_MIN : (r >= 2147483647.0 ? INT32_MAX : (int32_t)r));
+    return (size_t)(int64_t)i;
+}
+
+constexpr size_t kSyncChunkBytes = 64u << 20;          // records (and global key scratch) of one chunk of candidates
+constexpr double kMaxSyncCandidates = 1e7;             // per search stage
+
+// The pairs of one range on the device, and what every cost evaluation over them shares.
+struct SyncJob {
+    gf_cuda_gyro* g; const gf_compute_params* cp; int model; double fps; int clear;
+    const gf_sync_pair* pairs; size_t n_pairs;
+    ZoomKernels k; cudaStream_t st;
+    size_t total = 0; uint32_t max_n = 0;
+    GrowBuf<float2> d_p1, d_p2; GrowBuf<SyncPairDev> d_pairs; GrowBuf<PointFrame> d_recs; GrowBuf<uint32_t> d_scratch;
+    GrowBuf<unsigned long long> d_sums;
+};
+
+// Everything the cost calls refuse, before any CUDA call: GF_OK or the error, with `who` in the message.
+static int sync_check(const char* who, const gf_cuda_gyro* g, const gf_compute_params* cp, int model, int digital, double fps,
+                      const gf_sync_pair* pairs, size_t n_pairs) {
+    const std::string w(who);
+    if (!g || !cp || (n_pairs && !pairs)) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": null argument");
+    if (!pick_kernels(model, digital).sync_cost) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, w + ": no point-path kernel for this (lens, digital lens) pair");
+    if (cp->width < 1 || cp->height < 1 || cp->width > 32768 || cp->height > 32768)
+        return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": frame size outside 1..32768");
+    if (!(fps > 0.0) || !std::isfinite(fps)) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": scaled_fps must be finite and > 0");
+    unsigned __int128 total = 0;
+    for (size_t p = 0; p < n_pairs; ++p) {
+        if (pairs[p].n && (!pairs[p].pts1 || !pairs[p].pts2)) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": pair " + std::to_string(p) + " has a null point list");
+        total += pairs[p].n;
+    }
+    if (total > 0xFFFFFFFFu) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": more than 2^32 - 1 points");
+    // every distance is below width^2 + height^2, so below this bound the f64 sum of the reference is exact and equals the integer sum
+    const unsigned __int128 d2 = (unsigned __int128)cp->width * cp->width + (unsigned __int128)cp->height * cp->height;
+    if (total * d2 >= ((unsigned __int128)1 << 53))
+        return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": sum(n) * (width^2 + height^2) reaches 2^53, the cost would not be exact in f64");
+    return GF_OK;
+}
+
+static int sync_setup(SyncJob& J) {
+    std::vector<float2> h1, h2; std::vector<SyncPairDev> hp(J.n_pairs);
+    for (size_t p = 0; p < J.n_pairs; ++p) {
+        const gf_sync_pair& P = J.pairs[p];
+        hp[p] = SyncPairDev{ (uint32_t)h1.size(), (uint32_t)P.n };
+        J.max_n = std::max(J.max_n, (uint32_t)P.n);
+        for (size_t i = 0; i < P.n; ++i) { h1.push_back(make_float2(P.pts1[2 * i], P.pts1[2 * i + 1])); h2.push_back(make_float2(P.pts2[2 * i], P.pts2[2 * i + 1])); }
+    }
+    J.total = h1.size();
+    if (J.total == 0) return GF_OK;
+    CK(nullptr, J.d_p1.reserve(J.total, J.st));
+    CK(nullptr, J.d_p2.reserve(J.total, J.st));
+    CK(nullptr, J.d_pairs.reserve(J.n_pairs, J.st));
+    CK(nullptr, cudaMemcpyAsync(J.d_p1.ptr, h1.data(), J.total * sizeof(float2), cudaMemcpyHostToDevice, J.st));
+    CK(nullptr, cudaMemcpyAsync(J.d_p2.ptr, h2.data(), J.total * sizeof(float2), cudaMemcpyHostToDevice, J.st));
+    CK(nullptr, cudaMemcpyAsync(J.d_pairs.ptr, hp.data(), J.n_pairs * sizeof(SyncPairDev), cudaMemcpyHostToDevice, J.st));
+    CK(nullptr, cudaStreamSynchronize(J.st));           // the staging vectors go out of scope
+    return GF_OK;
+}
+
+// The records of candidates c0 .. c0 + nc: per pair, what gf_cuda_undistort_points builds for each of its two timestamps, on all host
+// threads (point_frame only reads).
+static void sync_records(const SyncJob& J, const double* offs, const double* rs, size_t c0, size_t nc, PointFrame* out) {
+    auto work = [&](size_t a, size_t b) {
+        gf_compute_params cp = *J.cp;
+        if (J.clear) { cp.gyro_offset_ms = 0.0; cp.sync_offset_ts_us = nullptr; cp.sync_offset_ms = nullptr; cp.n_sync_offsets = 0; }
+        for (size_t c = a; c < b; ++c) {
+            const double off = offs ? offs[c0 + c] : 0.0;
+            if (rs) cp.frame_readout_time = rs[c0 + c];
+            for (size_t p = 0; p < J.n_pairs; ++p) {
+                const gf_sync_pair& P = J.pairs[p];
+                const double t1 = (double)P.ts_us / 1000.0 - off, t2 = (double)P.next_ts_us / 1000.0 - off;     // :60-64
+                PointFrame* r = out + 2 * (c * J.n_pairs + p);
+                r[0] = point_frame(J.g, cp, J.model, sync_frame(t1, J.fps), t1, false, 1.0);
+                r[1] = point_frame(J.g, cp, J.model, sync_frame(t2, J.fps), t2, false, 1.0);
+                if (J.clear) r[0].A.offsets = r[1].A.offsets = SyncOffsets{ nullptr, nullptr, 0, 0.0 };
+            }
+        }
+    };
+    const size_t nt = std::min<size_t>({ (size_t)std::max(1u, std::thread::hardware_concurrency()), 16, (nc * J.n_pairs + 63) / 64, nc });
+    if (nt <= 1) { work(0, nc); return; }
+    std::vector<std::thread> th;
+    for (size_t t = 0; t < nt; ++t) th.emplace_back(work, nc * t / nt, nc * (t + 1) / nt);
+    for (auto& t : th) t.join();
+}
+
+// calculate_distance of n candidates over the job's pairs into out[]
+static int sync_run(SyncJob& J, const double* offs, const double* rs, size_t n, double* out) {
+    if (n == 0) return GF_OK;
+    if (J.total == 0) { for (size_t c = 0; c < n; ++c) out[c] = 0.0; return GF_OK; }
+    const bool big = J.max_n > SYNC_SMEM_KEYS;
+    const size_t per_cand = 2 * J.n_pairs * sizeof(PointFrame) + (big ? J.total * sizeof(uint32_t) : 0);
+    const size_t chunk = std::min({ std::max<size_t>(1, kSyncChunkBytes / per_cand), n, (size_t)0x7fffffff / J.n_pairs });
+    std::vector<PointFrame> host(2 * chunk * J.n_pairs);
+    CK(nullptr, J.d_recs.reserve(host.size(), J.st));
+    if (big) CK(nullptr, J.d_scratch.reserve(chunk * J.total, J.st));
+    CK(nullptr, J.d_sums.reserve(n, J.st));
+    CK(nullptr, cudaMemsetAsync(J.d_sums.ptr, 0, n * sizeof(unsigned long long), J.st));
+    cudaEvent_t e[2] = {};
+    CK(nullptr, cudaEventCreate(&e[0]));
+    const Event ev0(e[0]);
+    CK(nullptr, cudaEventCreate(&e[1]));
+    const Event ev1(e[1]);
+    const unsigned smem = std::min<unsigned>(J.max_n, SYNC_SMEM_KEYS) * (unsigned)sizeof(uint32_t);
+    float ms = 0.0f;
+    for (size_t c0 = 0; c0 < n; c0 += chunk) {
+        const size_t nc = std::min(chunk, n - c0);
+        const auto t0 = std::chrono::steady_clock::now();
+        sync_records(J, offs, rs, c0, nc, host.data());
+        J.g->sync_host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        if (c0) { CK(nullptr, cudaEventSynchronize(e[1])); CK(nullptr, cudaEventElapsedTime(&ms, e[0], e[1])); J.g->sync_device_ms += ms; }
+        // pageable source: the call returns once the records are staged, so the next chunk may overwrite `host`
+        CK(nullptr, cudaMemcpyAsync(J.d_recs.ptr, host.data(), 2 * nc * J.n_pairs * sizeof(PointFrame), cudaMemcpyHostToDevice, J.st));
+        CK(nullptr, cudaEventRecord(e[0], J.st));
+        J.k.sync_cost<<<(unsigned)(nc * J.n_pairs), SYNC_THREADS, smem, J.st>>>(J.d_recs.ptr, J.d_pairs.ptr, (unsigned)J.n_pairs, J.d_p1.ptr, J.d_p2.ptr,
+                                                                               (float)J.cp->width, (float)J.cp->height, big ? J.d_scratch.ptr : nullptr,
+                                                                               J.total, J.d_sums.ptr + c0);
+        CK(nullptr, cudaGetLastError());
+        CK(nullptr, cudaEventRecord(e[1], J.st));
+        ++J.g->sync_chunks;
+    }
+    std::vector<unsigned long long> sums(n);
+    CK(nullptr, cudaMemcpyAsync(sums.data(), J.d_sums.ptr, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, J.st));
+    CK(nullptr, cudaStreamSynchronize(J.st));
+    CK(nullptr, cudaEventElapsedTime(&ms, e[0], e[1])); J.g->sync_device_ms += ms;
+    for (size_t c = 0; c < n; ++c) out[c] = (double)sums[c];        // exact: every sum is below 2^53 (sync_check)
+    return GF_OK;
+}
+
+// find_min under reduce_with (:87): `if a.1 < b.1 { a } else { b }` folded in order keeps the LAST of equal minima
+static size_t sync_last_min(const std::vector<double>& cost) {
+    size_t b = 0;
+    for (size_t i = 1; i < cost.size(); ++i) if (!(cost[b] < cost[i])) b = i;
+    return b;
+}
 
 // ---- the temporal filters of zoom_dynamic.rs, on the host like in the reference ----
 
@@ -607,6 +843,75 @@ GF_API int gf_cuda_calculate_fovs(gf_cuda_gyro* g, const gf_compute_params* cp, 
     const int rc = gf_cuda_find_fovs(g, cp, distortion_model, digital_lens, timestamps_ms, n, zp->fov_algorithm_margin, fov_values.data(), cu_stream);
     if (rc != GF_OK) return rc;
     return gf_zoom_fovs(zp, timestamps_ms, fov_values.data(), n, out_fovs, out_minimal_fovs);
+}
+
+GF_API int gf_cuda_sync_costs(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, double scaled_fps,
+                              const gf_sync_pair* pairs, size_t n_pairs, const double* offsets_ms, const double* readout_ms,
+                              size_t n_candidates, int clear_offsets, double* out_costs, void* cu_stream) {
+    int rc = sync_check("gf_cuda_sync_costs", g, cp, distortion_model, digital_lens, scaled_fps, pairs, n_pairs);
+    if (rc != GF_OK) return rc;
+    if (n_candidates && !out_costs) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_sync_costs: null argument");
+    g->sync_host_ms = g->sync_device_ms = 0.0; g->sync_chunks = 0;
+    if (n_candidates == 0) return GF_OK;
+    CK(nullptr, cudaSetDevice(g->device));
+    SyncJob J{ g, cp, distortion_model, scaled_fps, clear_offsets != 0, pairs, n_pairs, pick_kernels(distortion_model, digital_lens), g->stream_of(cu_stream) };
+    if ((rc = sync_setup(J)) != GF_OK) return rc;
+    return sync_run(J, offsets_ms, readout_ms, n_candidates, out_costs);
+}
+
+GF_API int gf_cuda_find_sync_offsets(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, double scaled_fps,
+                                     double initial_offset_ms, double search_size_ms, int for_rs,
+                                     const gf_sync_range* ranges, size_t n_ranges, gf_sync_result* out, size_t* n_out, void* cu_stream) {
+    int rc = sync_check("gf_cuda_find_sync_offsets", g, cp, distortion_model, digital_lens, scaled_fps, nullptr, 0);
+    if (rc != GF_OK) return rc;
+    if (!n_out || (n_ranges && (!ranges || !out))) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_find_sync_offsets: null argument");
+    for (size_t r = 0; r < n_ranges; ++r)
+        if ((rc = sync_check("gf_cuda_find_sync_offsets", g, cp, distortion_model, digital_lens, scaled_fps, ranges[r].pairs, ranges[r].n_pairs)) != GF_OK) return rc;
+    *n_out = 0;
+    g->sync_host_ms = g->sync_device_ms = 0.0; g->sync_chunks = 0;
+    // the first stage: every 1 ms (:92-99, :118-125)
+    std::vector<double> coarse;
+    if (for_rs) {
+        const double max_rs = 1000.0 / scaled_fps;
+        if (max_rs >= kMaxSyncCandidates / 2) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_find_sync_offsets: more than 1e7 readout times (scaled_fps too small)");
+        const int64_t steps = (int64_t)max_rs;                                   // `as isize`
+        for (int64_t i = -steps; i < steps; ++i) coarse.push_back((double)i);
+    } else if (search_size_ms >= kMaxSyncCandidates) {
+        return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_find_sync_offsets: search_size of 1e7 ms or more");
+    } else {
+        const size_t steps = search_size_ms > 0.0 ? (size_t)search_size_ms : 0;       // `as usize` (NaN: 0)
+        for (size_t i = 0; i < steps; ++i) coarse.push_back(initial_offset_ms + (-(search_size_ms / 2.0) + (double)i));
+    }
+    if (n_ranges == 0 || coarse.empty()) return GF_OK;
+    CK(nullptr, cudaSetDevice(g->device));
+    for (size_t r = 0; r < n_ranges; ++r) {
+        const gf_sync_range& R = ranges[r];
+        SyncJob J{ g, cp, distortion_model, scaled_fps, for_rs ? 0 : 1, R.pairs, R.n_pairs, pick_kernels(distortion_model, digital_lens), g->stream_of(cu_stream) };
+        if ((rc = sync_setup(J)) != GF_OK) return rc;
+        // offsets for the offset search, readout times (at offset 0) for the rolling-shutter estimate
+        auto costs = [&](const std::vector<double>& cand, std::vector<double>& cost) {
+            cost.assign(cand.size(), 0.0);
+            return sync_run(J, for_rs ? nullptr : cand.data(), for_rs ? cand.data() : nullptr, cand.size(), cost.data());
+        };
+        std::vector<double> cost, fine(200), cost2;
+        if ((rc = costs(coarse, cost)) != GF_OK) return rc;
+        const double lowest = coarse[sync_last_min(cost)];
+        for (int i = 0; i < 200; ++i) fine[i] = lowest - 1.0 + ((double)i * 0.01);          // then refine to 0.01 ms (:100-108, :126-134)
+        if ((rc = costs(fine, cost2)) != GF_OK) return rc;
+        const size_t b = sync_last_min(cost2);
+        if (for_rs) { out[(*n_out)++] = gf_sync_result{ 0.0, fine[b], cost2[b] }; continue; }
+        const double middle = ((double)R.from_us + (double)(int64_t)((uint64_t)R.to_us - (uint64_t)R.from_us) / 2.0) / 1000.0;   // :139
+        if (fabs(fine[b] - initial_offset_ms) < search_size_ms * 0.9) out[(*n_out)++] = gf_sync_result{ middle, fine[b], cost2[b] };
+    }
+    return GF_OK;
+}
+
+GF_API int gf_cuda_sync_last_timing(const gf_cuda_gyro* g, double* host_record_ms, double* device_ms, size_t* chunks) {
+    if (!g) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_sync_last_timing: null argument");
+    if (host_record_ms) *host_record_ms = g->sync_host_ms;
+    if (device_ms) *device_ms = g->sync_device_ms;
+    if (chunks) *chunks = g->sync_chunks;
+    return GF_OK;
 }
 
 } // extern "C"

@@ -207,7 +207,8 @@ GF_API int         gf_cuda_supports(const gf_buffer_desc* in, const gf_buffer_de
 GF_API const char* gf_cuda_version(void);
 /* sizeof() of the structs that cross this ABI, for binding generators and their tests: 0 gf_kernel_params, 1 gf_buffer_desc,
  * 2 gf_compute_params, 3 gf_camera_stab, 4 gf_keyframe_track, 5 gf_stab_config, 6 gf_queue_config, 7 gf_lens_data, 8 gf_mesh_f64,
- * 9 gf_zoom_params, 11 gf_queue_plane, 12 gf_checksum_plane; 0 for any other index (10 is unassigned). */
+ * 9 gf_zoom_params, 11 gf_queue_plane, 12 gf_checksum_plane, 13 gf_sync_pair, 14 gf_sync_range, 15 gf_sync_result; 0 for any other
+ * index (10 is unassigned). */
 GF_API size_t gf_abi_struct_size(int which);
 
 /* ---- lens plugin surface: DistortionModel::from_name / id  distortion_models/mod.rs:79-90 -- */
@@ -519,6 +520,49 @@ GF_API int gf_cuda_generate_stmaps_dev(gf_cuda_gyro* g, const gf_compute_params*
                                        size_t dist_capacity_floats, size_t undist_capacity_floats, void* cu_stream);
 
 GF_API int gf_zoom_dynamic_compute(const double* fov_minimal, size_t n, double window_s, double fps, int method, double* out);
+
+/* ------------------------------------------------------------------------------------------
+ * Visual-features sync — the arithmetic of find_offsets (src/core/synchronization/find_offset/visual_features.rs:9-145), which
+ * the reference runs for the "Visual features" offset method (synchronization/mod.rs:385, for_rs = false) and for "Estimate rolling
+ * shutter" (autosync.rs:240-242, for_rs = true).  Optical flow, feature matching and the choice of pairs stay with the caller: matched
+ * point lists go in, (timestamp, offset, cost) comes out.
+ * A candidate's cost is calculate_distance (:46-84): every pair's points go through undistort_points_with_rolling_shutter at
+ * ts_us / 1000 - offset and next_ts_us / 1000 - offset (frame = frame_at_timestamp(that timestamp, scaled_fps), lib.rs:2069, whose
+ * negative values wrap and find no per-frame entry), each record exactly what gf_cuda_undistort_points builds for that list, timestamp
+ * and frame with use_fovs = 0 and lens_correction_amount = 1.  A point pair counts when both points lie strictly inside
+ * (0, width) x (0, height); its distance is the f32 squared distance truncated to an integer, and a pair contributes the sum of its
+ * smallest (count as f64 * 0.9) as usize distances.  The cost is the exact sum over all pairs (an integer below 2^53: a job whose bound
+ * sum(n) * (width^2 + height^2) reaches 2^53 is refused with GF_ERR_BAD_PARAMS).  Frames are limited to 32768 pixels per side.
+ * Both calls are synchronous; the reference's progress callback and cancel flag have no counterpart.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct gf_sync_pair {            /* one get_of_lines_for_timestamp result ((ts, pts1), (next_ts, pts2)), visual_features.rs:33-35 */
+    int64_t ts_us, next_ts_us;
+    const float* pts1;                   /* n x (x, y), frame pixels, at ts_us */
+    const float* pts2;                   /* n x (x, y), the matched points at next_ts_us */
+    size_t n;
+} gf_sync_pair;
+typedef struct gf_sync_range { int64_t from_us, to_us; const gf_sync_pair* pairs; size_t n_pairs; } gf_sync_range;
+typedef struct gf_sync_result { double timestamp_ms, value_ms, cost; } gf_sync_result;   /* (timestamp, offset or readout time, cost) */
+/* calculate_distance for n_candidates candidates over one range's pairs: out_costs[c] is the cost at offset offsets_ms[c] (NULL: 0)
+ * with frame_readout_time readout_ms[c] (NULL: cp's; a candidate may be negative).  clear_offsets != 0 evaluates the gyro without its
+ * sync offsets (GyroSource::clear_offsets, :12-15: both the uploaded multi-point offsets and gyro_offset_ms read as 0). */
+GF_API int gf_cuda_sync_costs(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, double scaled_fps,
+                              const gf_sync_pair* pairs, size_t n_pairs, const double* offsets_ms, const double* readout_ms,
+                              size_t n_candidates, int clear_offsets, double* out_costs, void* cu_stream);
+/* find_offsets over every range, in order.  for_rs = 0, the offset search (sync offsets cleared): offsets initial + (-(search_size / 2)
+ * + i) for i in 0..search_size as usize, then lowest - 1 + i * 0.01 for i in 0..200; the lowest cost wins, the LAST one among equal
+ * costs (rayon's reduce_with of find_min, :87); kept when |lowest - initial| < 0.9 * search_size, with timestamp
+ * (from + (to - from) / 2) / 1000 ms.  for_rs = 1, the rolling-shutter estimate (sync offsets kept, offset 0): readout times i for
+ * i in -(1000 / fps) as isize..(1000 / fps) as isize, then the same refinement; timestamp 0.  A range whose first stage is empty has
+ * no entry.  `out` holds n_ranges entries; *n_out receives the number written.  The caller selects each range's pairs
+ * ((from..to).contains(ts), equal non-empty lists) and runs the negated initial offset itself (autosync.rs:250-262). */
+GF_API int gf_cuda_find_sync_offsets(gf_cuda_gyro* g, const gf_compute_params* cp, int distortion_model, int digital_lens, double scaled_fps,
+                                     double initial_offset_ms, double search_size_ms, int for_rs,
+                                     const gf_sync_range* ranges, size_t n_ranges, gf_sync_result* out, size_t* n_out, void* cu_stream);
+/* The last gf_cuda_sync_costs / gf_cuda_find_sync_offsets call on `g`: milliseconds the host spent building point records, milliseconds
+ * the cost kernels ran on the device (CUDA events), and the number of record chunks (records are built and uploaded in chunks of
+ * candidates, so memory stays bounded).  Any pointer may be NULL. */
+GF_API int gf_cuda_sync_last_timing(const gf_cuda_gyro* g, double* host_record_ms, double* device_ms, size_t* chunks);
 
 /* ------------------------------------------------------------------------------------------
  * zooming::calculate_fovs (src/core/zooming/mod.rs:35-70) — what the reference runs before a render (lib.rs:515-523).
