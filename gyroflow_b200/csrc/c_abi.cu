@@ -261,7 +261,8 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     if (A.interior_span[0] < 0 || A.interior_span[1] < 0 || A.interior_span[0] >= (1 << 17) || A.interior_span[1] >= (1 << 17) || A.rs_lim >= (1 << 22)) { A.interior_span[0] = 0; A.interior_span[1] = 0; A.feat |= F_WILD; }   // no interior at all
     // source-rect maps of the packed kernel (see map_apply_x2): in_min == 0, moderate non-zero scale, divisor <= 2^20, |c| >= 2^-10,
     // source rect inside [0, 2^16) so that every coordinate the rounding shortcut cannot represent is outside the image anyway
-    auto smap_ok = [](const MapC& m) { return m.fast_div && m.in_min == 0.0f && m.mul != 0.0f && tame(m.mul) && m.div > 0.0f && m.div <= 0x1p20f && std::isfinite(m.add) && fabsf(m.add) <= 0x1p16f; };
+    // (in_min must be +0, not -0: map_apply_x2 skips x - in_min)
+    auto smap_ok = [](const MapC& m) { return m.fast_div && m.in_min == 0.0f && !std::signbit(m.in_min) && m.mul != 0.0f && tame(m.mul) && m.div > 0.0f && m.div <= 0x1p20f && std::isfinite(m.add) && fabsf(m.add) <= 0x1p16f; };
     if (!(smap_ok(A.smap_x) && smap_ok(A.smap_y) && fabsf(p->c[0]) >= 0x1p-10f && fabsf(p->c[1]) >= 0x1p-10f &&
           A.src_rect[0] >= 0 && A.src_rect[1] >= 0 && A.src_rect[2] <= (1 << 16) && A.src_rect[3] <= (1 << 16))) A.feat |= F_WILD;
     // pixel-index maps of the packed kernel: identity, or a positive moderate scale (map_apply_int_lean in warp_kernel_x2.cuh)
@@ -276,6 +277,7 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
     A.hot.wbias[0] = 0x4affffff + (tame_rect ? 64 * A.src_rect[0] : 0); A.hot.wbias[1] = 0x4affffff + (tame_rect ? 64 * A.src_rect[1] : 0);
     A.hot.wlim[0] = 64u * (unsigned)A.interior_span[0] + 63u; A.hot.wlim[1] = 64u * (unsigned)A.interior_span[1] + 63u;
     A.hot.src = tame_rect ? src + ((long long)A.src_rect[1] * (long long)p->stride + (long long)A.src_rect[0] * (long long)bpp) : src;
+    A.hot.full = 0;
     if (A.omap_x.identity && A.omap_y.identity && A.omap_x.add == truncf(A.omap_x.add) && A.omap_y.add == truncf(A.omap_y.add) &&
         fabsf(A.omap_x.add) < 0x1p20f && fabsf(A.omap_y.add) < 0x1p20f && fabsf(A.omap_x.in_min) < 0x1p20f && fabsf(A.omap_y.in_min) < 0x1p20f) {
         A.hot.x_off = (int)A.omap_x.add - (int)A.omap_x.in_min; A.hot.y_off = (int)A.omap_y.add - (int)A.omap_y.in_min;
@@ -293,6 +295,10 @@ void fill_uniforms(WarpArgs& A, const Combo& c) {
             else A.feat |= F_SHORTROW;
         }
         A.feat |= F_INTPRO;
+        // the packed launch (32 x 4 threads of two rows each) covers exactly [0, out_cols) x [0, out_rows), and every pixel of it is written
+        auto plus_zero = [](float v) { return v == 0.0f && !std::signbit(v); };
+        A.hot.full = (A.feat & (F_WILD | F_SHORTROW)) == 0 && A.hot.x0 == 0 && A.hot.x1 == A.out_cols && A.hot.y0 == 0 && A.hot.y1 == A.out_rows &&
+                     A.out_cols % GF_BLOCK_X == 0 && A.out_rows % (2 * kPackedBlockY) == 0 && plus_zero(A.smap_x.add) && plus_zero(A.smap_y.add);
     }
 }
 

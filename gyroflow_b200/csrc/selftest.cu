@@ -149,7 +149,7 @@ __global__ void filter_check_kernel(const FilterCfg* __restrict__ cfgs, const fl
             const float _y = (px * C.m[3] + py * C.m[4]) + C.m[5];
             const float _w = (px * C.m[6] + py * C.m[7]) + C.m[8];
             using L = Lens2<GF_LENS_OPENCV_FISHEYE>;
-            if (!(__float_as_uint(_w) - L::kWLo < L::kWSpan)) continue;
+            if (!L::divisors_ok(_w, _w)) continue;                                   // the kernel's divisor test
             const float tvc = L::approx_v(_x, _y, _w, P, rtab);
             const float tv = tvc + P.c[1];
             if (!(fabsf(tv) < 0x1p20f)) continue;                                     // also r^2 at or above the cap: NaN rows

@@ -97,7 +97,7 @@ constexpr int GF_RADIAL_FIT_ROWS = (14 + 30) * 16;
 
 // Tolerance of the filtered pre-pass's certificate (profiles/FILTER_ANALYSIS.md): eps = (rho + 2^-22) |t - c_y| + 2^-22 |c_y|, as
 // X2Filter's eps_rel and eps_abs.
-constexpr float kFilterRho = 0x1p-17f;
+constexpr float kFilterRho = 0x1.7p-18f;      // 92u: rho + 2^-22 = 96u = 0x1.8p-19, twice the first-order 45u plus 6u
 struct FilterEps { float rel, abs; };
 GF_HD FilterEps filter_eps(float c_y, float rho = kFilterRho) { return { rho + 0x1p-22f, 0x1p-22f * fabsf(c_y) }; }
 
@@ -157,6 +157,10 @@ struct WarpArgs {
         // in warp_kernel_x2.cuh), and the footprint is interior iff that word, unsigned, is <= wlim = 64 * span + 63
         int wbias[2];
         unsigned wlim[2];
+        // 1 = the packed launch's grid is exactly the written part of the output (F_INTPRO, x0 = y0 = 0, x1 = out_cols, y1 = out_rows,
+        // whole 32 x 8 blocks, no F_SHORTROW) and both source-rect maps add +0: without a digital lens the kernel then runs
+        // warp_x2_body's FULL form (no bounds exit, no lane tests, no + 0 after the source-rect maps)
+        int full;
     } hot;
 };
 

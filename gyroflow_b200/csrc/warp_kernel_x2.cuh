@@ -52,12 +52,16 @@ template <> struct Lens2<GF_LENS_OPENCV_FISHEYE> {
     // a = r^2 (`rtab`, built and checked by the host: build_radial_table in filter_prepass.cu), fused multiply-adds — together with a
     // proven bound on its distance from the reference's own float result (profiles/FILTER_ANALYSIS.md):
     //     |tv_approx - tv_exact| <= (rho + 2^-22) * |tv - c_y| + 2^-22 * |c_y|,   rho = kFilterRho (filter_eps),
-    // valid while the divisor w is in the window of the exact sequences and r^2 is below the host's conditioning cap (the polynomial
-    // stays within [3/4, 5/4]).  The table's rows from that cap on hold NaN, so tvc is NaN there and fails the certificate.
+    // valid while the divisor w is positive and r^2 is below the host's conditioning cap (the polynomial stays within [3/4, 5/4]).  The
+    // table's rows from that cap on hold NaN, so tvc is NaN there and fails the certificate.
     // (_x, _y, _w) are the reference's own unfused products — bit-identical to the exact chain — so only relative perturbations enter
-    // after them.  Returns tvc = (v - c_y), or NaN; the caller checks _w against the window kWLo / kWSpan.
-    static constexpr uint32_t kWLo = 0x23800000u, kWSpan = 0x57800000u - 0x23800000u;   // 2^-56 <= w < 2^48 <=> bits(w) - kWLo < kWSpan
-                                                                                        // (unsigned: NaN, zeros and negatives fail)
+    // after them.  Returns tvc = (v - c_y), or NaN; the caller checks the sign of _w (divisors_ok).
+    // Why the sign is the only test _w needs (profiles/FILTER_ANALYSIS.md "Validity conditions"): on the trusted path 0 < _w < 2^62, so
+    // a normal _w has a normal 1 / _w and the bound holds as for any other divisor; a subnormal or zero _w is flushed to zero by the
+    // MUFU.RCP (.ftz), which returns +-inf, so a is inf or NaN and selects a NaN row; a NaN _w gives a NaN a.  A negative _w (the
+    // reference's None, :138) would give a finite, wrong t: rejected here, and so are the zeros.  One FMNMX and a compare for the pair;
+    // a NaN _w passes only beside a positive one, and its own NaN row rejects it.
+    static GF_DEV bool divisors_ok(float wa, float wb) { return fminf(wa, wb) > 0.0f; }
     static GF_DEV float approx_v(float _x, float _y, float _w, const gf_kernel_params& P, const float4* __restrict__ rtab) {
         const float iw = p2::rcp_approx(_w);
         const float x = _x * iw, y = _y * iw;
@@ -478,15 +482,20 @@ static __device__ __noinline__ PairUV rotate_and_distort_cold(float px, float py
 }
 
 // map_coord with a uniform divisor on a pair (see div_uniform in warp_kernel.cuh).  The two-step division is exact for a numerator
-// that is +-0 or has 2^-80 < |a| < 2^60.  The host guarantees in_min == 0, 2^-40 <= |mul| and |c| >= 2^-10 (so a non-zero x is at
+// that is +-0 or has 2^-80 < |a| < 2^60.  The host guarantees in_min == +0, 2^-40 <= |mul| and |c| >= 2^-10 (so a non-zero x is at
 // least 2^-34 in magnitude and |a| >= 2^-74), and div <= 2^20 (so |a| >= 2^60 would give |result| >= 2^39): testing the RESULT
 // against 2^16 therefore covers the numerator window, catches NaN/Inf, and bounds what the rounding shortcut has to handle.
+// x - in_min is not computed: x - (+0) == x for every x, -0 included (NaN stays NaN, and is flagged).
+// ADD = false drops the final + add; the caller may ask for that only when add == +0 and x is never -0 (warp_x2_body, FULL): then
+// r is +0 (x == +0: mul, rcp, div > 0) or non-zero (|a| >= 2^-74 and |r0 * rcp| < |q0|) or NaN, and r + (+0) == r in each case.
+template <bool ADD = true>
 GF_DEV f2 map_apply_x2(f2 x, const MapC& m, bool& bad) {
     using namespace p2;
-    const f2 a = mul(sub(x, bc(m.in_min)), bc(m.mul));
+    const f2 a = mul(x, bc(m.mul));
     const f2 q0 = mul(a, bc(m.rcp));
     const f2 r0 = fma(bc(-m.div), q0, a);
-    const f2 r = add(fma(r0, bc(m.rcp), q0), bc(m.add));
+    f2 r = fma(r0, bc(m.rcp), q0);
+    if (ADD) r = add(r, bc(m.add));
     bad |= !(fabsf(r.x) < 0x1p16f) | !(fabsf(r.y) < 0x1p16f);
     return r;
 }
@@ -643,11 +652,15 @@ static __device__ __noinline__ void finish_pair_cold(const WarpArgs& A, int x, i
 // pixel size then comes from KernelParams, PIX is a placeholder).
 // exact_prepass: evaluate the mid-row transform with the reference's own arithmetic (always true unless the frame runs the filtered
 // pre-pass; true as well for the pairs the tail launch re-renders)
-template <int LENS, int DIGITAL, class PIX, bool TRUSTED, bool COORD>
+// FULL: the frame has X2Hot::full (host: fill_uniforms) and no digital lens — every thread of the launch writes both its pixels, from the
+// integer prologue, so the bounds exit and the lane tests are compiled out; and the source-rect maps add +0, which map_apply_x2 may drop
+// because ou = ux * f + c with |c| >= 2^-10 is never -0 (the rounded sum of two non-zero floats that cancel exactly is +0)
+template <int LENS, int DIGITAL, class PIX, bool TRUSTED, bool COORD, bool FULL = false>
 GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const bool exact_prepass) {
     using namespace p2;
+    static_assert(!FULL || DIGITAL == GF_LENS_NONE, "a digital lens may turn a coordinate into -0");
     const gf_kernel_params& P = A.p;
-    if (x >= A.out_cols || y0 >= A.out_rows) return;
+    if (!FULL && (x >= A.out_cols || y0 >= A.out_rows)) return;
     const unsigned long long BYTES = COORD ? (unsigned long long)P.bytes_per_pixel : (unsigned long long)PIX::BYTES;
     const unsigned long long ostride = (unsigned long long)P.output_stride;
     const unsigned long long off_a = (unsigned long long)y0 * ostride + (unsigned long long)x * BYTES;
@@ -655,7 +668,10 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
     // lane validity: row exists, pixel fits in the buffer (short last row), bounds test of :551
     float opx, opy_a, opy_b;
     bool wr_a, wr_b;
-    if (A.feat & F_INTPRO) {                                 // identity rect maps: the same tests on integers (host: fill_uniforms)
+    if (FULL) {
+        wr_a = wr_b = true;
+        opx = (float)(x + A.hot.x_off); opy_a = (float)(y0 + A.hot.y_off); opy_b = (float)(y0 + 1 + A.hot.y_off);
+    } else if (A.feat & F_INTPRO) {                                 // identity rect maps: the same tests on integers (host: fill_uniforms)
         const int y1 = y0 + 1;
         const bool in_x = (x >= A.hot.x0) & (x < A.hot.x1);
         wr_a = in_x & (y0 >= A.hot.y0) & (y0 < A.hot.y1);
@@ -674,8 +690,8 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
         wr_b = in_x & ((y0 + 1) < A.out_rows) & (off_b + BYTES <= A.dst_len) & (opy_b >= 0.0f) & (as_i32(opy_b) < P.output_height);
     }
     uint2* const cm_a = COORD ? A.coord_out + ((size_t)y0 * (size_t)A.out_cols + (size_t)x) : nullptr;
-    const bool row_b = (y0 + 1) < A.out_rows;
-    if (!(wr_a | wr_b)) {
+    const bool row_b = FULL || (y0 + 1) < A.out_rows;
+    if (!FULL && !(wr_a | wr_b)) {
         if (COORD) { *cm_a = make_uint2(GF_COORD_MARK, GF_COORD_SKIP); if (row_b) cm_a[A.out_cols] = make_uint2(GF_COORD_MARK, GF_COORD_SKIP); }
         return;
     }
@@ -698,8 +714,7 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
                 const float ya = (by + py.x * rm.m45.x) + rm.m45.y, yb = (by + py.y * rm.m45.x) + rm.m45.y;
                 const float wa = (bw + py.x * rm.m67.y) + rm.m8,    wb = (bw + py.y * rm.m67.y) + rm.m8;
                 const float ca = Lens2<LENS>::approx_v(xa, ya, wa, P, A.flt.rtab), cb = Lens2<LENS>::approx_v(xb, yb, wb, P, A.flt.rtab);
-                constexpr uint32_t wlo = Lens2<LENS>::kWLo;                   // both divisors in the window: the larger offset, unsigned
-                const bool w_ok = __viaddmax_u32(__float_as_uint(wa), 0u - wlo, __float_as_uint(wb) - wlo) < Lens2<LENS>::kWSpan;
+                const bool w_ok = Lens2<LENS>::divisors_ok(wa, wb);            // both divisors positive
                 const float ta = ca + P.c[1], tb = cb + P.c[1];
                 const float ea = __fmaf_rn(fabsf(ca), A.flt.eps_rel, A.flt.eps_abs), eb = __fmaf_rn(fabsf(cb), A.flt.eps_rel, A.flt.eps_abs);
                 const bool ca_ok = certify_row(ta, ea, lim, sy_a), cb_ok = certify_row(tb, eb, lim, sy_b);
@@ -730,8 +745,8 @@ GF_DEV void warp_x2_body(const WarpArgs& A, const int x, const int y0, const boo
     } while (false);
     f2 u, v; bool bad = false;
     rotate_and_distort_x2<LENS, DIGITAL, TRUSTED>(px, py, (uint32_t)sy_a, (uint32_t)sy_b, A, u, v, bad);    // :483
-    u = map_apply_x2(u, A.smap_x, bad);                                                                 // :510-515
-    v = map_apply_x2(v, A.smap_y, bad);
+    u = map_apply_x2<!FULL>(u, A.smap_x, bad);                                                          // :510-515
+    v = map_apply_x2<!FULL>(v, A.smap_y, bad);
     if (bad) { finish_pair_cold<LENS, DIGITAL, PIX, COORD>(A, x, y0, pxs, py, (uint32_t)sy_a, (uint32_t)sy_b, wr_a, wr_b); return; }
 
     // from here on both pixels are Some(..) with |u|, |v| < 2^16 (map_apply_x2)
@@ -789,8 +804,13 @@ warp_kernel_x2(const __grid_constant__ WarpArgs A) {
     }
     const int x = blockIdx.x * GF_BLOCK_X + threadIdx.x;
     const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * 2;          // blockDim.y: the host launches flatter blocks than the bounds allow (32 x 4)
-    if (trusted) warp_x2_body<LENS, DIGITAL, PIX, true, COORD>(A, x, y0, !(kFilter && (A.feat & F_FILTER)));
-    else         warp_x2_body<LENS, DIGITAL, PIX, false, COORD>(A, x, y0, true);
+    if (trusted) {
+        const bool exact_prepass = !(kFilter && (A.feat & F_FILTER));
+        if constexpr (DIGITAL == GF_LENS_NONE) if (A.hot.full) { warp_x2_body<LENS, DIGITAL, PIX, true, COORD, true>(A, x, y0, exact_prepass); return; }
+        warp_x2_body<LENS, DIGITAL, PIX, true, COORD>(A, x, y0, exact_prepass);
+    } else {
+        warp_x2_body<LENS, DIGITAL, PIX, false, COORD>(A, x, y0, true);
+    }
 }
 
 } // namespace gf
