@@ -246,6 +246,7 @@ EXPORTS = [
     ("gf_cuda_selftest_exhaustive", C.c_int, [C.c_int, C.POINTER(C.c_ulonglong)]),
     ("gf_cuda_selftest_filter", C.c_int, [C.c_int, C.c_ulonglong, C.c_int, C.c_int, C.POINTER(C.c_ulonglong)]),
     ("gf_cuda_selftest_certify", C.c_int, [C.c_int, C.c_void_p, C.c_size_t, C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
+    ("gf_cuda_selftest_sync_select", C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("gf_cuda_plan", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t]),
     ("gf_cuda_plan_features", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_size_t,
                                         _P(C.c_uint32)]),

@@ -407,6 +407,18 @@ def _sync_pairs(pairs, keep: list):
     return arr
 
 
+def selftest_sync_select(groups, device=0):
+    """The sync cost's k-smallest selection on raw uint32 keys (gf_cuda_selftest_sync_select): per group, the sum of its k smallest keys
+    other than 0xFFFFFFFF (a point pair outside the frame), k = int(m * 0.9) for its m such keys.  Returns a uint64 array."""
+    arrs = [np.ascontiguousarray(k, dtype=np.uint32).reshape(-1) for k in groups]
+    keys = np.concatenate(arrs) if arrs else np.zeros(0, np.uint32)
+    sizes = np.array([a.size for a in arrs], dtype=np.uintp)
+    out = np.zeros(len(arrs), np.uint64)
+    rc = abi.load_library().gf_cuda_selftest_sync_select(device, keys.ctypes.data, sizes.ctypes.data, len(arrs), out.ctypes.data)
+    check_call(rc, "gf_cuda_selftest_sync_select")
+    return out
+
+
 class DeviceGyro:
     """Quaternion tracks resident in HBM + the per-frame matrix kernel (gf_cuda_frame_transform_dev)."""
 

@@ -6,9 +6,11 @@
 #include <cstdlib>
 #include <cstring>
 #include <cmath>
+#include <algorithm>
 #include <vector>
 #include "../../include/gyroflow_cuda.h"
 #include "warp_kernel_x2.cuh"
+#include "sync_select.cuh"
 #include "c_abi_internal.h"
 
 using namespace gf;
@@ -240,6 +242,57 @@ extern "C" GF_API int gf_cuda_selftest_certify(int device, const float* t, size_
     CK(nullptr, cudaDeviceSynchronize());
     CK(nullptr, cudaMemcpy(cert_out, d_c.ptr, n, cudaMemcpyDeviceToHost));
     CK(nullptr, cudaMemcpy(row_out, d_r.ptr, n * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return GF_OK;
+}
+
+namespace {
+// One CTA per group, exactly as sync_cost_kernel treats a pair: the group's keys go to shared memory (<= SYNC_SMEM_KEYS) or to global
+// scratch, each thread counts its valid ones, and sync_select_add adds the group's k-smallest sum to sums[group].
+__global__ void __launch_bounds__(SYNC_THREADS) sync_select_kernel(const uint32_t* __restrict__ in, const uint2* __restrict__ groups,
+                                                                   uint32_t* __restrict__ scratch, unsigned long long* __restrict__ sums) {
+    extern __shared__ uint32_t skeys[];
+    __shared__ unsigned hist[256];
+    __shared__ uint64_t red[SYNC_THREADS / 32];
+    __shared__ uint32_t s_prefix, s_rank;
+    const uint2 gr = groups[blockIdx.x];             // first key, key count
+    if (gr.y == 0) return;
+    uint32_t* keys = gr.y <= SYNC_SMEM_KEYS ? skeys : scratch + gr.x;
+    uint64_t valid = 0;
+    for (uint32_t i = threadIdx.x; i < gr.y; i += SYNC_THREADS) {
+        const uint32_t key = in[gr.x + i];
+        if (key != SYNC_NO_KEY) ++valid;
+        keys[i] = key;
+    }
+    sync_select_add(keys, gr.y, valid, hist, red, s_prefix, s_rank, &sums[blockIdx.x]);
+}
+} // namespace
+
+extern "C" GF_API int gf_cuda_selftest_sync_select(int device, const uint32_t* keys, const size_t* group_sizes, size_t n_groups,
+                                                   unsigned long long* out_sums) {
+    if (n_groups == 0) return GF_OK;
+    if (!keys || !group_sizes || !out_sums || n_groups > 0x7fffffffu) return GF_ERR_BAD_PARAMS;
+    std::vector<uint2> groups(n_groups);
+    size_t total = 0, max_n = 0;
+    for (size_t i = 0; i < n_groups; ++i) {
+        if (group_sizes[i] > 0xFFFFFFFFu - total) return GF_ERR_BAD_PARAMS;       // offsets are 32-bit, as in sync_cost_kernel
+        groups[i] = make_uint2((unsigned)total, (unsigned)group_sizes[i]);
+        total += group_sizes[i];
+        max_n = std::max(max_n, group_sizes[i]);
+    }
+    CK(nullptr, cudaSetDevice(device));
+    GrowBuf<uint32_t> d_in, d_scratch; GrowBuf<uint2> d_groups; GrowBuf<unsigned long long> d_sums;
+    CK(nullptr, d_in.reserve(std::max<size_t>(total, 1), nullptr));
+    CK(nullptr, d_groups.reserve(n_groups, nullptr));
+    CK(nullptr, d_sums.reserve(n_groups, nullptr));
+    if (max_n > SYNC_SMEM_KEYS) CK(nullptr, d_scratch.reserve(total, nullptr));
+    if (total) CK(nullptr, cudaMemcpy(d_in.ptr, keys, total * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemcpy(d_groups.ptr, groups.data(), n_groups * sizeof(uint2), cudaMemcpyHostToDevice));
+    CK(nullptr, cudaMemset(d_sums.ptr, 0, n_groups * sizeof(unsigned long long)));
+    const unsigned smem = (unsigned)std::min<size_t>(max_n, SYNC_SMEM_KEYS) * (unsigned)sizeof(uint32_t);
+    sync_select_kernel<<<(unsigned)n_groups, SYNC_THREADS, smem>>>(d_in.ptr, d_groups.ptr, d_scratch.ptr, d_sums.ptr);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaDeviceSynchronize());
+    CK(nullptr, cudaMemcpy(out_sums, d_sums.ptr, n_groups * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     return GF_OK;
 }
 

@@ -21,6 +21,7 @@
 #include "lens_models.cuh"
 #include "warp_kernel.cuh"      // the warp's stage functions: lens correction, refraction, mesh
 #include "frame_geometry.cuh"
+#include "sync_select.cuh"
 #include "gyro_dev.h"
 #include "c_abi_internal.h"
 
@@ -265,26 +266,11 @@ __global__ void __launch_bounds__(128) stmap_size_kernel(const PointFrame* __res
 }
 
 // ---- visual-features sync: calculate_distance (synchronization/find_offset/visual_features.rs:46-84) ----
-constexpr int SYNC_THREADS = 256;
-constexpr unsigned SYNC_SMEM_KEYS = 8192;       // distance keys per pair held in shared memory; larger pairs keep them in global scratch
-constexpr uint32_t SYNC_NO_KEY = 0xFFFFFFFFu;   // a point pair outside the frame; every real key is <= 2^31 (frames of <= 32768 px a side)
 struct SyncPairDev { uint32_t off, n; };        // a pair's first point in the concatenated lists, and its point count
-
-__device__ __forceinline__ uint64_t block_sum_u64(uint64_t v, uint64_t* red) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
-    __syncthreads();                            // `red` may still be read from the previous reduction
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    uint64_t s = 0;
-    for (int w = 0; w < SYNC_THREADS / 32; ++w) s += red[w];
-    return s;
-}
 
 // One CTA per (candidate, pair).  recs: 2 PointFrames per CTA (the pair's two timestamps at this candidate), blockIdx.x = candidate *
 // n_pairs + pair.  Every thread undistorts its points, keeps the truncated f32 squared distance of each point pair inside the frame as a
-// 32-bit key, the CTA finds the k-th smallest key T by radix select (one 256-bin histogram per byte) and adds
-// sum(keys < T) + (k - count(keys < T)) * T — the sum of the k smallest — to sums[candidate] with an integer atomic, whose order does not
-// matter.
+// 32-bit key, and sync_select_add (sync_select.cuh) adds the sum of the k smallest keys to sums[candidate].
 template <int LENS, int DIGITAL>
 __global__ void __launch_bounds__(SYNC_THREADS) sync_cost_kernel(const PointFrame* __restrict__ recs, const SyncPairDev* __restrict__ pairs, unsigned n_pairs,
                                                                  const float2* __restrict__ pts1, const float2* __restrict__ pts2, float w, float h,
@@ -313,45 +299,7 @@ __global__ void __launch_bounds__(SYNC_THREADS) sync_cost_kernel(const PointFram
         }
         keys[i] = key;
     }
-    const uint64_t m = block_sum_u64(valid, red);
-    const uint64_t k = (uint64_t)((double)m * 0.9);     // (len as f64 * 0.9) as usize
-    if (k == 0) return;
-    if (threadIdx.x == 0) { s_prefix = 0; s_rank = (uint32_t)k; }
-    for (int shift = 24; shift >= 0; shift -= 8) {
-        for (int b = threadIdx.x; b < 256; b += SYNC_THREADS) hist[b] = 0;
-        __syncthreads();                                 // also publishes s_prefix / s_rank and (first pass) every key
-        const uint32_t prefix = s_prefix, hi = shift == 24 ? 0u : (0xFFFFFFFFu << (shift + 8));
-        for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
-            const uint32_t key = keys[i];
-            if ((key & hi) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (threadIdx.x < 32) {                          // one warp: lane l scans bins 8l..8l+7
-            const int l = threadIdx.x;
-            unsigned c[8], own = 0;
-            for (int j = 0; j < 8; ++j) { c[j] = hist[8 * l + j]; own += c[j]; }
-            unsigned incl = own;
-            for (int o = 1; o < 32; o <<= 1) { const unsigned t = __shfl_up_sync(0xffffffffu, incl, o); if (l >= o) incl += t; }
-            const uint32_t rank = s_rank;
-            unsigned before = incl - own;
-            if (before < rank && rank <= incl) {         // exactly one lane holds the bin of the rank-th key
-                int j = 0;
-                while (before + c[j] < rank) before += c[j++];
-                s_rank = rank - before;
-                s_prefix = prefix | ((uint32_t)(8 * l + j) << shift);
-            }
-        }
-        __syncthreads();                                 // the scan has read `hist` before the next pass clears it
-    }
-    const uint32_t T = s_prefix;
-    uint64_t below = 0, n_below = 0;
-    for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
-        const uint32_t key = keys[i];
-        if (key < T) { below += key; ++n_below; }
-    }
-    below = block_sum_u64(below, red);
-    n_below = block_sum_u64(n_below, red);
-    if (threadIdx.x == 0) atomicAdd(&sums[cand], (unsigned long long)(below + (k - n_below) * (uint64_t)T));
+    sync_select_add(keys, pr.n, valid, hist, red, s_prefix, s_rank, &sums[cand]);
 }
 
 // The kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye

@@ -354,6 +354,13 @@ GF_API int         gf_cuda_selftest_filter(int device, unsigned long long seed, 
 /* The pre-pass's certify-and-round step (certify_row in warp_kernel_x2.cuh, the device function the packed kernel runs) on n host
  * values t with one eps and row limit: cert_out[i] = 1 when t[i] is certified, row_out[i] = the clamped row it yields.  Test hook. */
 GF_API int         gf_cuda_selftest_certify(int device, const float* t, size_t n, float eps, int lim, uint8_t* cert_out, int32_t* row_out);
+/* The visual-features sync cost's selection (sync_select_add in sync_select.cuh, the device function sync_cost_kernel runs) on raw keys:
+ * keys holds n_groups groups back to back, group i of group_sizes[i] keys (0xFFFFFFFF = a point pair outside the frame, any other value a
+ * distance key), at most 2^32 - 1 keys in all.  One CTA per group, its keys in shared memory up to 8192 keys and in global scratch above,
+ * as in gf_cuda_sync_costs.  out_sums[i] = the sum of the k smallest valid keys of group i, k = (m as f64 * 0.9) as usize for its m
+ * valid keys.  Test hook. */
+GF_API int         gf_cuda_selftest_sync_select(int device, const uint32_t* keys, const size_t* group_sizes, size_t n_groups,
+                                                unsigned long long* out_sums);
 
 
 /* ------------------------------------------------------------------------------------------
