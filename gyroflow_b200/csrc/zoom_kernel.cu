@@ -29,7 +29,18 @@ using namespace gf;
 
 namespace {
 
-struct ZoomFrame {              // per-frame uniforms (host, f64)
+// Everything a point-path kernel reads about one frame: what undistort_points (cpu_undistort.rs:652-698) and at_timestamp_for_points
+// (frame_transform.rs:352-438) derive from ComputeParams for it (point_frame).  The lens may change per frame (lens_per_frame), so the
+// kernel params and K_new are per frame too.
+struct PointFrame {
+    gf_kernel_params kp;        // as built by undistort_points (:671-683)
+    Track org;                  // device-resident track
+    double duration_ms;
+    SyncOffsets offsets;        // device-resident multi-point sync offsets (or the scalar)
+    double new_k[9];
+    int horizontal, suppress_rotation, lens_noop;
+    float hstretch, vstretch;   // 0 = do not apply (:702-703)
+    float fov, out_cx, out_cy;  // lens-correction blend (:686-694); out_cx 8-byte aligned, so that the kernels load it with out_cy
     Quat q0;                    // smoothed(ts) * org(ts)^-1
     double start_ts, row_readout_time;
     int rs_on;                  // rolling-shutter correction: frame readout time != 0
@@ -42,30 +53,19 @@ struct ZoomFrame {              // per-frame uniforms (host, f64)
     float lrc;                  // light refraction coefficient
     int lc; float amount, factor, out_fx, out_fy;       // lens-correction blend (:686-694)
 };
-struct ZoomArgs {               // the call-wide values
-    gf_kernel_params kp;        // as built by undistort_points (:671-683)
-    Track org;                  // device-resident track
-    double duration_ms;
-    SyncOffsets offsets;        // device-resident multi-point sync offsets (or the scalar)
-    double new_k[9];
-    int horizontal, suppress_rotation, lens_noop;
-    float hstretch, vstretch;   // 0 = do not apply (:702-703)
-    float in_w, in_h, out_w, inv_aspect, margin;
-    float out_cx, out_cy, fov;  // lens-correction blend (:686-694)
-};
 
 // K_new * R for one point — frame_transform.rs:391-410 (f64, no inverted-framebuffer flips), narrowed to f32 like cpu_undistort.rs:764
-__device__ void point_rotation(const ZoomArgs& A, const ZoomFrame& F, float px, float py, float (&rot)[9]) {
-    const double quat_time = F.rs_on ? F.start_ts + F.row_readout_time * (double)(A.horizontal ? px : py) : F.start_ts;
-    const Quat q = qmul(F.q0, quat_at_timestamp(A.org, A.duration_ms, A.offsets, quat_time));
+__device__ void point_rotation(const PointFrame& F, float px, float py, float (&rot)[9]) {
+    const double quat_time = F.rs_on ? F.start_ts + F.row_readout_time * (double)(F.horizontal ? px : py) : F.start_ts;
+    const Quat q = qmul(F.q0, quat_at_timestamp(F.org, F.duration_ms, F.offsets, quat_time));
     double m[9];
-    frame_rotation(q, F.rot_c, F.rot_s, A.new_k, false, A.suppress_rotation, m);
+    frame_rotation(q, F.rot_c, F.rot_s, F.new_k, false, F.suppress_rotation, m);
     for (int t = 0; t < 9; ++t) rot[t] = (float)m[t];
 }
 
 // The IBIS / OIS shift of point `index` — frame_transform.rs:412-431.  points_iter is the point list when rolling-shutter correction is
 // on and the single point (0, 0) otherwise, so with correction off only index 0 has an entry (cpu_undistort.rs:748 `v.get(index)`).
-__device__ bool point_shift(const ZoomFrame& F, float py, size_t index, float (&sh)[5]) {
+__device__ bool point_shift(const PointFrame& F, float py, size_t index, float (&sh)[5]) {
     if (!F.stab.present) return false;
     if (!F.rs_on && index != 0) return false;
     double s[5];
@@ -76,7 +76,7 @@ __device__ bool point_shift(const ZoomFrame& F, float py, size_t index, float (&
 
 // The mesh block of undistort_points — cpu_undistort.rs:712-746: focal-plane distortion first, then the distorting mesh.  No
 // inverted-framebuffer flips on this path.
-__device__ void point_mesh(const ZoomFrame& F, float& x, float& y) {
+__device__ void point_mesh(const PointFrame& F, float& x, float& y) {
     const MeshView mesh{ F.mesh };
     const MeshAux& aux = F.mesh_aux;
     const double mesh0 = mesh[0];
@@ -98,13 +98,13 @@ __device__ void point_mesh(const ZoomFrame& F, float& x, float& y) {
 
 // one point of undistort_points — cpu_undistort.rs:699-857
 template <int LENS, int DIGITAL>
-__device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float px, float py, size_t index, float& outx, float& outy) {
-    const gf_kernel_params& P = A.kp;
+__device__ void undistort_point_rs(const PointFrame& F, float px, float py, size_t index, float& outx, float& outy) {
+    const gf_kernel_params& P = F.kp;
     float rot[9];
-    point_rotation(A, F, px, py, rot);                  // rotation time uses the *distorted* point (:393)
+    point_rotation(F, px, py, rot);                     // rotation time uses the *distorted* point (:393)
     float x = px, y = py;
-    if (A.hstretch != 0.0f) x *= A.hstretch;
-    if (A.vstretch != 0.0f) y *= A.vstretch;
+    if (F.hstretch != 0.0f) x *= F.hstretch;
+    if (F.vstretch != 0.0f) y *= F.vstretch;
     if (DIGITAL != GF_LENS_NONE) { float tx, ty; if (Lens<DIGITAL>::undistort(x, y, P, false, tx, ty)) { x = tx; y = ty; } }
     if (F.mesh && F.mesh_len > 9) point_mesh(F, x, y);             // cpu_undistort.rs:712-746
     float sh[5];
@@ -117,7 +117,7 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     }
     const float pwx = (x - P.c[0]) / P.f[0], pwy = (y - P.c[1]) / P.f[1];
     float ptx, pty;
-    if (!Lens<LENS>::undistort(pwx, pwy, P, A.lens_noop != 0, ptx, pty)) { outx = -1000000.0f; outy = -1000000.0f; return; }
+    if (!Lens<LENS>::undistort(pwx, pwy, P, F.lens_noop != 0, ptx, pty)) { outx = -1000000.0f; outy = -1000000.0f; return; }
     const bool refract = F.lrc != 1.0f && F.lrc > 0.0f;
     if (refract) refract_undistort(ptx, pty, F.lrc);
     const float pr0 = rot[0] * ptx + rot[1] * pty + rot[2] * 1.0f;
@@ -126,20 +126,20 @@ __device__ void undistort_point_rs(const ZoomArgs& A, const ZoomFrame& F, float 
     ptx = pr0 / pr2; pty = pr1 / pr2;
     if (F.lc) {                                         // :782-852
         const float amount = F.amount, factor = F.factor, out_fx = F.out_fx, out_fy = F.out_fy;
-        const float nx = (ptx - A.out_cx) / out_fx, ny = (pty - A.out_cy) / out_fy;
+        const float nx = (ptx - F.out_cx) / out_fx, ny = (pty - F.out_cy) / out_fy;
         float dx, dy;
-        Lens<LENS>::distort(nx, ny, 1.0f, P, A.lens_noop != 0, dx, dy);
-        float p2x = (dx * out_fx) + A.out_cx, p2y = (dy * out_fy) + A.out_cy;
+        Lens<LENS>::distort(nx, ny, 1.0f, P, F.lens_noop != 0, dx, dy);
+        float p2x = (dx * out_fx) + F.out_cx, p2y = (dy * out_fy) + F.out_cy;
         if (DIGITAL != GF_LENS_NONE) {
-            const float uzx = (p2x - A.out_cx) * A.fov + A.out_cx, uzy = (p2y - A.out_cy) * A.fov + A.out_cy;
+            const float uzx = (p2x - F.out_cx) * F.fov + F.out_cx, uzy = (p2y - F.out_cy) * F.fov + F.out_cy;
             float ddx, ddy;
             Lens<DIGITAL>::distort(uzx, uzy, 1.0f, P, false, ddx, ddy);
-            p2x = (ddx - A.out_cx) / A.fov + A.out_cx; p2y = (ddy - A.out_cy) / A.fov + A.out_cy;
+            p2x = (ddx - F.out_cx) / F.fov + F.out_cx; p2y = (ddy - F.out_cy) / F.fov + F.out_cy;
         }
         float ox = ptx, oy = pty;
         if (isfinite(p2x) && isfinite(p2y)) { ox = p2x * factor + ptx * amount; oy = p2y * factor + pty * amount; }
         auto r_of = [&](float qx, float qy, float& rx, float& ry) {          // :794-815
-            lens_correction_undistort<LENS, DIGITAL>(qx, qy, P, A.out_cx, A.out_cy, out_fx, out_fy, A.fov, A.lens_noop != 0, true, refract, F.lrc, rx, ry);
+            lens_correction_undistort<LENS, DIGITAL>(qx, qy, P, F.out_cx, F.out_cy, out_fx, out_fy, F.fov, F.lens_noop != 0, true, refract, F.lrc, rx, ry);
         };
         for (int it = 0; it < 10; ++it) {
             float rx, ry; r_of(ox, oy, rx, ry);
@@ -179,17 +179,24 @@ __device__ int nearest_edge(const float* poly, int plen, float cx, float cy, flo
     return idx;
 }
 
+// The sizes of FovIterative::new (fov_iterative.rs:78-89), the same for every frame of a call
+struct FovArgs { float in_w, in_h, out_w, inv_aspect, margin; };
+
 template <int LENS, int DIGITAL>
-__global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ ZoomArgs A, const ZoomFrame* __restrict__ frames, double* __restrict__ out) {
+__global__ void __launch_bounds__(128) find_fov_kernel(const PointFrame* __restrict__ frames, const FovArgs A, double* __restrict__ out) {
     __shared__ float rect[2 * ZOOM_RECT_LEN], poly[2 * ZOOM_RECT_LEN];
     __shared__ float sw, sh; __shared__ int sidx;
-    const ZoomFrame& F = frames[blockIdx.x];
+    // The frame's record, staged in shared memory: read from global memory instead, the compiler holds more of it in registers across the
+    // rounds below (up to 128 per thread instead of 94-126).
+    __shared__ PointFrame F;
     const int tid = threadIdx.x;
+    for (int i = tid; i < (int)(sizeof(PointFrame) / 8); i += 128) ((unsigned long long*)&F)[i] = ((const unsigned long long*)&frames[blockIdx.x])[i];
+    __syncthreads();
     const float cx = A.in_w / 2.0f, cy = A.in_h / 2.0f;
     if (tid < ZOOM_RECT_LEN) {
         float x, y; rect_point(A.in_w, A.in_h, A.margin, tid, x, y);
         rect[2 * tid] = x; rect[2 * tid + 1] = y;
-        float ux, uy; undistort_point_rs<LENS, DIGITAL>(A, F, x, y, (size_t)tid, ux, uy);
+        float ux, uy; undistort_point_rs<LENS, DIGITAL>(F, x, y, (size_t)tid, ux, uy);
         poly[2 * tid] = ux - F.zc_x; poly[2 * tid + 1] = uy - F.zc_y;
     }
     if (tid == 0) { sw = 1000000.0f; sh = 1000000.0f * A.inv_aspect; }
@@ -210,7 +217,7 @@ __global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ Z
             const float f = (float)(tid % d) / (float)d;
             const float dx = rect[2 * ra] + f * (rect[2 * rb] - rect[2 * ra]);
             const float dy = rect[2 * ra + 1] + f * (rect[2 * rb + 1] - rect[2 * ra + 1]);
-            undistort_point_rs<LENS, DIGITAL>(A, F, dx, dy, (size_t)tid, nx, ny);
+            undistort_point_rs<LENS, DIGITAL>(F, dx, dy, (size_t)tid, nx, ny);
         }
         __syncthreads();                                 // everyone has read rect/poly of this round
         if (tid < ZOOM_INTERP_LEN) { poly[2 * tid] = nx - F.zc_x; poly[2 * tid + 1] = ny - F.zc_y; }
@@ -225,32 +232,28 @@ __global__ void __launch_bounds__(128) find_fov_kernel(const __grid_constant__ Z
 // undistort_points over an explicit point list (pts != nullptr: out = n x (x, y)) or over every pixel centre of a w x h grid
 // (pts == nullptr: out = w*h x RGB, the ST-map encoding of stmap.rs:131-135: x / w, 1 - y / h, 0).
 template <int LENS, int DIGITAL>
-__global__ void __launch_bounds__(128) points_kernel(const ZoomArgs A, const ZoomFrame F, const float2* __restrict__ pts, size_t n, int grid_w, int grid_h, float* __restrict__ out) {
+__global__ void __launch_bounds__(128) points_kernel(const __grid_constant__ PointFrame F, const float2* __restrict__ pts, size_t n, int grid_w, int grid_h, float* __restrict__ out) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     float px, py;
     if (pts) { const float2 p = pts[i]; px = p.x; py = p.y; }
     else     { px = (float)(int)(i % (size_t)grid_w); py = (float)(int)(i / (size_t)grid_w); }
     float ox, oy;
-    undistort_point_rs<LENS, DIGITAL>(A, F, px, py, pts ? i : (size_t)0, ox, oy);      // ST map: every pixel is its own one-point call (stmap.rs:114-116)
+    undistort_point_rs<LENS, DIGITAL>(F, px, py, pts ? i : (size_t)0, ox, oy);      // ST map: every pixel is its own one-point call (stmap.rs:114-116)
     if (pts) { out[2 * i] = ox; out[2 * i + 1] = oy; }
     else     { out[3 * i] = ox / (float)grid_w; out[3 * i + 1] = 1.0f - (oy / (float)grid_h); out[3 * i + 2] = 0.0f; }
 }
-// What gf_cuda_undistort_points derives for one frame (point_frame).  The lens may change per frame (lens_per_frame), so in a call over
-// several frames (gf_cuda_stmap_sizes) the call-wide values are per frame.
-struct PointFrame { ZoomArgs A; ZoomFrame F; };
-
 // The undistorted size of one frame per CTA — stmap.rs:58-77: the 120 points_around_rect(w, h, 31, 31) edge points with margin 0
 // (fov_iterative.rs:154-175) through undistort_points, their bounding box folded in order from 0 with f32::min / max (NaN is
 // ignored, :62-71), then `ceil(max - min) as usize` for each extent.
 template <int LENS, int DIGITAL>
 __global__ void __launch_bounds__(128) stmap_size_kernel(const PointFrame* __restrict__ frames, float w, float h, int2* __restrict__ out) {
     __shared__ float und[2 * RECT_POINTS];
-    const PointFrame& S = frames[blockIdx.x];
+    const PointFrame& F = frames[blockIdx.x];
     const int tid = threadIdx.x;
     if (tid < RECT_POINTS) {
         float x, y; rect_point(w, h, 0.0f, tid, x, y);
-        undistort_point_rs<LENS, DIGITAL>(S.A, S.F, x, y, (size_t)tid, und[2 * tid], und[2 * tid + 1]);
+        undistort_point_rs<LENS, DIGITAL>(F, x, y, (size_t)tid, und[2 * tid], und[2 * tid + 1]);
     }
     __syncthreads();
     if (tid != 0) return;
@@ -268,7 +271,7 @@ __global__ void __launch_bounds__(128) stmap_size_kernel(const PointFrame* __res
 // ---- visual-features sync: calculate_distance (synchronization/find_offset/visual_features.rs:46-84) ----
 struct SyncPairDev { uint32_t off, n; };        // a pair's first point in the concatenated lists, and its point count
 
-// One CTA per (candidate, pair).  recs: 2 PointFrames per CTA (the pair's two timestamps at this candidate), blockIdx.x = candidate *
+// One CTA per (candidate, pair).  recs: 2 records per CTA (the pair's two timestamps at this candidate), blockIdx.x = candidate *
 // n_pairs + pair.  Every thread undistorts its points, keeps the truncated f32 squared distance of each point pair inside the frame as a
 // 32-bit key, and sync_select_add (sync_select.cuh) adds the sum of the k smallest keys to sums[candidate].
 template <int LENS, int DIGITAL>
@@ -289,8 +292,8 @@ __global__ void __launch_bounds__(SYNC_THREADS) sync_cost_kernel(const PointFram
     for (uint32_t i = threadIdx.x; i < pr.n; i += SYNC_THREADS) {
         const float2 a = pts1[pr.off + i], b = pts2[pr.off + i];
         float x1, y1, x2, y2;
-        undistort_point_rs<LENS, DIGITAL>(S1.A, S1.F, a.x, a.y, (size_t)i, x1, y1);
-        undistort_point_rs<LENS, DIGITAL>(S2.A, S2.F, b.x, b.y, (size_t)i, x2, y2);
+        undistort_point_rs<LENS, DIGITAL>(S1, a.x, a.y, (size_t)i, x1, y1);
+        undistort_point_rs<LENS, DIGITAL>(S2, b.x, b.y, (size_t)i, x2, y2);
         uint32_t key = SYNC_NO_KEY;
         if (x1 > 0.0f && x1 < w && y1 > 0.0f && y1 < h && x2 > 0.0f && x2 < w && y2 > 0.0f && y2 < h) {      // :66-67
             const float dx = x2 - x1, dy = y2 - y1;
@@ -302,30 +305,31 @@ __global__ void __launch_bounds__(SYNC_THREADS) sync_cost_kernel(const PointFram
     sync_select_add(keys, pr.n, valid, hist, red, s_prefix, s_rank, &sums[cand]);
 }
 
-// The kernels of a (lens, digital lens) pair; nullptr for a pair the reference does not combine (the GoPro views need the fisheye
-// model, GoPro warp the GoPro model).
+// The kernels of a (lens, digital lens) pair, compiled only for the pairs the reference combines (the GoPro views need the fisheye
+// model, GoPro warp the GoPro model); nullptr for any other pair.
 struct ZoomKernels {
-    void (*find_fov)(const ZoomArgs, const ZoomFrame*, double*);
-    void (*points)(const ZoomArgs, const ZoomFrame, const float2*, size_t, int, int, float*);
+    void (*find_fov)(const PointFrame*, const FovArgs, double*);
+    void (*points)(const PointFrame, const float2*, size_t, int, int, float*);
     void (*stmap_size)(const PointFrame*, float, float, int2*);
     void (*sync_cost)(const PointFrame*, const SyncPairDev*, unsigned, const float2*, const float2*, float, float, uint32_t*, size_t, unsigned long long*);
 };
-template <int LENS, int DIGITAL> ZoomKernels kernels_of() {
-    return { find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL>, sync_cost_kernel<LENS, DIGITAL> };
+template <int LENS, int DIGITAL> const ZoomKernels* kernels_of() {
+    static const ZoomKernels k{ find_fov_kernel<LENS, DIGITAL>, points_kernel<LENS, DIGITAL>, stmap_size_kernel<LENS, DIGITAL>, sync_cost_kernel<LENS, DIGITAL> };
+    return &k;
 }
-template <int LENS> ZoomKernels pick_digital(int digital) {
+template <int LENS> const ZoomKernels* pick_digital(int digital) {
     switch (digital) {
     case GF_LENS_NONE:             return kernels_of<LENS, GF_LENS_NONE>();
     case GF_LENS_DIGITAL_STRETCH:  return kernels_of<LENS, GF_LENS_DIGITAL_STRETCH>();
-    case GF_LENS_GOPRO_SUPERVIEW:  if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_SUPERVIEW>();  break;
-    case GF_LENS_GOPRO6_SUPERVIEW: if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO6_SUPERVIEW>(); break;
-    case GF_LENS_GOPRO_HYPERVIEW:  if (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_HYPERVIEW>();  break;
-    case GF_LENS_GOPRO_WARP:       if (LENS == GF_LENS_GOPRO) return kernels_of<LENS, GF_LENS_GOPRO_WARP>();                break;
+    case GF_LENS_GOPRO_SUPERVIEW:  if constexpr (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_SUPERVIEW>();  break;
+    case GF_LENS_GOPRO6_SUPERVIEW: if constexpr (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO6_SUPERVIEW>(); break;
+    case GF_LENS_GOPRO_HYPERVIEW:  if constexpr (LENS == GF_LENS_OPENCV_FISHEYE) return kernels_of<LENS, GF_LENS_GOPRO_HYPERVIEW>();  break;
+    case GF_LENS_GOPRO_WARP:       if constexpr (LENS == GF_LENS_GOPRO) return kernels_of<LENS, GF_LENS_GOPRO_WARP>();                break;
     default: break;
     }
-    return { nullptr, nullptr, nullptr, nullptr };
+    return nullptr;
 }
-ZoomKernels pick_kernels(int lens, int digital) {
+const ZoomKernels* pick_kernels(int lens, int digital) {
     switch (lens) {
     case GF_LENS_OPENCV_FISHEYE:     return pick_digital<GF_LENS_OPENCV_FISHEYE>(digital);
     case GF_LENS_OPENCV_STANDARD:    return pick_digital<GF_LENS_OPENCV_STANDARD>(digital);
@@ -336,7 +340,7 @@ ZoomKernels pick_kernels(int lens, int digital) {
     case GF_LENS_SONY:               return pick_digital<GF_LENS_SONY>(digital);
     case GF_LENS_GENERIC_POLYNOMIAL: return pick_digital<GF_LENS_GENERIC_POLYNOMIAL>(digital);
     case GF_LENS_GOPRO:              return pick_digital<GF_LENS_GOPRO>(digital);
-    default: return { nullptr, nullptr, nullptr, nullptr };
+    default: return nullptr;
     }
 }
 
@@ -348,33 +352,46 @@ static double points_fov(const gf_compute_params* cp, size_t frame, bool use_fov
     return fov_unscaled(cp, frame, use_fovs, timestamp_ms, false) * (double)cp->width / (double)(cp->output_width > 1 ? cp->output_width : 1);
 }
 
-// Everything undistort_points (cpu_undistort.rs:652-698) and at_timestamp_for_points (frame_transform.rs:352-410) derive from
-// ComputeParams for one call: kernel params, K_new.
-static void setup_points_args(const gf_cuda_gyro* g, const gf_compute_params& cp, int distortion_model, double fov, ZoomArgs& A) {
-    memset(&A, 0, sizeof(A));
+// What the callers of point_frame choose, in this order
+struct PointOpts {
+    bool use_fovs = false;                  // get_fov with the clip's fovs
+    double lens_correction_amount = 1.0;    // the lens-correction strength
+    bool zoom_keys = false;                 // find_fov (fov_iterative.rs:44-46): the zoom centre and the strength follow their tracks,
+                                            // lens_correction_amount being the strength without one
+    bool clear_offsets = false;             // the offset search (visual_features.rs:14 clear_offsets): no gyro or sync offsets, on the host
+                                            // or the device
+};
+// One frame of undistort_points at timestamp `ts`.  The lens is get_lens_data_at_timestamp of this frame (frame_transform.rs:360) for ONE
+// timestamp: the per-frame lens in a private copy of `cp_user`.  From it: kernel params and K_new, readout timing, smoothed(ts) *
+// org(ts)^-1, shifts and distorting mesh (frame_transform.rs:366-388, 412-434), video rotation (:354), refraction (cpu_undistort.rs:661)
+// and the lens-correction blend (:686-694).
+static PointFrame point_frame(const gf_cuda_gyro* g, const gf_compute_params& cp_user, int distortion_model, size_t frame, double ts,
+                              const PointOpts& o) {
+    gf_compute_params cp = cp_user;
+    if (cp_user.lens_per_frame && frame < cp_user.n_lens_per_frame) {
+        const gf_lens_data& L = cp_user.lens_per_frame[frame];
+        memcpy(cp.camera_matrix, L.camera_matrix, sizeof(cp.camera_matrix)); memcpy(cp.distortion_coeffs, L.distortion_coeffs, sizeof(cp.distortion_coeffs));
+        cp.radial_distortion_limit = L.radial_distortion_limit;
+    }
+    if (o.clear_offsets) { cp.gyro_offset_ms = 0.0; cp.sync_offset_ts_us = nullptr; cp.sync_offset_ms = nullptr; cp.n_sync_offsets = 0; }
+    PointFrame f{};
+    const double fov = points_fov(&cp, frame, o.use_fovs, ts);
     const double* K = cp.camera_matrix;
-    get_new_k(&cp, K, fov, A.new_k);
-    A.horizontal = cp.readout_horizontal; A.suppress_rotation = cp.suppress_rotation;
-    A.org = g->org_track();
-    A.duration_ms = cp.duration_ms;
-    A.offsets = g->sync_offsets(cp.gyro_offset_ms);
-    gf_kernel_params& kp = A.kp;                                                            // cpu_undistort.rs:671-683
+    get_new_k(&cp, K, fov, f.new_k);
+    f.horizontal = cp.readout_horizontal; f.suppress_rotation = cp.suppress_rotation;
+    f.org = g->org_track();
+    f.duration_ms = cp.duration_ms;
+    f.offsets = o.clear_offsets ? SyncOffsets{} : g->sync_offsets(cp.gyro_offset_ms);
+    gf_kernel_params& kp = f.kp;                                                            // cpu_undistort.rs:671-683
     kp.width = cp.width; kp.height = cp.height; kp.output_width = cp.output_width; kp.output_height = cp.output_height;
     kp.f[0] = (float)K[0]; kp.f[1] = (float)K[4]; kp.c[0] = (float)K[2]; kp.c[1] = (float)K[5];
     for (int i = 0; i < 12; ++i) kp.k[i] = (float)cp.distortion_coeffs[i];
     for (int i = 0; i < 16 && i < cp.n_digital_lens_params; ++i) kp.digital_lens_params[i] = (float)cp.digital_lens_params[i];
-    A.lens_noop = lens_noop(distortion_model, kp.k) ? 1 : 0;
-    A.hstretch = cp.input_horizontal_stretch > 0.001 ? (float)cp.input_horizontal_stretch : 0.0f;
-    A.vstretch = cp.input_vertical_stretch   > 0.001 ? (float)cp.input_vertical_stretch   : 0.0f;
-    A.out_cx = (float)cp.output_width / 2.0f; A.out_cy = (float)cp.output_height / 2.0f; A.fov = (float)fov;
-}
-// One frame's record at timestamp `ts`: readout timing, smoothed(ts) * org(ts)^-1, shifts and distorting mesh (frame_transform.rs:366-388,
-// 412-434), video rotation (:354), refraction (cpu_undistort.rs:661) and the lens-correction blend (:686-694) of strength
-// `lens_correction_amount`.  `zoom_keys` (find_fov, fov_iterative.rs:44-46): the zoom centre and the lens-correction strength follow their
-// tracks, `lens_correction_amount` being the value without one.
-static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& cp, const ZoomArgs& A, double ts, size_t frame,
-                                double lens_correction_amount, bool zoom_keys) {
-    ZoomFrame f{};
+    f.lens_noop = lens_noop(distortion_model, kp.k) ? 1 : 0;
+    f.hstretch = cp.input_horizontal_stretch > 0.001 ? (float)cp.input_horizontal_stretch : 0.0f;
+    f.vstretch = cp.input_vertical_stretch   > 0.001 ? (float)cp.input_vertical_stretch   : 0.0f;
+    f.out_cx = (float)cp.output_width / 2.0f; f.out_cy = (float)cp.output_height / 2.0f; f.fov = (float)fov;
+
     const FrameTiming t = frame_timing(&cp, frame, ts, false);
     f.q0 = t.q0; f.start_ts = t.start_ts; f.row_readout_time = t.row_readout_time;
     f.rs_on = fabs(t.frame_readout_time) > 0.0 ? 1 : 0;
@@ -386,34 +403,34 @@ static ZoomFrame frame_uniforms(const gf_cuda_gyro* g, const gf_compute_params& 
     const double a = keyframed(&cp, GF_KF_VIDEO_ROTATION, ts, cp.video_rotation) * (M_PI / 180.0);
     f.rot_c = cos(a); f.rot_s = sin(a);
     f.lrc = (float)keyframed(&cp, GF_KF_LIGHT_REFRACTION_COEFF, ts, cp.light_refraction_coefficient);
-    double lca = lens_correction_amount;
-    if (zoom_keys) {
-        f.zc_x = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * A.in_w;
-        f.zc_y = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * A.in_h;
-        lca = keyframed(&cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, lens_correction_amount);
+    double lca = o.lens_correction_amount;
+    if (o.zoom_keys) {
+        f.zc_x = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_X, ts, cp.adaptive_zoom_center_offset[0]) * (float)cp.width;
+        f.zc_y = (float)keyframed(&cp, GF_KF_ZOOMING_CENTER_Y, ts, cp.adaptive_zoom_center_offset[1]) * (float)cp.height;
+        lca = keyframed(&cp, GF_KF_LENS_CORRECTION_STRENGTH, ts, o.lens_correction_amount);
     }
     f.lc = lca < 1.0 ? 1 : 0;
     f.amount = (float)lca; f.factor = fmaxf(1.0f - f.amount, 0.001f);
-    f.out_fx = A.kp.f[0] / A.fov / f.factor; f.out_fy = A.kp.f[1] / A.fov / f.factor;
+    f.out_fx = kp.f[0] / f.fov / f.factor; f.out_fy = kp.f[1] / f.fov / f.factor;
     return f;
 }
-// One frame of undistort_points at `timestamp_ms`: its lens, fov (get_fov with `use_fovs`), call-wide values and uniforms.  The lens is
-// get_lens_data_at_timestamp of this frame (frame_transform.rs:360) for ONE timestamp: the per-frame lens in a private copy of `cp_user`.
-static PointFrame point_frame(const gf_cuda_gyro* g, const gf_compute_params& cp_user, int distortion_model, size_t frame, double timestamp_ms,
-                              bool use_fovs, double lens_correction_amount) {
-    gf_compute_params cp = cp_user;
-    if (cp_user.lens_per_frame && frame < cp_user.n_lens_per_frame) {
-        const gf_lens_data& L = cp_user.lens_per_frame[frame];
-        memcpy(cp.camera_matrix, L.camera_matrix, sizeof(cp.camera_matrix)); memcpy(cp.distortion_coeffs, L.distortion_coeffs, sizeof(cp.distortion_coeffs));
-        cp.radial_distortion_limit = L.radial_distortion_limit;
-    }
-    PointFrame p;
-    setup_points_args(g, cp, distortion_model, points_fov(&cp, frame, use_fovs, timestamp_ms), p.A);
-    p.F = frame_uniforms(g, cp, p.A, timestamp_ms, frame, lens_correction_amount, false);
-    return p;
-}
 
-bool gf::point_path_supported(int lens, int digital) { return pick_kernels(lens, digital).points != nullptr; }
+bool gf::point_path_supported(int lens, int digital) { return pick_kernels(lens, digital) != nullptr; }
+
+// The synchronous calls: `in` to a device buffer of the call, launch(d_in, d_out, stream), `out` back from one, then wait for the stream.
+template <class In, class Out, class Launch>
+static int round_trip(gf_cuda_gyro* g, void* cu_stream, const In* in, size_t n_in, Out* out, size_t n_out, Launch launch) {
+    const cudaStream_t st = g->stream_of(cu_stream);
+    GrowBuf<In> d_in; GrowBuf<Out> d_out;
+    CK(nullptr, d_in.reserve(n_in, st));
+    CK(nullptr, d_out.reserve(n_out, st));
+    CK(nullptr, cudaMemcpyAsync(d_in.ptr, in, n_in * sizeof(In), cudaMemcpyHostToDevice, st));
+    launch(d_in.ptr, d_out.ptr, st);
+    CK(nullptr, cudaGetLastError());
+    CK(nullptr, cudaMemcpyAsync(out, d_out.ptr, n_out * sizeof(Out), cudaMemcpyDeviceToHost, st));
+    CK(nullptr, cudaStreamSynchronize(st));
+    return GF_OK;
+}
 
 // ---- visual-features sync on the host: argument checks, point records in chunks of candidates, the two-stage search ----
 
@@ -431,7 +448,7 @@ constexpr double kMaxSyncCandidates = 1e7;             // per search stage
 struct SyncJob {
     gf_cuda_gyro* g; const gf_compute_params* cp; int model; double fps; int clear;
     const gf_sync_pair* pairs; size_t n_pairs;
-    ZoomKernels k; cudaStream_t st;
+    const ZoomKernels* k; cudaStream_t st;
     size_t total = 0; uint32_t max_n = 0;
     GrowBuf<float2> d_p1, d_p2; GrowBuf<SyncPairDev> d_pairs; GrowBuf<PointFrame> d_recs; GrowBuf<uint32_t> d_scratch;
     GrowBuf<unsigned long long> d_sums;
@@ -442,7 +459,7 @@ static int sync_check(const char* who, const gf_cuda_gyro* g, const gf_compute_p
                       const gf_sync_pair* pairs, size_t n_pairs) {
     const std::string w(who);
     if (!g || !cp || (n_pairs && !pairs)) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": null argument");
-    if (!pick_kernels(model, digital).sync_cost) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, w + ": no point-path kernel for this (lens, digital lens) pair");
+    if (!pick_kernels(model, digital)) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, w + ": no point-path kernel for this (lens, digital lens) pair");
     if (cp->width < 1 || cp->height < 1 || cp->width > 32768 || cp->height > 32768)
         return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": frame size outside 1..32768");
     if (!(fps > 0.0) || !std::isfinite(fps)) return fail(nullptr, GF_ERR_BAD_PARAMS, w + ": scaled_fps must be finite and > 0");
@@ -484,7 +501,7 @@ static int sync_setup(SyncJob& J) {
 static void sync_records(const SyncJob& J, const double* offs, const double* rs, size_t c0, size_t nc, PointFrame* out) {
     auto work = [&](size_t a, size_t b) {
         gf_compute_params cp = *J.cp;
-        if (J.clear) { cp.gyro_offset_ms = 0.0; cp.sync_offset_ts_us = nullptr; cp.sync_offset_ms = nullptr; cp.n_sync_offsets = 0; }
+        const PointOpts o{ false, 1.0, false, J.clear != 0 };
         for (size_t c = a; c < b; ++c) {
             const double off = offs ? offs[c0 + c] : 0.0;
             if (rs) cp.frame_readout_time = rs[c0 + c];
@@ -492,9 +509,8 @@ static void sync_records(const SyncJob& J, const double* offs, const double* rs,
                 const gf_sync_pair& P = J.pairs[p];
                 const double t1 = (double)P.ts_us / 1000.0 - off, t2 = (double)P.next_ts_us / 1000.0 - off;     // :60-64
                 PointFrame* r = out + 2 * (c * J.n_pairs + p);
-                r[0] = point_frame(J.g, cp, J.model, sync_frame(t1, J.fps), t1, false, 1.0);
-                r[1] = point_frame(J.g, cp, J.model, sync_frame(t2, J.fps), t2, false, 1.0);
-                if (J.clear) r[0].A.offsets = r[1].A.offsets = SyncOffsets{ nullptr, nullptr, 0, 0.0 };
+                r[0] = point_frame(J.g, cp, J.model, sync_frame(t1, J.fps), t1, o);
+                r[1] = point_frame(J.g, cp, J.model, sync_frame(t2, J.fps), t2, o);
             }
         }
     };
@@ -533,7 +549,7 @@ static int sync_run(SyncJob& J, const double* offs, const double* rs, size_t n, 
         // pageable source: the call returns once the records are staged, so the next chunk may overwrite `host`
         CK(nullptr, cudaMemcpyAsync(J.d_recs.ptr, host.data(), 2 * nc * J.n_pairs * sizeof(PointFrame), cudaMemcpyHostToDevice, J.st));
         CK(nullptr, cudaEventRecord(e[0], J.st));
-        J.k.sync_cost<<<(unsigned)(nc * J.n_pairs), SYNC_THREADS, smem, J.st>>>(J.d_recs.ptr, J.d_pairs.ptr, (unsigned)J.n_pairs, J.d_p1.ptr, J.d_p2.ptr,
+        J.k->sync_cost<<<(unsigned)(nc * J.n_pairs), SYNC_THREADS, smem, J.st>>>(J.d_recs.ptr, J.d_pairs.ptr, (unsigned)J.n_pairs, J.d_p1.ptr, J.d_p2.ptr,
                                                                                (float)J.cp->width, (float)J.cp->height, big ? J.d_scratch.ptr : nullptr,
                                                                                J.total, J.d_sums.ptr + c0);
         CK(nullptr, cudaGetLastError());
@@ -612,33 +628,26 @@ GF_API int gf_cuda_find_fovs(gf_cuda_gyro* g, const gf_compute_params* cp_user, 
                              const double* timestamps_ms, size_t n, float fov_algorithm_margin, double* out_fov_minimal, void* cu_stream) {
     if (!g || !cp_user || !timestamps_ms || !out_fov_minimal) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_find_fovs: null argument");
     if (n == 0) return GF_OK;
-    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.find_fov) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_find_fovs: no point-path kernel for this (lens, digital lens) pair");
+    const ZoomKernels* k = pick_kernels(distortion_model, digital_lens);
+    if (!k) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_find_fovs: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
     gf_compute_params cp = *cp_user;
     const int org_ow = cp.output_width, org_oh = cp.output_height;
     cp.fov_scale = 1.0; cp.n_fovs = 0; cp.n_minimal_fovs = 0; cp.output_width = cp.width; cp.output_height = cp.height;
+    cp.lens_per_frame = nullptr; cp.n_lens_per_frame = 0;          // the FOVs are those of the clip's base lens
 
-    ZoomArgs A;
-    const double fov = points_fov(&cp, 0, false, 0.0);            // use_fovs = false: 1 after the adjustments
-    setup_points_args(g, cp, distortion_model, fov, A);
+    FovArgs A;
     const float ratio = (float)cp.width / (float)(org_ow > 1 ? org_ow : 1);                // FovIterative::new :78-89
     A.in_w = (float)cp.width; A.in_h = (float)cp.height;
     A.out_w = (float)org_ow * ratio; const float out_h = (float)org_oh * ratio;
     A.inv_aspect = out_h / A.out_w; A.margin = fov_algorithm_margin;
-    // per-frame uniforms on the host: two O(log n) lookups per frame
-    std::vector<ZoomFrame> hf(n);
-    for (size_t i = 0; i < n; ++i) hf[i] = frame_uniforms(g, cp, A, timestamps_ms[i], i, cp.lens_correction_amount, true);
-    const cudaStream_t st = g->stream_of(cu_stream);
-    GrowBuf<ZoomFrame> d_frames; GrowBuf<double> d_out;
-    CK(nullptr, d_frames.reserve(n, st));
-    CK(nullptr, d_out.reserve(n, st));
-    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(ZoomFrame), cudaMemcpyHostToDevice, st));
-    k.find_fov<<<(unsigned)n, 128, 0, st>>>(A, d_frames.ptr, d_out.ptr);
-    CK(nullptr, cudaGetLastError());
-    CK(nullptr, cudaMemcpyAsync(out_fov_minimal, d_out.ptr, n * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CK(nullptr, cudaStreamSynchronize(st));
-    return GF_OK;
+    // use_fovs = false: every record's fov is 1 after the adjustments
+    const PointOpts o{ false, cp.lens_correction_amount, true };
+    std::vector<PointFrame> hf(n);
+    for (size_t i = 0; i < n; ++i) hf[i] = point_frame(g, cp, distortion_model, i, timestamps_ms[i], o);
+    return round_trip(g, cu_stream, hf.data(), n, out_fov_minimal, n, [&](const PointFrame* d_in, double* d_out, cudaStream_t st) {
+        k->find_fov<<<(unsigned)n, 128, 0, st>>>(d_in, A, d_out);
+    });
 }
 
 // undistort_points_with_rolling_shutter for an arbitrary point list (cpu_undistort.rs:636-641): host in / host out, synchronous.
@@ -647,20 +656,13 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
                                     const float* points_xy, size_t n, float* out_xy, void* cu_stream) {
     if (!g || !cp_user || !points_xy || !out_xy) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_undistort_points: null argument");
     if (n == 0) return GF_OK;
-    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.points) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_undistort_points: no point-path kernel for this (lens, digital lens) pair");
+    const ZoomKernels* k = pick_kernels(distortion_model, digital_lens);
+    if (!k) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_undistort_points: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
-    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, use_fovs != 0, lens_correction_amount);
-    const cudaStream_t st = g->stream_of(cu_stream);
-    GrowBuf<float2> d_in; GrowBuf<float> d_out;
-    CK(nullptr, d_in.reserve(n, st));
-    CK(nullptr, d_out.reserve(n * 2, st));
-    CK(nullptr, cudaMemcpyAsync(d_in.ptr, points_xy, n * sizeof(float2), cudaMemcpyHostToDevice, st));
-    k.points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(p.A, p.F, d_in.ptr, n, 0, 0, d_out.ptr);
-    CK(nullptr, cudaGetLastError());
-    CK(nullptr, cudaMemcpyAsync(out_xy, d_out.ptr, n * 2 * sizeof(float), cudaMemcpyDeviceToHost, st));
-    CK(nullptr, cudaStreamSynchronize(st));
-    return GF_OK;
+    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, PointOpts{ use_fovs != 0, lens_correction_amount });
+    return round_trip(g, cu_stream, (const float2*)points_xy, n, out_xy, n * 2, [&](const float2* d_in, float* d_out, cudaStream_t st) {
+        k->points<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(p, d_in, n, 0, 0, d_out);
+    });
 }
 
 // The "redistort" ST map (stmap.rs:112-116): undistort_points of every pixel centre of the width x height frame, written to
@@ -668,14 +670,14 @@ GF_API int gf_cuda_undistort_points(gf_cuda_gyro* g, const gf_compute_params* cp
 GF_API int gf_cuda_stmap_distort_dev(gf_cuda_gyro* g, const gf_compute_params* cp_user, int distortion_model, int digital_lens,
                                      double timestamp_ms, size_t frame, float* out_rgb_dev, void* cu_stream) {
     if (!g || !cp_user || !out_rgb_dev) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_distort_dev: null argument");
-    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.points) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_distort_dev: no point-path kernel for this (lens, digital lens) pair");
+    const ZoomKernels* k = pick_kernels(distortion_model, digital_lens);
+    if (!k) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_distort_dev: no point-path kernel for this (lens, digital lens) pair");
     const int w = cp_user->width, h = cp_user->height;
     if (w < 1 || h < 1) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_distort_dev: frame size < 1");
     CK(nullptr, cudaSetDevice(g->device));
-    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, true, 1.0);
+    const PointFrame p = point_frame(g, *cp_user, distortion_model, frame, timestamp_ms, PointOpts{ true });
     const size_t n = (size_t)w * (size_t)h;
-    k.points<<<(unsigned)((n + 127) / 128), 128, 0, g->stream_of(cu_stream)>>>(p.A, p.F, nullptr, n, w, h, out_rgb_dev);
+    k->points<<<(unsigned)((n + 127) / 128), 128, 0, g->stream_of(cu_stream)>>>(p, nullptr, n, w, h, out_rgb_dev);
     CK(nullptr, cudaGetLastError());
     return GF_OK;
 }
@@ -691,21 +693,16 @@ GF_API int gf_cuda_stmap_sizes(gf_cuda_gyro* g, const gf_compute_params* cp_user
     if (n > 0x7fffffffu) return fail(nullptr, GF_ERR_BAD_PARAMS, "gf_cuda_stmap_sizes: too many frames");
     const gf_compute_params cp = stmap_params(*cp_user, per_frame);
     if (cp.width < 4 || cp.height < 4) return fail(nullptr, GF_ERR_SIZE_TOO_SMALL, "gf_cuda_stmap_sizes: SizeTooSmall");
-    const ZoomKernels k = pick_kernels(distortion_model, digital_lens);
-    if (!k.stmap_size) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_sizes: no point-path kernel for this (lens, digital lens) pair");
+    const ZoomKernels* k = pick_kernels(distortion_model, digital_lens);
+    if (!k) return fail(nullptr, GF_ERR_UNSUPPORTED_COMBO, "gf_cuda_stmap_sizes: no point-path kernel for this (lens, digital lens) pair");
     CK(nullptr, cudaSetDevice(g->device));
     std::vector<PointFrame> hf(n);
-    for (size_t i = 0; i < n; ++i) hf[i] = point_frame(g, cp, distortion_model, frames[i], timestamps_ms[i], false, 1.0);
-    const cudaStream_t st = g->stream_of(cu_stream);
-    GrowBuf<PointFrame> d_frames; GrowBuf<int2> d_out;
-    CK(nullptr, d_frames.reserve(n, st));
-    CK(nullptr, d_out.reserve(n, st));
-    CK(nullptr, cudaMemcpyAsync(d_frames.ptr, hf.data(), n * sizeof(PointFrame), cudaMemcpyHostToDevice, st));
-    k.stmap_size<<<(unsigned)n, 128, 0, st>>>(d_frames.ptr, (float)cp.width, (float)cp.height, d_out.ptr);
-    CK(nullptr, cudaGetLastError());
+    for (size_t i = 0; i < n; ++i) hf[i] = point_frame(g, cp, distortion_model, frames[i], timestamps_ms[i], PointOpts{});
     std::vector<int2> sizes(n);
-    CK(nullptr, cudaMemcpyAsync(sizes.data(), d_out.ptr, n * sizeof(int2), cudaMemcpyDeviceToHost, st));
-    CK(nullptr, cudaStreamSynchronize(st));
+    const int rc = round_trip(g, cu_stream, hf.data(), n, sizes.data(), n, [&](const PointFrame* d_in, int2* d_out, cudaStream_t st) {
+        k->stmap_size<<<(unsigned)n, 128, 0, st>>>(d_in, (float)cp.width, (float)cp.height, d_out);
+    });
+    if (rc != GF_OK) return rc;
     size_t bad = n;
     for (size_t i = 0; i < n; ++i) {
         out_new_width[i] = sizes[i].x; out_new_height[i] = sizes[i].y;
