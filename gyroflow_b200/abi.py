@@ -302,6 +302,12 @@ EXPORTS = [
     ("gf_cuda_find_sync_offsets", C.c_int, [C.c_void_p, _P(ComputeParams), C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int,
                                             _P(SyncRange), C.c_size_t, _P(SyncResult), _P(C.c_size_t), C.c_void_p]),
     ("gf_cuda_sync_last_timing", C.c_int, [C.c_void_p, _P(C.c_double), _P(C.c_double), _P(C.c_size_t)]),
+    ("gf_optimal_sync_sizes", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, _P(C.c_double), _P(C.c_size_t), _P(C.c_size_t), _P(C.c_size_t)]),
+    ("gf_optimal_sync_select", C.c_int, [C.c_void_p, C.c_size_t, C.c_double, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                         _P(C.c_size_t), C.c_void_p, _P(C.c_double)]),
+    ("gf_cuda_optimal_sync_points", C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
+                                              C.c_void_p, _P(C.c_size_t), C.c_void_p, C.c_void_p, _P(C.c_double), C.c_void_p]),
+    ("gf_cuda_selftest_optimal_sync_resample", C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
 ]
 
 _lib = None

@@ -419,6 +419,91 @@ def selftest_sync_select(groups, device=0):
     return out
 
 
+def _optsync_log(timestamps_ms, gyro, has_gyro):
+    """A gyro log as the optimal-sync calls take it: float64 timestamps, n x 3 float64 gyro, uint8 has_gyro or None."""
+    ts = np.ascontiguousarray(timestamps_ms, dtype=np.float64).reshape(-1)
+    gy = None if gyro is None else np.ascontiguousarray(gyro, dtype=np.float64).reshape(-1, 3)
+    if gy is not None and gy.shape[0] != ts.size:
+        raise ValueError("%d timestamps and %d gyro samples" % (ts.size, gy.shape[0]))
+    hg = None if has_gyro is None else np.ascontiguousarray(has_gyro, dtype=np.uint8).reshape(-1)
+    if hg is not None and hg.size != ts.size:
+        raise ValueError("%d timestamps and %d has_gyro flags" % (ts.size, hg.size))
+    return ts, gy, hg
+
+
+def _trim(trim_ranges_s):
+    t = np.ascontiguousarray(trim_ranges_s, dtype=np.float64).reshape(-1, 2)
+    return t, (t.ctypes.data if t.size else None), t.shape[0]
+
+
+def _ptr(a):
+    return None if a is None else a.ctypes.data
+
+
+def optimal_sync_sizes(timestamps_ms, has_gyro=None):
+    """OptimSync::new's arithmetic (gf_optimal_sync_sizes): (sample_rate, fft_size, n_resampled, n_windows).  Raises GyroflowCoreError
+    for a log the call refuses."""
+    ts, _, hg = _optsync_log(timestamps_ms, None, has_gyro)
+    sr = C.c_double(); n = C.c_size_t(); nr = C.c_size_t(); nw = C.c_size_t()
+    rc = abi.load_library().gf_optimal_sync_sizes(ts.ctypes.data, _ptr(hg), ts.size, C.byref(sr), C.byref(n), C.byref(nr), C.byref(nw))
+    check_call(rc, "gf_optimal_sync_sizes")
+    return sr.value, n.value, nr.value, nw.value
+
+
+def optimal_sync_select(bands, sample_rate, fft_size, target=3, trim_ranges_s=((-np.inf, np.inf),)):
+    """OptimSync::run after the spectra (gf_optimal_sync_select), on the host: bands is n_windows x (lf, mf, hf) float32.
+    Returns (points_ms float64, rank float32, ratio)."""
+    b = np.ascontiguousarray(bands, dtype=np.float32).reshape(-1, 3)
+    t, tp, nt = _trim(trim_ranges_s)
+    pts = np.zeros(max(int(target), 1)); rank = np.zeros(b.shape[0], np.float32)
+    n = C.c_size_t(); ratio = C.c_double()
+    rc = abi.load_library().gf_optimal_sync_select(b.ctypes.data, b.shape[0], sample_rate, fft_size, target, tp, nt, pts.ctypes.data,
+                                                   C.byref(n), rank.ctypes.data, C.byref(ratio))
+    check_call(rc, "gf_optimal_sync_select")
+    return pts[:n.value].copy(), rank, ratio.value
+
+
+def optimal_sync_points(timestamps_ms, gyro, has_gyro=None, target=3, trim_ranges_s=((-np.inf, np.inf),), device=0, stream=0):
+    """OptimSync::new + run on `device` (gf_cuda_optimal_sync_points): the log's resampling and per-window band energies on the GPU, the
+    selection on the host.  trim_ranges_s: (start, end) seconds from the log's time 0.  Returns (points_ms, rank, ratio, bands) with
+    rank the ranks before masking (SyncData::rank) and bands the device's n_windows x (lf, mf, hf) band energies."""
+    ts, gy, hg = _optsync_log(timestamps_ms, gyro, has_gyro)
+    t, tp, nt = _trim(trim_ranges_s)
+    nw = optimal_sync_sizes(ts, hg)[3] if ts.size else 0
+    pts = np.zeros(max(int(target), 1)); rank = np.zeros(nw, np.float32); bands = np.zeros((nw, 3), np.float32)
+    n = C.c_size_t(); ratio = C.c_double()
+    rc = abi.load_library().gf_cuda_optimal_sync_points(device, ts.ctypes.data, gy.ctypes.data, _ptr(hg), ts.size, target, tp, nt,
+                                                        pts.ctypes.data, C.byref(n), rank.ctypes.data, bands.ctypes.data, C.byref(ratio),
+                                                        stream or None)
+    check_call(rc, "gf_cuda_optimal_sync_points")
+    return pts[:n.value].copy(), rank, ratio.value, bands
+
+
+def get_optimal_sync_points(timestamps_ms, gyro, target, duration_ms, trim_ranges_frac=(), initial_offset_ms=0.0, has_gyro=None, device=0):
+    """Stabilization::get_optimal_sync_points (lib.rs:2043-2065) over optimal_sync_points: the trim ranges in seconds from the clip's
+    fractions (the whole clip when there are none) shifted by the initial offset, and the points back to fractions of the clip, those
+    outside [0, 1] dropped.  duration_ms is the clip's scaled duration.  Returns (fractions, rank, ratio)."""
+    if len(trim_ranges_frac) == 0:
+        trim = [((0.0 - initial_offset_ms) / 1000.0, (duration_ms - initial_offset_ms) / 1000.0)]
+    else:
+        trim = [((a * duration_ms - initial_offset_ms) / 1000.0, (b * duration_ms - initial_offset_ms) / 1000.0) for a, b in trim_ranges_frac]
+    if len(timestamps_ms) == 0:                 # OptimSync::new returns None: no points, rank and ratio untouched
+        return [], None, None
+    pts, rank, ratio, _ = optimal_sync_points(timestamps_ms, gyro, has_gyro, target, trim, device)
+    fr = [(float(x) + initial_offset_ms) / duration_ms for x in pts]
+    return [v for v in fr if v >= 0.0 and v <= 1.0], rank, ratio
+
+
+def selftest_optimal_sync_resample(timestamps_ms, gyro, has_gyro=None, device=0):
+    """The device's resampling of OptimSync::new (gf_cuda_selftest_optimal_sync_resample): n_resampled x 3 float32."""
+    ts, gy, hg = _optsync_log(timestamps_ms, gyro, has_gyro)
+    nr = optimal_sync_sizes(ts, hg)[2]
+    out = np.zeros((3, nr), np.float32)
+    rc = abi.load_library().gf_cuda_selftest_optimal_sync_resample(device, ts.ctypes.data, gy.ctypes.data, _ptr(hg), ts.size, out.ctypes.data, nr)
+    check_call(rc, "gf_cuda_selftest_optimal_sync_resample")
+    return out.T.copy()
+
+
 class DeviceGyro:
     """Quaternion tracks resident in HBM + the per-frame matrix kernel (gf_cuda_frame_transform_dev)."""
 

@@ -572,6 +572,48 @@ GF_API int gf_cuda_find_sync_offsets(gf_cuda_gyro* g, const gf_compute_params* c
 GF_API int gf_cuda_sync_last_timing(const gf_cuda_gyro* g, double* host_record_ms, double* device_ms, size_t* chunks);
 
 /* ------------------------------------------------------------------------------------------
+ * Automatic sync points — OptimSync::new + OptimSync::run (src/core/synchronization/optimsync.rs:30-225), the arithmetic of
+ * Stabilization::get_optimal_sync_points (src/core/lib.rs:2043-2065) that chooses where autosync runs.  The caller keeps the rest of
+ * get_optimal_sync_points: the trim ranges in seconds from the clip's fractions and initial offset, and the points back to fractions.
+ * The log: n samples, timestamps_ms[i] (non-decreasing) with gyro_xyz[3 i .. 3 i + 2]; has_gyro (NULL: every sample) marks the samples
+ * that have a gyro reading (`gyro.is_some()`): the others count for nothing in the rate and read as (0, 0, 0).
+ *   new (:30-66): sample_rate = count(has_gyro) / (last - first) * 1000; n_resampled = (duration * sample_rate / 1000) as usize samples
+ *   at i * 1000 / sample_rate ms (from 0, not from the first timestamp), linearly interpolated between the partition_point neighbours in
+ *   f64 (extrapolated past the last sample).
+ *   run (:68-225): fft_size N = round(sample_rate); windows of N resampled samples every 16 (n_windows of them); per window the f32 DFT
+ *   of gyro * blackman(N) per axis, |X[k] + X[N-1-k]| * sqrt(1 / N) / N * 256 for k < N / 2, summed over the axes and over the bins
+ *   [0, map(2)), [map(2), map(30)), [map(30), map(2000)) (map(f) = round(N / sample_rate * f) clamped to [0, N / 2 - 1]) into the band
+ *   energies lf, mf, hf; then the rank, the masks (rank < 50, outside every trim range with both ends inclusive, the first and last 2 s
+ *   of a log over 12 s), the NMS over (sample_rate / 32 * 8) as usize windows and the maximum of each of `target` segments (the last of
+ *   equal ones, NaN comparing equal), kept when >= 0.1, at (index * 16 + N / 2) / sample_rate * 1000 ms.
+ * Refused with GF_ERR_BAD_PARAMS, where the reference panics or cannot allocate: target == 0; NaN or decreasing timestamps; a log that
+ * spans no time; N < 4 (no gyro sample, or a rate below 3.5 Hz); N > 8192 (a rate of 8192.5 Hz or more).  An empty log (n == 0, where
+ * new returns None) gives GF_ERR_NO_DATA.
+ * Exact: the sizes, the resampled gyro, and the selection from the band energies (bit for bit the reference's f32 / f64 operations).
+ * Not exact: the band energies themselves, an f32 Bluestein FFT whose distance from the exact values is bounded in DESIGN.md §7.
+ * ---------------------------------------------------------------------------------------- */
+/* new's arithmetic and the refusals above, on the host: any output pointer may be NULL. */
+GF_API int gf_optimal_sync_sizes(const double* timestamps_ms, const uint8_t* has_gyro, size_t n, double* sample_rate, size_t* fft_size,
+                                 size_t* n_resampled, size_t* n_windows);
+/* run after the spectra (:141-211), on the host: bands is n_windows x (lf, mf, hf), trim_ranges_s n_trim x (start, end) seconds from
+ * the log's time 0.  points_ms holds `target` entries, *n_points receives the number written; rank (NULL: not wanted) receives the
+ * n_windows ranks before masking (rank_clone) and *ratio (NULL: not wanted) 16 / sample_rate, the seconds between windows.  The NMS is a
+ * sliding maximum in O(n_windows), equal to the reference's double loop. */
+GF_API int gf_optimal_sync_select(const float* bands, size_t n_windows, double sample_rate, size_t fft_size, size_t target,
+                                  const double* trim_ranges_s, size_t n_trim, double* points_ms, size_t* n_points, float* rank, double* ratio);
+/* The whole of new + run: resampling and band energies on `device` (on cu_stream, NULL: the default stream), then
+ * gf_optimal_sync_select on the host.  Synchronous.  Every refusal is returned before any device work, and a log shorter than one
+ * window launches nothing (empty rank, no points).  rank holds n_windows floats (gf_optimal_sync_sizes), bands (NULL: not wanted)
+ * n_windows x 3 and receives the device's band energies, from which gf_optimal_sync_select gives this call's rank and points. */
+GF_API int gf_cuda_optimal_sync_points(int device, const double* timestamps_ms, const double* gyro_xyz, const uint8_t* has_gyro, size_t n,
+                                       size_t target, const double* trim_ranges_s, size_t n_trim, double* points_ms, size_t* n_points,
+                                       float* rank, float* bands, double* ratio, void* cu_stream);
+/* The device's resampling alone: out receives 3 x n_out floats, axis by axis (n_out must be gf_optimal_sync_sizes's n_resampled).
+ * Test hook. */
+GF_API int gf_cuda_selftest_optimal_sync_resample(int device, const double* timestamps_ms, const double* gyro_xyz, const uint8_t* has_gyro,
+                                                  size_t n, float* out, size_t n_out);
+
+/* ------------------------------------------------------------------------------------------
  * zooming::calculate_fovs (src/core/zooming/mod.rs:35-70) — what the reference runs before a render (lib.rs:515-523).
  * gf_zoom_params holds the ComputeParams fields it reads besides find_fov's inputs (compute_params.rs:33-53).
  * gf_zoom_fovs takes the per-frame find_fov values and applies, in the reference's order:
